@@ -11,6 +11,8 @@ import os
 import numpy as np
 
 AFC_OK, AFC_EINVAL, AFC_ECUDA, AFC_ENOMEM, AFC_ENCCL, AFC_ESTATE = 0, -1, -2, -3, -4, -5
+DOC_EXECUTION_VC, DOC_WORKFLOW_VC = 0, 1
+VC_INVALID, VC_VALID, VC_HOST, VC_UNRESOLVED, VC_BAD_ENCODING = 0, 1, 2, 3, 4
 MERKLE_STATE_BYTES = 8 + 64 * 32
 SHA256_STATE_BYTES = 108
 
@@ -64,6 +66,9 @@ SYMBOLS = {
     "afc_keyset_info": (C.c_int, [vp, u32p, u64p]),
     "afc_ed25519_verify_keyed_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_uint32, vp]),
     "afc_ed25519_verify_keyed_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_uint32, vp, vp]),
+    "afc_keyset_new_named": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.POINTER(vp)]),
+    "afc_vc_verify_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp]),
+    "afc_vc_verify_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),
     "afc_merkle_free": (None, [vp]),
     "afc_merkle_append": (C.c_int, [vp, vp, vp, C.c_uint32, vp, u64p]),

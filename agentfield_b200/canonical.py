@@ -176,3 +176,50 @@ def webhook_payload_values(p):
     if p.get("error_message") is not None:
         opt += b',"error_message":' + go_json.string(p["error_message"]).encode("utf-8")
     return [u(p["event"]), u(p["execution_id"]), u(p["workflow_id"]), u(p["status"]), u(p["target"]), u(p["type"]), opt, u(p["timestamp"])]
+
+
+def synthetic_stored_vcs_dev(ctx, d_expanded, dids, d_key_index, n, seed=0, str_len=48):
+    """n stored execution-VC documents of realistic size (~1.3 KB: DIDs, hashes, timestamps; nothing to escape) built on the device
+    the way an issuer would: values -> template without proof -> signing bytes -> expanded-key signatures -> base64url ->
+    template with proof.  d_expanded: K x 96 expanded keys; dids: their K DIDs (all of one length); d_key_index: n int32 issuer
+    indices.  Returns (d_docs uint8, d_doc_off int64 [n+1], d_msgs, d_msg_off, d_sigs) — the signing bytes are those the
+    reference verifies, for comparison."""
+    import torch
+    dev = d_key_index.device
+    t0, t1 = vc_document_template(False, ctx), vc_document_template(True, ctx)
+    did_len = len(dids[0])
+    if any(len(d) != did_len for d in dids):
+        raise ValueError("DIDs of one length")
+    g = torch.Generator(device=dev); g.manual_seed(seed)
+    alphabet = torch.tensor(list(b"abcdefghijklmnopqrstuvwxyzABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789-_:"), dtype=torch.uint8, device=dev)
+    d_dids = torch.tensor(np.frombuffer(b"".join(d.encode() for d in dids), dtype=np.uint8).reshape(len(dids), did_len).copy(), device=dev)
+    const = lambda b: torch.tensor(list(b), dtype=torch.uint8, device=dev).expand(n, len(b))
+    rand = lambda w: alphabet[torch.randint(0, alphabet.numel(), (n, w), device=dev, generator=g)]
+    issuer = d_dids[d_key_index.long()]
+    dur = torch.cat([torch.randint(1, 10, (n, 1), device=dev, generator=g), torch.randint(0, 10, (n, 5), device=dev, generator=g)], 1).to(torch.uint8) + 0x30
+    cols = [const(b'["https://www.w3.org/2018/credentials/v1","https://agentfield.example.com/contexts/execution/v1"]'),
+            const(b'["VerifiableCredential","AgentFieldExecutionCredential"]'), rand(str_len), issuer, const(b"2026-09-21T06:00:00Z"),
+            rand(str_len), rand(str_len), rand(str_len), issuer, const(b"agent"), rand(str_len), rand(str_len), rand(str_len), rand(24),
+            rand(43), rand(43), const(b"2026-09-21T06:00:00Z"), dur, const(b"succeeded"), const(b""), rand(43), rand(43),
+            const(b'{"agentfield_version":"1.0.0","vc_version":"1.0"}')]
+
+    def packed(columns):
+        widths = [c.shape[1] for c in columns]
+        rows = torch.cat(columns, 1).contiguous()
+        F, row = len(columns), sum(widths)
+        starts = torch.tensor(np.concatenate([[0], np.cumsum(widths)[:-1]]), dtype=torch.int64, device=dev)
+        off = torch.empty(n * F + 1, dtype=torch.int64, device=dev)
+        off[:-1] = (torch.arange(n, device=dev, dtype=torch.int64)[:, None] * row + starts[None, :]).reshape(-1)
+        off[-1] = n * row
+        return rows.view(-1), off
+    vals, voff = packed(cols)
+    d_msgs, d_moff = t0.fill_dev(vals, voff, n)
+    d_sigs = torch.empty((n, 64), dtype=torch.uint8, device=dev)
+    ctx.sign_expanded_dev(d_expanded, d_key_index, d_msgs, d_moff, n, d_sigs)
+    d_pv = torch.empty((n, 86), dtype=torch.uint8, device=dev)
+    ctx.b64url_encode_dev(d_sigs, 64, n, d_pv)
+    cols += [const(b"Ed25519Signature2020"), const(b"2026-09-21T06:00:01Z"), torch.cat([issuer, const(b"#key-1")], 1), const(b"assertionMethod"), d_pv]
+    del vals, voff
+    vals, voff = packed(cols)
+    d_docs, d_doff = t1.fill_dev(vals, voff, n)
+    return d_docs, d_doff, d_msgs, d_moff, d_sigs

@@ -65,9 +65,23 @@ cudaError_t json_fill_sizes(const uint8_t* segs, const uint32_t* seg_off, const 
                             const uint64_t* field_off, uint32_t n, uint64_t* out_off, uint64_t* scan_scratch, cudaStream_t s, LaunchLog* lg);
 cudaError_t json_fill(const uint8_t* segs, const uint32_t* seg_off, const uint8_t* kinds, uint32_t F, const uint8_t* fields,
                       const uint64_t* field_off, uint32_t n, const uint64_t* out_off, uint8_t* out, cudaStream_t s, LaunchLog* lg);
+// n lengths in out_off[1..n] -> n+1 offsets (out_off[0] = 0); scan_scratch: json_scan_scratch_bytes(n)
+cudaError_t offsets_from_lengths(uint64_t* out_off, uint32_t n, uint64_t* scan_scratch, cudaStream_t s, LaunchLog* lg);
 cudaError_t b64url_encode(const uint8_t* in, uint32_t item, uint32_t n, uint8_t* out, cudaStream_t s, LaunchLog* lg);
 cudaError_t hex_encode(const uint8_t* in, uint64_t total, uint8_t* out, cudaStream_t s, LaunchLog* lg);
 cudaError_t microbench_hash(int which, uint32_t iters, uint32_t blocks, uint32_t threads, uint32_t* sink, cudaStream_t s, LaunchLog* lg);
+
+// ---- k_vcdoc.cu: stored credential documents (afc_vcdoc.cuh).  schema: a VcSchema on the device (vc_schema_bytes()).
+size_t vc_schema_bytes();
+int vc_schema_host(int doc_kind, void* out);           // builds the host copy of a schema; -1 for an unknown kind
+// status: the verdict so far (VC_VALID = a candidate for verification); len_out[i]: signing-message length (0 unless candidate);
+// sigs: n x 64 (16-byte aligned); key_index: n; fields: n x 4 or nullptr
+cudaError_t vc_parse(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint8_t* dids, const uint32_t* did_off,
+                     const uint32_t* slots, uint32_t slot_mask, uint8_t* status, uint64_t* len_out, uint8_t* sigs, uint32_t* key_index,
+                     uint32_t* fields, cudaStream_t s, LaunchLog* lg);
+cudaError_t vc_emit(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint64_t* msg_off, uint8_t* msgs,
+                    cudaStream_t s, LaunchLog* lg);
+cudaError_t vc_fold(uint8_t* status, const uint8_t* ok, uint32_t n, cudaStream_t s, LaunchLog* lg);
 
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)

@@ -69,8 +69,9 @@ struct PinBuf {
 // One stage of a lane's ring of in-flight chunks
 struct Slot {
     cudaStream_t stream = nullptr;
-    DevBuf msgs, off, a, b, k, out, koff;   // a: pks/seeds/keys  b: sigs
-    PinBuf h_in, h_out;                      // bounce buffers when the caller's memory is not pinned
+    DevBuf msgs, off, a, b, k, out, koff;   // a: pks/seeds/keys  b: sigs (stored documents: their field spans)
+    DevBuf vc;                               // stored documents: signing messages, signatures, key indices, verify scratch
+    PinBuf h_in, h_out, h_out2;              // bounce buffers when the caller's memory is not pinned
 };
 struct Lane {
     Slot slot[kSlots];
@@ -120,6 +121,14 @@ struct afc_keyset {
     uint8_t* d_valid = nullptr;    // n_keys
     void* d_tabs = nullptr;        // n_keys x 32 x 128 ge_precomp
     size_t tab_bytes = 0;
+    // afc_keyset_new_named: the keys' DIDs and an open-addressing table DID -> key index (FNV-1a, linear probing), plus the two
+    // document schemas the stored-document call parses with (afc_vcdoc.cuh)
+    bool named = false;
+    uint8_t* d_dids = nullptr;     // DID bytes back to back
+    uint32_t* d_did_off = nullptr; // n_keys + 1
+    uint32_t* d_slots = nullptr;   // slot_mask + 1 entries, 0xffffffff = empty
+    uint32_t slot_mask = 0;
+    uint8_t* d_schemas = nullptr;  // 2 x launch::vc_schema_bytes(): execution VC, workflow VC
 };
 
 struct afc_merkle_tree {
@@ -276,7 +285,7 @@ cudaError_t h2d(Slot& sl, void* dst, const void* src, size_t bytes, bool pinned,
 
 inline bool aligned16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED };
+enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED };
 
 struct BatchArgs {
     Op op;
@@ -286,8 +295,41 @@ struct BatchArgs {
     const uint8_t* keys = nullptr; const uint32_t* koff = nullptr;   // HMAC keys
     const uint8_t* d_expanded = nullptr; const uint32_t* key_index = nullptr;  // sign-expanded / keyed verify
     const afc_keyset* keyset = nullptr;
+    int doc_kind = 0;                                  // stored documents
     uint8_t* out; size_t out_item;
+    uint8_t* out2 = nullptr; size_t out2_item = 0;     // optional second per-item output
 };
+
+// ---- stored credential documents: parse -> scan -> emit -> keyed verify -> fold, in one scratch area
+size_t vc_align(size_t x) { return (x + 255) & ~(size_t)255; }
+size_t vc_scratch_bytes(uint32_t n, uint64_t doc_bytes, uint32_t n_keys) {
+    return vc_align(doc_bytes + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) + vc_align((size_t)n * 4) + vc_align(n) +
+           vc_align(launch::json_scan_scratch_bytes(n)) + vc_align((size_t)n * 32 + launch::ed_keyed_scratch_bytes(n_keys, n));
+}
+// docs + doc_off[i] is document i (absolute offsets); the signing messages of a batch are never longer than its documents
+// (D[0:p] plus the zero-proof text, which is no longer than the proof object it replaces), so doc_bytes bounds their buffer
+cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                              uint64_t doc_bytes, uint8_t* status, uint32_t* fields, uint8_t* scratch, cudaStream_t st, launch::LaunchLog* lg) {
+    if (n == 0) return cudaSuccess;
+    uint8_t* p = scratch;
+    auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
+    uint8_t* msgs = take(doc_bytes + 64);
+    uint64_t* msg_off = (uint64_t*)take(((size_t)n + 1) * 8);
+    uint8_t* sigs = take((size_t)n * 64);
+    uint32_t* kidx = (uint32_t*)take((size_t)n * 4);
+    uint8_t* ok = take(n);
+    uint64_t* scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n));
+    uint32_t* kscr = (uint32_t*)take((size_t)n * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, n));
+    const void* schema = ks->d_schemas + (size_t)kind * launch::vc_schema_bytes();
+    cudaError_t e = launch::vc_parse(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
+                                     kidx, fields, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(msg_off, n, scan, st, lg);
+    if (e == cudaSuccess) e = launch::vc_emit(schema, docs, doc_off, n, msg_off, msgs, st, lg);
+    if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, kidx, sigs, msgs, msg_off, n, ok,
+                                                            kscr, kscr + (size_t)n * 8, st, lg);
+    if (e == cudaSuccess) e = launch::vc_fold(status, ok, n, st, lg);
+    return e;
+}
 
 // Generic chunked pipeline for host-buffer calls: a ring of kSlots chunks in flight so the H2D of later chunks overlaps the kernels of earlier ones.
 // offsets must be non-decreasing: a caller's slip would otherwise turn into an out-of-bounds copy from its own buffer
@@ -316,6 +358,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
     const bool pin_a = A.a ? is_pinned(A.a) : true, pin_b = A.b ? is_pinned(A.b) : true;
     const bool pin_keys = A.keys ? is_pinned(A.keys) : true, pin_koff = A.koff ? is_pinned(A.koff) : true;
     const bool pin_ki = A.key_index ? is_pinned(A.key_index) : true;
+    const bool pin_out2 = A.out2 ? is_pinned(A.out2) : true;
     CallLog lc(ctx, 12 * (int)(A.n / kChunkItems + 8) + 8);
     // AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments
     static const uint32_t max_chunk = [] { const char* e = getenv("AFC_CHUNK_ITEMS"); uint32_t v = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return v ? v : kChunkItems; }();
@@ -328,6 +371,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         Slot& sl = lane.slot[w];
         CK(cudaStreamSynchronize(sl.stream));
         if (!pin_out) memcpy(A.out + (size_t)pend[w].i0 * A.out_item, sl.h_out.p, (size_t)pend[w].cnt * A.out_item);
+        if (A.out2 && !pin_out2) memcpy(A.out2 + (size_t)pend[w].i0 * A.out2_item, sl.h_out2.p, (size_t)pend[w].cnt * A.out2_item);
         if (A.op == OP_SIGN && !pin_a && sl.h_in.p) memset(sl.h_in.p, 0, sl.h_in.cap);         // nor in the pinned bounce buffer
         pend[w].active = false;
         return AFC_OK;
@@ -367,6 +411,8 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
             CK(sl.koff.reserve((size_t)(cnt + 1) * 4));
         }
         if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index) CK(sl.koff.reserve((size_t)cnt * 4));
+        if (A.op == OP_VC_STORED) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys)));
+        if (A.out2) CK(sl.b.reserve((size_t)cnt * A.out2_item + 16));
         size_t bounce = 0;
         if (!pin_msgs) bounce += (mbytes + 255) & ~(size_t)255;
         if (!pin_off) bounce += ((size_t)(cnt + 1) * 8 + 255) & ~(size_t)255;
@@ -376,6 +422,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index && !pin_ki) bounce += ((size_t)cnt * 4 + 255) & ~(size_t)255;
         CK(sl.h_in.reserve(bounce + 256, ctx));
         if (!pin_out) CK(sl.h_out.reserve((size_t)cnt * A.out_item, ctx));
+        if (A.out2 && !pin_out2) CK(sl.h_out2.reserve((size_t)cnt * A.out2_item, ctx));
         size_t used = 0;
         // keep the device copy of the messages congruent mod 16 with the absolute offsets so that the kernels see the
         // same alignment whatever the chunking (d_base + off[i] == sl.msgs.p + pad + off[i] - base)
@@ -406,6 +453,10 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
                                               (uint32_t*)(sl.k.p + (size_t)cnt * 32), sl.stream, lc);
             break;
         }
+        case OP_VC_STORED:
+            e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, A.out2 ? (uint32_t*)sl.b.p : nullptr, sl.vc.p,
+                                  sl.stream, lc);
+            break;
         case OP_SIGN: e = launch::ed_sign_batch(ctx->comb, afc_internal_sign_table(ctx), sl.a.p, d_base, d_off, cnt, sl.out.p, sl.stream, lc); break;
         case OP_SIGN_EXP: {
             const uint32_t* d_ki = nullptr;
@@ -418,6 +469,8 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         if (A.op == OP_SIGN) CK(cudaMemsetAsync(sl.a.p, 0, (size_t)cnt * A.a_item, sl.stream));   // seeds do not stay behind in the staging slot
         CK(cudaMemcpyAsync(pin_out ? A.out + (size_t)i0 * A.out_item : sl.h_out.p, sl.out.p, (size_t)cnt * A.out_item,
                            cudaMemcpyDeviceToHost, sl.stream));
+        if (A.out2) CK(cudaMemcpyAsync(pin_out2 ? A.out2 + (size_t)i0 * A.out2_item : sl.h_out2.p, sl.b.p, (size_t)cnt * A.out2_item,
+                                       cudaMemcpyDeviceToHost, sl.stream));
         pend[which] = {i0, cnt, true};
         which = (which + 1) % kSlots;
         i0 = i1;
@@ -549,7 +602,7 @@ void afc_destroy(afc_ctx* ctx) {
             Slot& sl = ctx->lanes[l].slot[s];
             if (sl.stream) { cudaStreamSynchronize(sl.stream); cudaStreamDestroy(sl.stream); }
             sl.msgs.release(); sl.off.release(); sl.a.release(); sl.b.release(); sl.k.release(); sl.out.release(); sl.koff.release();
-            sl.h_in.release(); sl.h_out.release();
+            sl.vc.release(); sl.h_in.release(); sl.h_out.release(); sl.h_out2.release();
         }
     kc_free(ctx);
     if (ctx->kc_event) cudaEventDestroy(ctx->kc_event);
@@ -915,6 +968,8 @@ void afc_keyset_free(afc_keyset* ks) {
     if (ks->d_pks) cudaFree(ks->d_pks);
     if (ks->d_valid) cudaFree(ks->d_valid);
     if (ks->d_tabs) cudaFree(ks->d_tabs);
+    void* named[] = {ks->d_dids, ks->d_did_off, ks->d_slots, ks->d_schemas};
+    for (void* p : named) if (p) cudaFree(p);
     delete ks;
 }
 int afc_keyset_info(afc_keyset* ks, uint32_t* n_keys, uint64_t* table_bytes) {
@@ -942,6 +997,91 @@ int afc_ed25519_verify_keyed_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint3
     cudaError_t e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_key_index, d_sigs, d_msgs,
                                                   d_msg_off, n, d_ok, d_k, n ? d_k + (size_t)n * 8 : nullptr, st, lc);
     if (n) cudaFreeAsync(d_k, st);
+    CK(e);
+    return AFC_OK;
+}
+
+// ---------------------------------------------------------------------------------- stored credential documents
+static uint32_t did_hash(const uint8_t* p, uint64_t n) {
+    uint32_t h = 2166136261u;
+    for (uint64_t j = 0; j < n; j++) h = (h ^ p[j]) * 16777619u;          // = vc_did_hash_byte (afc_vcdoc.cuh)
+    return h;
+}
+int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, const uint64_t* did_off, uint32_t n_keys, afc_keyset** out) {
+    if (!ctx || !out || !pks || !dids || !did_off || n_keys == 0) return AFC_EINVAL;
+    *out = nullptr;
+    const uint64_t base = did_off[0], total = did_off[n_keys] - base;
+    for (uint32_t k = 0; k < n_keys; k++) if (did_off[k + 1] < did_off[k]) return AFC_EINVAL;
+    if (total >= 0xffffffffull) return AFC_EINVAL;
+    uint32_t cap = 2; while (cap < 2ull * n_keys) cap <<= 1;
+    std::vector<uint32_t> slots(cap, 0xffffffffu), off(n_keys + 1);
+    for (uint32_t k = 0; k <= n_keys; k++) off[k] = (uint32_t)(did_off[k] - base);
+    for (uint32_t k = 0; k < n_keys; k++) {
+        const uint8_t* d = dids + did_off[k];
+        const uint64_t len = did_off[k + 1] - did_off[k];
+        uint32_t s = did_hash(d, len) & (cap - 1);
+        for (; slots[s] != 0xffffffffu; s = (s + 1) & (cap - 1)) {
+            const uint32_t o = slots[s];
+            if (did_off[o + 1] - did_off[o] == len && memcmp(dids + did_off[o], d, len) == 0) return AFC_EINVAL;     // duplicate DID
+        }
+        slots[s] = k;
+    }
+    int rc = afc_keyset_new(ctx, pks, n_keys, out);
+    if (rc != AFC_OK) return rc;
+    afc_keyset* ks = *out;
+    ks->slot_mask = cap - 1;
+    const size_t sb = launch::vc_schema_bytes();
+    std::vector<uint8_t> schemas(2 * sb);
+    if (launch::vc_schema_host(0, schemas.data()) != 0 || launch::vc_schema_host(1, schemas.data() + sb) != 0) {
+        afc_keyset_free(ks); *out = nullptr; return AFC_EINVAL;
+    }
+    cudaError_t e = cudaMalloc((void**)&ks->d_dids, total + 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_did_off, ((size_t)n_keys + 1) * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_slots, (size_t)cap * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_schemas, 2 * sb);
+    if (e == cudaSuccess && total) e = cudaMemcpy(ks->d_dids, dids + base, total, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(ks->d_did_off, off.data(), ((size_t)n_keys + 1) * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(ks->d_slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(ks->d_schemas, schemas.data(), 2 * sb, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        set_err(ctx, e, "afc_keyset_new_named");
+        afc_keyset_free(ks); *out = nullptr;
+        return e == cudaErrorMemoryAllocation ? AFC_ENOMEM : AFC_ECUDA;
+    }
+    ks->named = true;
+    return AFC_OK;
+}
+static int vc_stored_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, uint8_t* status) {
+    if (!ctx || !ks || ks->ctx != ctx || !doc_off || (n && (!docs || !status))) return AFC_EINVAL;
+    if (doc_kind != AFC_DOC_EXECUTION_VC && doc_kind != AFC_DOC_WORKFLOW_VC) return AFC_EINVAL;
+    if (!ks->named) return AFC_ESTATE;
+    return AFC_OK;
+}
+int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                               uint8_t* status, uint32_t* fields) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
+    if (rc != AFC_OK) return rc;
+    BatchArgs A{}; A.op = OP_VC_STORED; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
+    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)fields; A.out2_item = fields ? 16 : 0;
+    return run_host_batch(ctx, A);
+}
+int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
+                                   uint8_t* d_status, uint32_t* d_fields, void* stream) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status);
+    if (rc != AFC_OK || n == 0) return rc;
+    if (d_fields && !aligned16(d_fields)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    CallLog lc(ctx);
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t ends[2];                       // the batch's byte size bounds the message buffer: read it once (one synchronisation)
+    CK(cudaMemcpyAsync(&ends[0], d_doc_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[1], d_doc_off + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ends[1] < ends[0]) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys), st));
+    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, d_fields, scratch, st, lc);
+    cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;
 }

@@ -466,10 +466,14 @@ cudaError_t merkle_verify_consistency(const uint64_t* first_sizes, const uint8_t
 size_t json_scan_scratch_bytes(uint32_t n) { return (((size_t)n + SCAN_TILE - 1) / SCAN_TILE + 1) * 8; }
 cudaError_t json_fill_sizes(const uint8_t* segs, const uint32_t* seg_off, const uint8_t* kinds, uint32_t F, const uint8_t* fields,
                             const uint64_t* field_off, uint32_t n, uint64_t* out_off, uint64_t* scan_scratch, cudaStream_t s, LaunchLog* lg) {
+    if (n == 0) { k_set_u64<<<1, 1, 0, s>>>(out_off, 0); return cudaGetLastError(); }
+    AFC_LAUNCH(lg, "k_json_sizes", s, k_json_sizes<<<blocks_for(n, HASH_THREADS), HASH_THREADS, 0, s>>>(segs, seg_off, kinds, F, fields, field_off, n, out_off + 1));
+    return offsets_from_lengths(out_off, n, scan_scratch, s, lg);
+}
+cudaError_t offsets_from_lengths(uint64_t* out_off, uint32_t n, uint64_t* scan_scratch, cudaStream_t s, LaunchLog* lg) {
     k_set_u64<<<1, 1, 0, s>>>(out_off, 0);          // (a kernel, not cudaMemsetAsync: see k_fill_u32 in k_ed25519.cu)
     if (n == 0) return cudaGetLastError();
     const uint32_t tiles = blocks_for(n, SCAN_TILE);
-    AFC_LAUNCH(lg, "k_json_sizes", s, k_json_sizes<<<blocks_for(n, HASH_THREADS), HASH_THREADS, 0, s>>>(segs, seg_off, kinds, F, fields, field_off, n, out_off + 1));
     AFC_LAUNCH(lg, "k_scan_tiles", s, k_scan_tiles<<<tiles, SCAN_THREADS, 0, s>>>(out_off + 1, n, scan_scratch));
     AFC_LAUNCH(lg, "k_scan_tile_sums", s, k_scan_tile_sums<<<1, 1024, 0, s>>>(scan_scratch, tiles));
     AFC_LAUNCH(lg, "k_scan_add", s, k_scan_add<<<tiles, SCAN_THREADS, 0, s>>>(out_off + 1, n, scan_scratch));

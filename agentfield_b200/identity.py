@@ -68,9 +68,10 @@ class ExpandedKeys:
 
 
 class KeySet:
-    """afc_keyset: issuer public keys with device-resident verification tables (384 KB per key)."""
+    """afc_keyset: issuer public keys with device-resident verification tables (384 KB per key).  With `dids` (one per key) the
+    set also resolves issuers by DID on the device, which the stored-document verification (verify_stored) needs."""
 
-    def __init__(self, pks, ctx=None):
+    def __init__(self, pks, ctx=None, dids=None):
         self.ctx = ctx or default_context()
         self._lib = _abi.load()
         for p in pks:
@@ -79,7 +80,16 @@ class KeySet:
         self.pks = [bytes(p) for p in pks]
         arr = np.frombuffer(b"".join(self.pks), dtype=np.uint8).reshape(-1, 32).copy()
         h = C.c_void_p()
-        _abi.check(self._lib.afc_keyset_new(self.ctx.handle, _abi.ptr(arr), arr.shape[0], C.byref(h)), self.ctx.handle)
+        if dids is None:
+            self.dids = None
+            _abi.check(self._lib.afc_keyset_new(self.ctx.handle, _abi.ptr(arr), arr.shape[0], C.byref(h)), self.ctx.handle)
+        else:
+            if len(dids) != len(self.pks):
+                raise ValueError("one DID per key")
+            self.dids = [d.encode() if isinstance(d, str) else bytes(d) for d in dids]
+            buf, off = pack(self.dids)
+            _abi.check(self._lib.afc_keyset_new_named(self.ctx.handle, _abi.ptr(arr), _abi.ptr(buf), _abi.ptr(off), arr.shape[0], C.byref(h)),
+                       self.ctx.handle)
         self.handle = h
         self._index = {p: i for i, p in enumerate(self.pks)}
 
@@ -130,3 +140,24 @@ class KeySet:
         buf, off = pack(msgs)
         ok = self.verify_packed(ki, sg, buf, off)
         return [bool(o) and not b for o, b in zip(ok, bad_len)]
+
+    def verify_stored_packed(self, doc_kind, buf, off, fields=True):
+        """afc_vc_verify_stored_batch: n stored documents (packed bytes + n+1 offsets) -> (status uint8 [n], fields uint32 [n, 4] or
+        None).  doc_kind: _abi.DOC_EXECUTION_VC or _abi.DOC_WORKFLOW_VC; statuses are _abi.VC_*."""
+        n = len(off) - 1
+        st = np.empty(n, dtype=np.uint8)
+        fl = np.empty((n, 4), dtype=np.uint32) if fields else None
+        _abi.check(self._lib.afc_vc_verify_stored_batch(self.ctx.handle, self.handle, doc_kind, _abi.ptr(buf), _abi.ptr(off), n, _abi.ptr(st),
+                                                        _abi.ptr(fl)), self.ctx.handle)
+        return st, fl
+
+    def verify_stored_dev(self, doc_kind, d_docs, d_off, n, d_status, d_fields=None, stream=None):
+        _abi.check(self._lib.afc_vc_verify_stored_batch_dev(self.ctx.handle, self.handle, doc_kind, _abi.ptr(d_docs), _abi.ptr(d_off), n,
+                                                            _abi.ptr(d_status), _abi.ptr(d_fields), self.ctx._stream(stream)), self.ctx.handle)
+
+    def verify_stored(self, doc_kind, docs):
+        """Host convenience: a list of stored documents (bytes) -> (statuses, fields)."""
+        if not docs:
+            return np.zeros(0, dtype=np.uint8), np.zeros((0, 4), dtype=np.uint32)
+        buf, off = pack(docs)
+        return self.verify_stored_packed(doc_kind, buf, off)

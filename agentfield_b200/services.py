@@ -16,10 +16,11 @@ every hash / signature on the GPU through the C ABI.  The canonical JSON bytes c
 canonical_on_device=True, from the device template (canonical.py): values -> documents -> signatures without a host round trip.
 """
 import base64
+import json
 
 import numpy as np
 
-from . import go_json
+from . import _abi, go_json
 from .crypto import Hasher, MAC, default_context, pack
 from .identity import ExpandedKeys, KeySet
 
@@ -275,6 +276,75 @@ class VCService:
                                  [d["proof"]["proofValue"] for d in docs])
         return [bool(r) for r in res]
 
+    # -- stored documents verified on the device (afc_vc_verify_stored_batch)
+    def verify_stored_vc_batch(self, stored_docs):
+        """VerifyVC (vc_service.go:242-289) for many stored execution-VC documents (bytes as stored): one VCVerificationResponse-shaped
+        dict per document (valid, error, message, issuer_did, issued_at; "" where Go omits the field).  Documents in the exact form
+        json.Marshal writes are parsed, re-assembled and verified on the GPU; only the others are parsed and re-marshalled here."""
+        return self._verify_stored(_abi.DOC_EXECUTION_VC, stored_docs)
+
+    def verify_stored_workflow_vc_batch(self, stored_docs):
+        """The same for stored workflow-VC documents (verifyWorkflowVCSignature, vc_service.go:1589-1625)."""
+        return self._verify_stored(_abi.DOC_WORKFLOW_VC, stored_docs)
+
+    def _named_keyset(self):
+        dids = sorted(self.keys._index)
+        if getattr(self, "_stored_keyset", None) is None or self._stored_keyset_dids != dids:
+            if getattr(self, "_stored_keyset", None) is not None:
+                self._stored_keyset.close()
+            self._stored_keyset = KeySet([self.keys.public_key(d) for d in dids], self.ctx, dids=dids) if dids else None
+            self._stored_keyset_dids = dids
+        return self._stored_keyset
+
+    def _verify_stored(self, kind, stored_docs):
+        docs = [bytes(d) for d in stored_docs]
+        n = len(docs)
+        ks = self._named_keyset()
+        if ks is not None and n:
+            status, fields = ks.verify_stored(kind, docs)
+        else:
+            status, fields = np.full(n, _abi.VC_HOST, dtype=np.uint8), np.zeros((n, 4), dtype=np.uint32)
+        out = [None] * n
+        host = []
+        for i, (raw, st) in enumerate(zip(docs, status)):
+            if st == _abi.VC_VALID:
+                iss = raw[fields[i, 0]:fields[i, 0] + fields[i, 1]].decode("utf-8")
+                date = json.loads(b'"' + raw[fields[i, 2]:fields[i, 2] + fields[i, 3]] + b'"')
+                out[i] = _vc_response(True, message="VC verified successfully", issuer_did=iss, issued_at=date)
+            elif st == _abi.VC_INVALID:
+                out[i] = _vc_response(False, message="Invalid signature")
+            elif st == _abi.VC_UNRESOLVED:
+                iss = raw[fields[i, 0]:fields[i, 0] + fields[i, 1]].decode("utf-8")
+                out[i] = _vc_response(False, error="failed to resolve issuer DID: DID not found: %s" % iss)
+            elif st == _abi.VC_BAD_ENCODING:
+                pv = json.loads(raw)["proof"]["proofValue"]
+                out[i] = _vc_response(False, error="failed to verify signature: failed to decode signature: illegal base64 data at input byte %d"
+                                      % _b64url_error_at(pv))
+            else:
+                host.append(i)
+        # the documents the device declined: today's path (Unmarshal -> Marshal with a zero proof -> keyed verify), batched
+        parsed = []
+        for i in host:
+            try:
+                parsed.append((i, go_unmarshal_vc(docs[i], kind)))
+            except ValueError as ex:
+                out[i] = _vc_response(False, error="failed to parse VC document: %s" % ex)
+        if parsed:
+            marshal = go_json.vc_document if kind == _abi.DOC_EXECUTION_VC else go_json.workflow_vc_document
+            verdicts = self._keyed_verify([d["issuer"] for _, d in parsed], [marshal(d) for _, d in parsed],
+                                          [d["proof"]["proofValue"] for _, d in parsed])
+            for (i, d), v in zip(parsed, verdicts):
+                if v is None and d["issuer"] not in self.keys._index:
+                    out[i] = _vc_response(False, error="failed to resolve issuer DID: DID not found: %s" % d["issuer"])
+                elif v is None:
+                    out[i] = _vc_response(False, error="failed to verify signature: failed to decode signature: illegal base64 data at input byte %d"
+                                          % _b64url_error_at(d["proof"]["proofValue"]))
+                elif v:
+                    out[i] = _vc_response(True, message="VC verified successfully", issuer_did=d["issuer"], issued_at=d["issuanceDate"])
+                else:
+                    out[i] = _vc_response(False, message="Invalid signature")
+        return out
+
     def verify_workflow_vc_comprehensive(self, chain):
         """VerifyWorkflowVCComprehensive (vc_service.go:1386-1586) over one workflow's VC chain: chain = {"component_vcs": [ExecutionVC
         records: vc_id, execution_id, workflow_id, session_id, issuer_did, target_did, caller_did, vc_document (bytes), signature,
@@ -393,6 +463,106 @@ class VCService:
         return {"valid": not critical, "overall_score": score, "critical_issues": critical, "warnings": warnings, "integrity_checks": integrity,
                 "security_analysis": security, "compliance_checks": compliance,
                 "verification_timestamp": chain.get("verification_timestamp", "")}
+
+
+def _vc_response(valid, error="", message="", issuer_did="", issued_at=""):
+    """types.VCVerificationResponse (pkg/types/did_types.go:273-279); "" stands for an omitted field."""
+    return {"valid": valid, "error": error, "message": message, "issuer_did": issuer_did, "issued_at": issued_at}
+
+
+def _b64url_error_at(s: str) -> int:
+    """The input byte base64.RawURLEncoding.DecodeString reports in its CorruptInputError: the first character outside the URL
+    alphabet, else (length = 1 mod 4) the last one."""
+    import re
+    m = re.search(r"[^A-Za-z0-9_-]", s)
+    return m.start() if m else len(s) - 1
+
+
+class _Obj(list):
+    """A JSON object as its (key, value) pairs in document order (json.loads object_pairs_hook)."""
+
+
+_STR, _STRLIST, _INT, _PTRSTR, _MAP = "string", "[]string", "int", "*string", "map[string]interface {}"
+_CALLER = {"did": _STR, "type": _STR, "agentNodeDid": _STR}
+_AUDIT = {"inputDataHash": _STR, "outputDataHash": _STR, "metadata": _MAP}
+_PROOF = {"type": _STR, "created": _STR, "verificationMethod": _STR, "proofPurpose": _STR, "proofValue": _STR}
+_VC_DOC = {"@context": _STRLIST, "type": _STRLIST, "id": _STR, "issuer": _STR, "issuanceDate": _STR,
+           "credentialSubject": {"executionId": _STR, "workflowId": _STR, "sessionId": _STR, "caller": _CALLER,
+                                 "target": {"did": _STR, "agentNodeDid": _STR, "functionName": _STR},
+                                 "execution": {"inputHash": _STR, "outputHash": _STR, "timestamp": _STR, "durationMs": _INT, "status": _STR,
+                                               "errorMessage": _STR},
+                                 "audit": _AUDIT},
+           "proof": _PROOF}
+_WF_DOC = {"@context": _STRLIST, "type": _STRLIST, "id": _STR, "issuer": _STR, "issuanceDate": _STR,
+           "credentialSubject": {"workflowId": _STR, "sessionId": _STR, "componentVcIds": _STRLIST, "totalSteps": _INT, "completedSteps": _INT,
+                                 "status": _STR, "startTime": _STR, "endTime": _PTRSTR, "snapshotTime": _STR, "orchestrator": _CALLER,
+                                 "audit": _AUDIT},
+           "proof": _PROOF}
+
+
+def _zero(t):
+    if isinstance(t, dict):
+        return {k: _zero(v) for k, v in t.items()}
+    return {_STR: "", _INT: 0}.get(t)
+
+
+def _interface(v):
+    """json.Unmarshal into interface{}: objects -> maps (the last duplicate wins), numbers -> float64."""
+    if isinstance(v, _Obj):
+        return {k: _interface(x) for k, x in v}
+    if isinstance(v, list):
+        return [_interface(x) for x in v]
+    return go_json.unmarshal_numbers(v)
+
+
+def _go_into(v, t, cur):
+    """Decodes JSON value v into a Go value of type t whose current value is cur (json.Unmarshal: null leaves non-pointer values
+    alone, struct members match exactly or else case-insensitively, unknown members are ignored)."""
+    if isinstance(t, dict):
+        if v is None:
+            return cur
+        if not isinstance(v, _Obj):
+            raise ValueError("json: cannot unmarshal into Go struct")
+        for k, x in v:
+            name = k if k in t else next((f for f in t if f.lower() == k.lower()), None)
+            if name is not None:
+                cur[name] = _go_into(x, t[name], cur[name])
+        return cur
+    if t in (_STR, _PTRSTR):
+        if v is None:
+            return None if t == _PTRSTR else cur
+        if not isinstance(v, str):
+            raise ValueError("json: cannot unmarshal %s into Go value of type string" % type(v).__name__)
+        return v
+    if t == _STRLIST:
+        if v is None:
+            return None
+        if not isinstance(v, list) or isinstance(v, _Obj) or not all(x is None or isinstance(x, str) for x in v):
+            raise ValueError("json: cannot unmarshal into Go value of type []string")
+        return ["" if x is None else x for x in v]
+    if t == _INT:
+        if v is None:
+            return cur
+        if isinstance(v, bool) or not isinstance(v, int) or not -2**63 <= v < 2**63:
+            raise ValueError("json: cannot unmarshal number into Go value of type int")
+        return v
+    if v is None:                                   # map
+        return None
+    if not isinstance(v, _Obj):
+        raise ValueError("json: cannot unmarshal into Go value of type map[string]interface {}")
+    return _interface(v)
+
+
+def go_unmarshal_vc(raw: bytes, kind=0):
+    """json.Unmarshal(raw, &types.VCDocument) (kind 0) or &types.WorkflowVCDocument (kind 1) as the host mirror's dict; raises
+    ValueError where Go returns an error."""
+    import json
+    try:
+        v = json.loads(raw.decode("utf-8", "replace"), object_pairs_hook=_Obj)
+    except ValueError as ex:
+        raise ValueError(str(ex))
+    schema = _VC_DOC if kind == 0 else _WF_DOC
+    return _go_into(v, schema, _zero(schema))
 
 
 def _b64url_decode_strict(s: str) -> bytes:

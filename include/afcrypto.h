@@ -140,6 +140,39 @@ int afc_ed25519_verify_keyed_batch(afc_ctx* ctx, afc_keyset* ks, const uint32_t*
 int afc_ed25519_verify_keyed_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint32_t* d_key_index, const uint8_t* d_sigs,
                                        const uint8_t* d_msgs, const uint64_t* d_msg_off, uint32_t n, uint8_t* d_ok, void* stream);
 
+/* ---- N3: stored credential documents verified on the device ----------------------------------------------------------------
+ * replaces, per document, VCService.VerifyVC (internal/services/vc_service.go:242-289: json.Unmarshal :250, ResolveDID :259,
+ * verifyVCSignature :469-505 with its zero-Proof json.Marshal :472-476 and base64url decode :498), verifyWorkflowVCSignature
+ * (:1589-1625) and EnhancedVCVerifier.verifyVCSignature (internal/cli/vc_verification_enhanced.go:418-454).
+ * The device proves that a stored document is byte for byte what json.Marshal writes for the struct (VCDocument / WorkflowVCDocument,
+ * pkg/types/did_types.go:135-220) — then the signed message is the document up to "proof": plus the zero proof, built on the device
+ * and verified with the key set's tables.  A document it cannot prove canonical is AFC_VC_HOST: the caller parses, re-marshals and
+ * verifies that one itself (the Go adapter through its stdlib path), so a verdict is never wrong, a decline only slower.
+ * status[i], in the reference's order of errors (parse, resolve, decode signature, verify):
+ *   AFC_VC_HOST          not provably canonical: the caller runs Unmarshal -> Marshal -> Verify
+ *   AFC_VC_UNRESOLVED    issuer not in the key set ("failed to resolve issuer DID")
+ *   AFC_VC_BAD_ENCODING  proofValue is not base64.RawURLEncoding ("failed to decode signature")
+ *   AFC_VC_INVALID       ed25519.Verify false, including a decoded signature length other than 64 ("Invalid signature")
+ *   AFC_VC_VALID         verified
+ * afc_keyset_new_named: afc_keyset_new plus the keys' DIDs (did i = dids[did_off[i] .. did_off[i+1]), n_keys + 1 offsets), looked
+ * up by the issuer bytes of each document; a duplicate DID is AFC_EINVAL.  A key set made by afc_keyset_new gives AFC_ESTATE here.
+ * fields (NULL or n x 4): issuer offset and length, issuanceDate offset and length as they stand in document i (relative to its
+ * start, JSON string bodies without the quotes); valid where status != AFC_VC_HOST.  The host-buffer call streams chunks (documents
+ * never straddle one); the _dev call reads doc_off[0] and doc_off[n] once (one synchronisation of `stream`) to size its scratch. */
+#define AFC_DOC_EXECUTION_VC 0
+#define AFC_DOC_WORKFLOW_VC 1
+#define AFC_VC_INVALID 0
+#define AFC_VC_VALID 1
+#define AFC_VC_HOST 2
+#define AFC_VC_UNRESOLVED 3
+#define AFC_VC_BAD_ENCODING 4
+int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks /* n_keys x 32 */, const uint8_t* dids, const uint64_t* did_off /* n_keys+1 */,
+                         uint32_t n_keys, afc_keyset** out);
+int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                               uint8_t* status, uint32_t* fields);
+int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
+                                   uint8_t* d_status, uint32_t* d_fields, void* stream);
+
 /* ---- E1/K1: Ed25519 sign, public keys -----------------------------------------------------------
  * replaces ed25519.NewKeyFromSeed + ed25519.Sign in VCService.signVC / signWorkflowVC
  * (internal/services/vc_service.go:434-466, :686-718) and NewKeyFromSeed in

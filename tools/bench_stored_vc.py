@@ -1,0 +1,98 @@
+#!/usr/bin/env python
+"""Stored execution-VC documents verified from their bytes (afc_vc_verify_stored_batch[_dev]) against the keyed-verify floor.
+Prints one JSON line: documents/s of the device-pointer call with its per-kernel split, of the keyed verify alone over the same
+signing bytes already rendered, and of the host-buffer call; host_fallback and all_expected; the card and its power limit, read
+in the same run.  Needs a CUDA device; writes nothing.
+usage: python tools/bench_stored_vc.py [--reps R]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def stored_vc_block(ctx, dev, timed):
+    """Stored execution-VC documents verified from their bytes (afc_vc_verify_stored_batch): 2^20 documents of ~1.3 KB from 1024
+    issuers, built on the device (template fill + expanded-key signing), 1 % with a corrupted signature.  Against the floor: the
+    keyed verify alone over the same signing bytes, already rendered.  host_fallback counts documents the device left to the host
+    (0 expected: these are exactly what json.Marshal writes)."""
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import canonical as CA
+    from agentfield_b200.identity import KeySet
+    n, K = 1 << 20, 1024
+    rng = np.random.default_rng(0xAF07)
+    cache = afb.ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (6000 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    d_ki = (torch.arange(n, device=dev) % K).to(torch.int32)
+    d_docs, d_doff, d_msgs, d_moff, d_sigs = CA.synthetic_stored_vcs_dev(ctx, d_exp, dids, d_ki, n, seed=0xAF07)
+    bad = torch.arange(n, device=dev) % 100 == 37
+    pv_at = d_doff[1:] - 3 - 40                                      # inside proofValue (the document ends with "}})
+    d_docs[pv_at[bad]] = torch.where(d_docs[pv_at[bad]] == 0x41, 0x42, 0x41).to(torch.uint8)
+    ks = KeySet([cache.public_key(d) for d in dids], ctx, dids=dids)
+    d_st = torch.empty(n, dtype=torch.uint8, device=dev)
+    d_f = torch.empty((n, 4), dtype=torch.int32, device=dev)
+    run = lambda: ks.verify_stored_dev(0, d_docs, d_doff, n, d_st, d_f)
+    ms_dev = timed(run)
+    expect = torch.where(bad, 0, 1).to(torch.uint8)
+    all_expected = bool(torch.equal(d_st, expect))
+    host_fallback = int((d_st == 2).sum())
+    ctx.profile_begin()
+    timed(run, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    d_ok = torch.empty(n, dtype=torch.uint8, device=dev)
+    ms_floor = timed(lambda: ks.verify_dev(d_ki, d_sigs, d_msgs, d_moff, n, d_ok))
+    buf, off = d_docs.cpu().numpy(), d_doff.cpu().numpy().view(np.uint64)
+    st_host = np.empty(n, dtype=np.uint8)
+    fl_host = np.empty((n, 4), dtype=np.uint32)
+    lib, P = afb._abi.load(), afb._abi.ptr
+
+    def host_call():
+        afb._abi.check(lib.afc_vc_verify_stored_batch(ctx.handle, ks.handle, 0, P(buf), P(off), n, P(st_host), P(fl_host)))
+    host_call()
+    t0 = time.perf_counter()
+    for _ in range(3):
+        host_call()
+    ms_host = (time.perf_counter() - t0) / 3 * 1e3
+    all_expected = all_expected and bool((st_host == expect.cpu().numpy()).all())
+    ks.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"docs": n, "issuers": K, "bytes": int(off[-1]), "avg_doc_bytes": int(off[-1]) / n, "gpu": gpu,
+            "dev_call": {"docs_per_s": n / (ms_dev * 1e-3), "ms": ms_dev, "kernels_ms": kms},
+            "keyed_verify_floor": {"docs_per_s": n / (ms_floor * 1e-3), "ms": ms_floor,
+                                   "note": "afc_ed25519_verify_keyed_batch_dev over the same signing bytes, pre-rendered"},
+            "host_call": {"docs_per_s": n / (ms_host * 1e-3), "ms": ms_host, "note": "documents in pageable host memory, statuses and fields back"},
+            "host_fallback": host_fallback, "all_expected": all_expected}
+
+
+def main():
+    import torch
+    import agentfield_b200 as afb
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    args = ap.parse_args()
+    dev = torch.device("cuda", 0)
+    ctx = afb.Context(0)
+
+    def timed(fn, reps=args.reps):
+        fn(); torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / reps
+    print(json.dumps({"stored_vc_verify": stored_vc_block(ctx, dev, timed)}), flush=True)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
