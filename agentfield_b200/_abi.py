@@ -13,6 +13,12 @@ import numpy as np
 AFC_OK, AFC_EINVAL, AFC_ECUDA, AFC_ENOMEM, AFC_ENCCL, AFC_ESTATE = 0, -1, -2, -3, -4, -5
 DOC_EXECUTION_VC, DOC_WORKFLOW_VC = 0, 1
 VC_INVALID, VC_VALID, VC_HOST, VC_UNRESOLVED, VC_BAD_ENCODING = 0, 1, 2, 3, 4
+AUDIT_COLUMNS = ("issuer_did", "execution_id", "workflow_id", "session_id", "caller_did", "target_did", "status", "input_hash", "output_hash",
+                 "signature")
+# AFC_AUDIT_*: bit k < 10 = column k of AUDIT_COLUMNS differs from the document
+AUDIT_INVALID_TIMESTAMP, AUDIT_MISSING_CONTEXT, AUDIT_MISSING_TYPE, AUDIT_MISSING_ID = 1 << 10, 1 << 11, 1 << 12, 1 << 13
+AUDIT_MISSING_ISSUER, AUDIT_MISSING_ISSUANCE_DATE, AUDIT_NOT_W3C, AUDIT_NOT_AGENTFIELD = 1 << 14, 1 << 15, 1 << 16, 1 << 17
+AUDIT_STATUS_UNDECIDED, AUDIT_TIMESTAMP_UNDECIDED = 1 << 18, 1 << 19
 MERKLE_STATE_BYTES = 8 + 64 * 32
 SHA256_STATE_BYTES = 108
 
@@ -69,6 +75,8 @@ SYMBOLS = {
     "afc_keyset_new_named": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.POINTER(vp)]),
     "afc_vc_verify_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_verify_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
+    "afc_vc_audit_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp]),
+    "afc_vc_audit_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),
     "afc_merkle_free": (None, [vp]),
     "afc_merkle_append": (C.c_int, [vp, vp, vp, C.c_uint32, vp, u64p]),

@@ -178,12 +178,13 @@ def webhook_payload_values(p):
     return [u(p["event"]), u(p["execution_id"]), u(p["workflow_id"]), u(p["status"]), u(p["target"]), u(p["type"]), opt, u(p["timestamp"])]
 
 
-def synthetic_stored_vcs_dev(ctx, d_expanded, dids, d_key_index, n, seed=0, str_len=48):
+def synthetic_stored_vcs_dev(ctx, d_expanded, dids, d_key_index, n, seed=0, str_len=48, audit_columns=False):
     """n stored execution-VC documents of realistic size (~1.3 KB: DIDs, hashes, timestamps; nothing to escape) built on the device
     the way an issuer would: values -> template without proof -> signing bytes -> expanded-key signatures -> base64url ->
     template with proof.  d_expanded: K x 96 expanded keys; dids: their K DIDs (all of one length); d_key_index: n int32 issuer
     indices.  Returns (d_docs uint8, d_doc_off int64 [n+1], d_msgs, d_msg_off, d_sigs) — the signing bytes are those the
-    reference verifies, for comparison."""
+    reference verifies, for comparison.  With audit_columns, also (d_cols uint8, d_col_off int64 [n*10+1]): the ExecutionVC
+    record written with each document, its _abi.AUDIT_COLUMNS columns packed as afc_vc_audit_stored_batch takes them."""
     import torch
     dev = d_key_index.device
     t0, t1 = vc_document_template(False, ctx), vc_document_template(True, ctx)
@@ -222,4 +223,9 @@ def synthetic_stored_vcs_dev(ctx, d_expanded, dids, d_key_index, n, seed=0, str_
     del vals, voff
     vals, voff = packed(cols)
     d_docs, d_doff = t1.fill_dev(vals, voff, n)
-    return d_docs, d_doff, d_msgs, d_moff, d_sigs
+    if not audit_columns:
+        return d_docs, d_doff, d_msgs, d_moff, d_sigs
+    del vals, voff
+    # issuer, executionId, workflowId, sessionId, caller.did, target.did, status, inputHash, outputHash, proofValue
+    d_cols, d_col_off = packed([cols[k] for k in (3, 5, 6, 7, 8, 11, 18, 14, 15, 27)])
+    return d_docs, d_doff, d_msgs, d_moff, d_sigs, d_cols, d_col_off

@@ -79,6 +79,14 @@ int vc_schema_host(int doc_kind, void* out);           // builds the host copy o
 cudaError_t vc_parse(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint8_t* dids, const uint32_t* did_off,
                      const uint32_t* slots, uint32_t slot_mask, uint8_t* status, uint64_t* len_out, uint8_t* sigs, uint32_t* key_index,
                      uint32_t* fields, cudaStream_t s, LaunchLog* lg);
+// k_vc_parse plus the audit capture: caps = vc_capture_bytes(n), 16-byte aligned
+cudaError_t vc_parse_capture(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint8_t* dids, const uint32_t* did_off,
+                             const uint32_t* slots, uint32_t slot_mask, uint8_t* status, uint64_t* len_out, uint8_t* sigs, uint32_t* key_index,
+                             uint32_t* caps, cudaStream_t s, LaunchLog* lg);
+size_t vc_capture_bytes(uint32_t n);
+// issue masks of the captured documents against their records (col_off: 10 per record + 1, nullptr for workflow documents)
+cudaError_t vc_crosscheck(int kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint32_t* caps, const uint8_t* status,
+                          const uint8_t* cols, const uint64_t* col_off, uint32_t* issues, cudaStream_t s, LaunchLog* lg);
 cudaError_t vc_emit(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint64_t* msg_off, uint8_t* msgs,
                     cudaStream_t s, LaunchLog* lg);
 cudaError_t vc_fold(uint8_t* status, const uint8_t* ok, uint32_t n, cudaStream_t s, LaunchLog* lg);

@@ -285,7 +285,7 @@ cudaError_t h2d(Slot& sl, void* dst, const void* src, size_t bytes, bool pinned,
 
 inline bool aligned16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED };
+enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED, OP_VC_AUDIT };
 
 struct BatchArgs {
     Op op;
@@ -296,20 +296,25 @@ struct BatchArgs {
     const uint8_t* d_expanded = nullptr; const uint32_t* key_index = nullptr;  // sign-expanded / keyed verify
     const afc_keyset* keyset = nullptr;
     int doc_kind = 0;                                  // stored documents
+    const uint8_t* cols = nullptr; const uint64_t* col_off = nullptr;   // audit: the records' columns (AFC_AUDIT_COLUMNS per item)
     uint8_t* out; size_t out_item;
     uint8_t* out2 = nullptr; size_t out2_item = 0;     // optional second per-item output
 };
 
 // ---- stored credential documents: parse -> scan -> emit -> keyed verify -> fold, in one scratch area
 size_t vc_align(size_t x) { return (x + 255) & ~(size_t)255; }
-size_t vc_scratch_bytes(uint32_t n, uint64_t doc_bytes, uint32_t n_keys) {
+size_t vc_scratch_bytes(uint32_t n, uint64_t doc_bytes, uint32_t n_keys, bool audit = false) {
     return vc_align(doc_bytes + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) + vc_align((size_t)n * 4) + vc_align(n) +
-           vc_align(launch::json_scan_scratch_bytes(n)) + vc_align((size_t)n * 32 + launch::ed_keyed_scratch_bytes(n_keys, n));
+           vc_align(launch::json_scan_scratch_bytes(n)) + vc_align((size_t)n * 32 + launch::ed_keyed_scratch_bytes(n_keys, n)) +
+           (audit ? vc_align(launch::vc_capture_bytes(n)) : 0);
 }
 // docs + doc_off[i] is document i (absolute offsets); the signing messages of a batch are never longer than its documents
-// (D[0:p] plus the zero-proof text, which is no longer than the proof object it replaces), so doc_bytes bounds their buffer
+// (D[0:p] plus the zero-proof text, which is no longer than the proof object it replaces), so doc_bytes bounds their buffer.
+// With `issues` (the audit) the parse also captures each document and k_vc_crosscheck compares it with its record's columns; the
+// scratch area then needs vc_scratch_bytes(..., true).
 cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
-                              uint64_t doc_bytes, uint8_t* status, uint32_t* fields, uint8_t* scratch, cudaStream_t st, launch::LaunchLog* lg) {
+                              uint64_t doc_bytes, uint8_t* status, uint32_t* fields, uint8_t* scratch, cudaStream_t st, launch::LaunchLog* lg,
+                              uint32_t* issues = nullptr, const uint8_t* cols = nullptr, const uint64_t* col_off = nullptr) {
     if (n == 0) return cudaSuccess;
     uint8_t* p = scratch;
     auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
@@ -321,8 +326,16 @@ cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, cons
     uint64_t* scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n));
     uint32_t* kscr = (uint32_t*)take((size_t)n * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, n));
     const void* schema = ks->d_schemas + (size_t)kind * launch::vc_schema_bytes();
-    cudaError_t e = launch::vc_parse(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
-                                     kidx, fields, st, lg);
+    cudaError_t e;
+    if (issues) {
+        uint32_t* caps = (uint32_t*)take(launch::vc_capture_bytes(n));
+        e = launch::vc_parse_capture(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
+                                     kidx, caps, st, lg);
+        if (e == cudaSuccess) e = launch::vc_crosscheck(kind, docs, doc_off, n, caps, status, cols, col_off, issues, st, lg);
+    } else {
+        e = launch::vc_parse(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
+                             kidx, fields, st, lg);
+    }
     if (e == cudaSuccess) e = launch::offsets_from_lengths(msg_off, n, scan, st, lg);
     if (e == cudaSuccess) e = launch::vc_emit(schema, docs, doc_off, n, msg_off, msgs, st, lg);
     if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, kidx, sigs, msgs, msg_off, n, ok,
@@ -359,6 +372,8 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
     const bool pin_keys = A.keys ? is_pinned(A.keys) : true, pin_koff = A.koff ? is_pinned(A.koff) : true;
     const bool pin_ki = A.key_index ? is_pinned(A.key_index) : true;
     const bool pin_out2 = A.out2 ? is_pinned(A.out2) : true;
+    const bool pin_cols = A.cols ? is_pinned(A.cols) : true, pin_coff = A.col_off ? is_pinned(A.col_off) : true;
+    const uint32_t C = AFC_AUDIT_COLUMNS;
     CallLog lc(ctx, 12 * (int)(A.n / kChunkItems + 8) + 8);
     // AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments
     static const uint32_t max_chunk = [] { const char* e = getenv("AFC_CHUNK_ITEMS"); uint32_t v = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return v ? v : kChunkItems; }();
@@ -388,6 +403,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         // the walk that sizes the chunk also checks that the offsets never run backwards (no separate pass over n offsets)
         while (i1 < A.n && (i1 - i0) < limit) {
             if (A.off[i1 + 1] < A.off[i1]) return AFC_EINVAL;
+            if (A.col_off) for (uint32_t k = 0; k < C; k++) if (A.col_off[(size_t)i1 * C + k + 1] < A.col_off[(size_t)i1 * C + k]) return AFC_EINVAL;
             if (A.off[i1 + 1] - base > kChunkBytes && i1 != i0) break;
             i1++;
         }
@@ -412,6 +428,13 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         }
         if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index) CK(sl.koff.reserve((size_t)cnt * 4));
         if (A.op == OP_VC_STORED) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys)));
+        if (A.op == OP_VC_AUDIT) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys, true)));
+        uint64_t cbase = 0, cbytes = 0;             // audit: this chunk's columns (slot buffers a: bytes, koff: offsets)
+        if (A.col_off) {
+            cbase = A.col_off[(size_t)i0 * C]; cbytes = A.col_off[(size_t)i1 * C] - cbase;
+            CK(sl.a.reserve(cbytes + 32));
+            CK(sl.koff.reserve(((size_t)cnt * C + 1) * 8));
+        }
         if (A.out2) CK(sl.b.reserve((size_t)cnt * A.out2_item + 16));
         size_t bounce = 0;
         if (!pin_msgs) bounce += (mbytes + 255) & ~(size_t)255;
@@ -420,6 +443,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
         if (A.b && !pin_b) bounce += ((size_t)cnt * A.b_item + 255) & ~(size_t)255;
         if (A.op == OP_HMAC) { if (!pin_keys) bounce += (kbytes + 255) & ~(size_t)255; if (!pin_koff) bounce += ((size_t)(cnt + 1) * 4 + 255) & ~(size_t)255; }
         if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index && !pin_ki) bounce += ((size_t)cnt * 4 + 255) & ~(size_t)255;
+        if (A.col_off) { if (!pin_cols) bounce += (cbytes + 255) & ~(size_t)255; if (!pin_coff) bounce += (((size_t)cnt * C + 1) * 8 + 255) & ~(size_t)255; }
         CK(sl.h_in.reserve(bounce + 256, ctx));
         if (!pin_out) CK(sl.h_out.reserve((size_t)cnt * A.out_item, ctx));
         if (A.out2 && !pin_out2) CK(sl.h_out2.reserve((size_t)cnt * A.out2_item, ctx));
@@ -457,6 +481,17 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
             e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, A.out2 ? (uint32_t*)sl.b.p : nullptr, sl.vc.p,
                                   sl.stream, lc);
             break;
+        case OP_VC_AUDIT: {
+            const uint8_t* d_cols = nullptr; const uint64_t* d_coff = nullptr;
+            if (A.col_off) {
+                CK(h2d(sl, sl.a.p + (cbase & 15), A.cols + cbase, cbytes, pin_cols, &used));
+                CK(h2d(sl, sl.koff.p, A.col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
+                d_cols = sl.a.p + (cbase & 15) - cbase; d_coff = (const uint64_t*)sl.koff.p;
+            }
+            e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, nullptr, sl.vc.p, sl.stream, lc,
+                                  (uint32_t*)sl.b.p, d_cols, d_coff);
+            break;
+        }
         case OP_SIGN: e = launch::ed_sign_batch(ctx->comb, afc_internal_sign_table(ctx), sl.a.p, d_base, d_off, cnt, sl.out.p, sl.stream, lc); break;
         case OP_SIGN_EXP: {
             const uint32_t* d_ki = nullptr;
@@ -1081,6 +1116,45 @@ int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, c
     uint8_t* scratch = nullptr;
     CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys), st));
     cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, d_fields, scratch, st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+// audit: the arguments of afc_vc_verify_stored_batch, plus columns exactly for execution documents
+static int vc_audit_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                          const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
+    if (rc != AFC_OK && rc != AFC_ESTATE) return rc;
+    if (n && !issues) return AFC_EINVAL;
+    if (doc_kind == AFC_DOC_EXECUTION_VC ? (!col_off || (n && !cols)) : (cols || col_off)) return AFC_EINVAL;
+    return rc;
+}
+int afc_vc_audit_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                              const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
+    int rc = vc_audit_check(ctx, ks, doc_kind, docs, doc_off, cols, col_off, n, status, issues);
+    if (rc != AFC_OK) return rc;
+    BatchArgs A{}; A.op = OP_VC_AUDIT; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
+    A.cols = cols; A.col_off = col_off;
+    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)issues; A.out2_item = 4;
+    return run_host_batch(ctx, A);
+}
+int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
+                                  const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_issues, void* stream) {
+    int rc = vc_audit_check(ctx, ks, doc_kind, d_docs, d_doc_off, d_cols, d_col_off, n, d_status, d_issues);
+    if (rc != AFC_OK || n == 0) return rc;
+    CK(cudaSetDevice(ctx->device));
+    CallLog lc(ctx);
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t ends[2];                       // the batch's byte size bounds the message buffer: read it once (one synchronisation)
+    CK(cudaMemcpyAsync(&ends[0], d_doc_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[1], d_doc_off + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ends[1] < ends[0]) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys, true), st));
+    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, nullptr, scratch, st, lc, d_issues,
+                                      d_cols, d_col_off);
     cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;

@@ -161,3 +161,32 @@ class KeySet:
             return np.zeros(0, dtype=np.uint8), np.zeros((0, 4), dtype=np.uint32)
         buf, off = pack(docs)
         return self.verify_stored_packed(doc_kind, buf, off)
+
+    def audit_stored_packed(self, doc_kind, buf, off, cols=None, col_off=None):
+        """afc_vc_audit_stored_batch: n stored documents (packed bytes + n+1 offsets) and, for execution documents, their records'
+        _abi.AUDIT_COLUMNS columns (packed bytes + n*10+1 offsets) -> (status uint8 [n], issues uint32 [n] of _abi.AUDIT_* bits)."""
+        n = len(off) - 1
+        st = np.empty(n, dtype=np.uint8)
+        iss = np.empty(n, dtype=np.uint32)
+        _abi.check(self._lib.afc_vc_audit_stored_batch(self.ctx.handle, self.handle, doc_kind, _abi.ptr(buf), _abi.ptr(off), _abi.ptr(cols),
+                                                       _abi.ptr(col_off), n, _abi.ptr(st), _abi.ptr(iss)), self.ctx.handle)
+        return st, iss
+
+    def audit_stored_dev(self, doc_kind, d_docs, d_off, d_cols, d_col_off, n, d_status, d_issues, stream=None):
+        _abi.check(self._lib.afc_vc_audit_stored_batch_dev(self.ctx.handle, self.handle, doc_kind, _abi.ptr(d_docs), _abi.ptr(d_off), _abi.ptr(d_cols),
+                                                           _abi.ptr(d_col_off), n, _abi.ptr(d_status), _abi.ptr(d_issues), self.ctx._stream(stream)),
+                   self.ctx.handle)
+
+    def audit_stored(self, doc_kind, docs, columns=None):
+        """Host convenience: stored documents (bytes) and, for execution documents, one sequence of _abi.AUDIT_COLUMNS values (str or
+        bytes; str is encoded as UTF-8, lone surrogates kept as their three bytes) per document -> (statuses, issue masks)."""
+        if not docs:
+            return np.zeros(0, dtype=np.uint8), np.zeros(0, dtype=np.uint32)
+        buf, off = pack(docs)
+        if columns is None:
+            return self.audit_stored_packed(doc_kind, buf, off)
+        if len(columns) != len(docs) or any(len(c) != len(_abi.AUDIT_COLUMNS) for c in columns):
+            raise ValueError("one row of %d columns per document" % len(_abi.AUDIT_COLUMNS))
+        flat = [v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v) for row in columns for v in row]
+        cbuf, coff = pack(flat)
+        return self.audit_stored_packed(doc_kind, buf, off, cbuf, coff)

@@ -345,124 +345,289 @@ class VCService:
                     out[i] = _vc_response(False, message="Invalid signature")
         return out
 
+    # -- comprehensive audit (vc_service.go:926-1005, 1008-1359, 1386-1644)
+    def _audit_component(self, ev, doc, verdict, integrity, security, compliance):
+        """The checks of one execution VC against its record (performIntegrityChecks, performSecurityAnalysis with
+        detectTamperEvidence, performComplianceChecks; vc_service.go:1008-1359), added to the three running results.  doc: the parsed
+        document (_parse_execution_doc); verdict: its signature check as _keyed_verify reports it (True, False, or None when the
+        issuer does not resolve or proofValue does not decode).  Nothing is verified here."""
+        cs, ex = doc["credentialSubject"], doc["credentialSubject"]["execution"]
+        ic_issues, tamper = [], []
+        pairs = (("issuer_mismatch", "metadata_consistency", "issuer_did", ev["issuer_did"], doc["issuer"], "Issuer DID"),
+                 ("execution_id_mismatch", "field_consistency", "execution_id", ev["execution_id"], cs["executionId"], "Execution ID"),
+                 ("workflow_id_mismatch", "field_consistency", "workflow_id", ev["workflow_id"], cs["workflowId"], "Workflow ID"),
+                 ("session_id_mismatch", "field_consistency", "session_id", ev["session_id"], cs["sessionId"], "Session ID"),
+                 ("caller_did_mismatch", "field_consistency", "caller_did", ev["caller_did"], cs["caller"]["did"], "Caller DID"),
+                 ("target_did_mismatch", "field_consistency", "target_did", ev["target_did"], cs["target"]["did"], "Target DID"))
+        for kind, flag, field, want, got, label in pairs:
+            if want != got:
+                integrity[flag] = False
+                ic_issues.append(_issue(kind, "critical", ev["vc_id"], "%s mismatch between metadata and VC document" % label, field, want, got))
+        if normalize_execution_status(ev["status"]) != normalize_execution_status(ex["status"]):
+            integrity["field_consistency"] = False
+            ic_issues.append(_issue("status_mismatch", "critical", ev["vc_id"], "Status mismatch between metadata and VC document", "status", ev["status"],
+                                    ex["status"]))
+        for kind, field, want, got, label in (("input_hash_mismatch", "input_hash", ev["input_hash"], ex["inputHash"], "Input hash"),
+                                              ("output_hash_mismatch", "output_hash", ev["output_hash"], ex["outputHash"], "Output hash")):
+            if want != got:
+                integrity["hash_validation"] = False
+                ic_issues.append(_issue(kind, "critical", ev["vc_id"], "%s mismatch between metadata and VC document" % label, field, want, got))
+        if ev["signature"] != doc["proof"]["proofValue"]:
+            integrity["structural_integrity"] = False
+            ic_issues.append(_issue("signature_mismatch", "critical", ev["vc_id"], "Signature mismatch between metadata and VC document", "signature",
+                                    ev["signature"], doc["proof"]["proofValue"]))
+        if not _is_rfc3339(doc["issuanceDate"]):
+            integrity["timestamp_validation"] = False
+            ic_issues.append(_issue("invalid_timestamp", "critical", ev["vc_id"], "Invalid timestamp", "issuance_date"))
+        missing = next((name for name, v in (("@context", doc.get("@context")), ("type", doc.get("type")), ("id", doc.get("id")),
+                                             ("issuer", doc.get("issuer")), ("issuanceDate", doc.get("issuanceDate"))) if not v), None)
+        if missing:
+            integrity["structural_integrity"] = False
+            ic_issues.append(_issue("invalid_structure", "critical", ev["vc_id"], "Invalid VC structure: missing %s" % missing))
+        integrity["issues"] += ic_issues
+        score = 100.0
+        if verdict is None and doc["issuer"] not in self.keys._index:
+            security["did_authenticity"] = False; score -= 50.0
+            security["issues"].append(_issue("did_resolution_failed", "critical", ev["vc_id"], "Failed to resolve issuer DID"))
+        elif not verdict:
+            security["key_validation"] = False; score -= 40.0
+            security["issues"].append(_issue("signature_verification_failed", "critical", ev["vc_id"], "Signature verification failed"))
+        if ev["issuer_did"] != doc["issuer"]:
+            tamper.append("issuer_did_inconsistency")
+        if ev["execution_id"] != cs["executionId"]:
+            tamper.append("execution_id_inconsistency")
+        if ev["signature"] != doc["proof"]["proofValue"]:
+            tamper.append("signature_inconsistency")
+        if tamper:
+            score -= 20.0
+            security["tamper_evidence"] += tamper
+            security["issues"].append(_issue("tamper_evidence", "warning", ev["vc_id"], "Tamper evidence detected: %s" % tamper))
+        security["security_score"] = min(security["security_score"], score)
+        if "https://www.w3.org/2018/credentials/v1" not in (doc.get("@context") or []):
+            compliance["w3c_compliance"] = False
+            compliance["issues"].append(_issue("w3c_compliance_failure", "warning", doc.get("id", ""), "VC does not meet W3C standards"))
+        if not {"VerifiableCredential", "AgentFieldExecutionCredential"} <= set(doc.get("type") or []):
+            compliance["agentfield_standard_compliance"] = False
+            compliance["issues"].append(_issue("agentfield_compliance_failure", "warning", doc.get("id", ""),
+                                               "VC does not meet AgentField standard requirements"))
+
+    def _audit_workflow_vc(self, wf, wf_doc, verdict, security, compliance):
+        """The workflow VC's part of VerifyWorkflowVCComprehensive (vc_service.go:1515-1567, checkWorkflowVCCompliance :1628-1644)."""
+        if verdict is None and wf_doc["issuer"] not in self.keys._index:
+            security["did_authenticity"] = False
+            security["issues"].append(_issue("workflow_did_resolution_failed", "critical", wf["workflow_vc_id"], "Failed to resolve workflow VC issuer DID"))
+        elif not verdict:
+            security["key_validation"] = False
+            security["issues"].append(_issue("workflow_signature_verification_failed", "critical", wf["workflow_vc_id"],
+                                             "Workflow VC signature verification failed"))
+        if not {"VerifiableCredential", "AgentFieldWorkflowCredential"} <= set(wf_doc.get("type") or []):
+            compliance["agentfield_standard_compliance"] = False
+            compliance["issues"].append(_issue("workflow_compliance_failure", "warning", wf["workflow_vc_id"],
+                                               "Workflow VC does not meet AgentField standard requirements"))
+
+    def verify_execution_vc_comprehensive(self, record, verification_timestamp=""):
+        """VerifyExecutionVCComprehensive (vc_service.go:926-1005) of one ExecutionVC record (the dict vc_store.ExecutionVCStore returns,
+        vc_document as str or bytes).  The caller passes the record, so the vc_not_found / system_disabled branches do not arise; a
+        document that does not parse gives the early result (parse_error, score 0).  The signature goes through _keyed_verify."""
+        try:
+            doc = _parse_execution_doc(record["vc_document"])
+        except (ValueError, KeyError, TypeError) as ex:
+            return _parse_error_result(record, ex, verification_timestamp)
+        verdict = self._keyed_verify([doc["issuer"]], [go_json.vc_document(doc)], [doc["proof"]["proofValue"]])[0]
+        integrity, security, compliance = _new_checks()
+        self._audit_component(record, doc, verdict, integrity, security, compliance)
+        return _comprehensive_result([], integrity, security, compliance, verification_timestamp)
+
     def verify_workflow_vc_comprehensive(self, chain):
         """VerifyWorkflowVCComprehensive (vc_service.go:1386-1586) over one workflow's VC chain: chain = {"component_vcs": [ExecutionVC
         records: vc_id, execution_id, workflow_id, session_id, issuer_did, target_did, caller_did, vc_document (bytes), signature,
         input_hash, output_hash, status], "workflow_vc": WorkflowVC record or None}.  Every signature of the chain — the component
         VCs' and the workflow VC's — goes through ONE keyed GPU batch (the reference verifies them one by one, :1442-1546).
         `verification_timestamp` is the caller's (the reference reads the clock)."""
-        import json
-        integrity = {"metadata_consistency": True, "field_consistency": True, "timestamp_validation": True, "hash_validation": True,
-                     "structural_integrity": True, "issues": []}
-        security = {"signature_strength": "Ed25519", "key_validation": True, "did_authenticity": True, "replay_protection": True,
-                    "tamper_evidence": [], "security_score": 100.0, "issues": []}
-        compliance = {"w3c_compliance": True, "agentfield_standard_compliance": True, "audit_trail_integrity": True,
-                      "data_integrity_checks": True, "issues": []}
+        integrity, security, compliance = _new_checks()
         critical = []
-
-        def issue(kind, severity, component, description, field="", expected="", actual=""):
-            return {"type": kind, "severity": severity, "component": component, "field": field, "expected": expected, "actual": actual,
-                    "description": description}
         parsed = []
         for ev in chain["component_vcs"]:
             try:
-                doc = json.loads(ev["vc_document"], parse_int=float)
-                doc["credentialSubject"]["audit"]["metadata"] = go_json.unmarshal_numbers(doc["credentialSubject"]["audit"].get("metadata"))
-                doc["credentialSubject"]["execution"].setdefault("errorMessage", "")
-                parsed.append((ev, doc))
+                parsed.append((ev, _parse_execution_doc(ev["vc_document"])))
             except (ValueError, KeyError, TypeError) as ex:
-                critical.append(issue("parse_error", "critical", ev["vc_id"], "Failed to parse VC document: %s" % ex))
+                critical.append(_issue("parse_error", "critical", ev["vc_id"], "Failed to parse VC document: %s" % ex))
         wf, wf_doc = chain.get("workflow_vc"), None
         if wf is not None and wf.get("vc_document") is not None:
             try:
-                wf_doc = json.loads(wf["vc_document"], parse_int=float)
-                wf_doc["credentialSubject"]["audit"]["metadata"] = go_json.unmarshal_numbers(wf_doc["credentialSubject"]["audit"].get("metadata"))
+                wf_doc = _parse_workflow_doc(wf["vc_document"])
             except (ValueError, KeyError, TypeError) as ex:
-                critical.append(issue("workflow_vc_parse_error", "critical", wf["workflow_vc_id"], "Failed to parse workflow VC document: %s" % ex))
+                critical.append(_issue("workflow_vc_parse_error", "critical", wf["workflow_vc_id"], "Failed to parse workflow VC document: %s" % ex))
         # one GPU batch for every signature of the chain
         dids = [d["issuer"] for _, d in parsed] + ([wf_doc["issuer"]] if wf_doc else [])
         msgs = [go_json.vc_document(d) for _, d in parsed] + ([go_json.workflow_vc_document(wf_doc)] if wf_doc else [])
         pvs = [d["proof"]["proofValue"] for _, d in parsed] + ([wf_doc["proof"]["proofValue"]] if wf_doc else [])
         verdicts = self._keyed_verify(dids, msgs, pvs) if dids else []
-        for (ev, doc), verdict, did in zip(parsed, verdicts, dids):
-            cs, ex = doc["credentialSubject"], doc["credentialSubject"]["execution"]
-            ic_issues, tamper = [], []
-            pairs = (("issuer_mismatch", "metadata_consistency", "issuer_did", ev["issuer_did"], doc["issuer"], "Issuer DID"),
-                     ("execution_id_mismatch", "field_consistency", "execution_id", ev["execution_id"], cs["executionId"], "Execution ID"),
-                     ("workflow_id_mismatch", "field_consistency", "workflow_id", ev["workflow_id"], cs["workflowId"], "Workflow ID"),
-                     ("session_id_mismatch", "field_consistency", "session_id", ev["session_id"], cs["sessionId"], "Session ID"),
-                     ("caller_did_mismatch", "field_consistency", "caller_did", ev["caller_did"], cs["caller"]["did"], "Caller DID"),
-                     ("target_did_mismatch", "field_consistency", "target_did", ev["target_did"], cs["target"]["did"], "Target DID"))
-            for kind, flag, field, want, got, label in pairs:
-                if want != got:
-                    integrity[flag] = False
-                    ic_issues.append(issue(kind, "critical", ev["vc_id"], "%s mismatch between metadata and VC document" % label, field, want, got))
-            if normalize_execution_status(ev["status"]) != normalize_execution_status(ex["status"]):
-                integrity["field_consistency"] = False
-                ic_issues.append(issue("status_mismatch", "critical", ev["vc_id"], "Status mismatch between metadata and VC document", "status", ev["status"], ex["status"]))
-            for kind, field, want, got, label in (("input_hash_mismatch", "input_hash", ev["input_hash"], ex["inputHash"], "Input hash"),
-                                                  ("output_hash_mismatch", "output_hash", ev["output_hash"], ex["outputHash"], "Output hash")):
-                if want != got:
-                    integrity["hash_validation"] = False
-                    ic_issues.append(issue(kind, "critical", ev["vc_id"], "%s mismatch between metadata and VC document" % label, field, want, got))
-            if ev["signature"] != doc["proof"]["proofValue"]:
-                integrity["structural_integrity"] = False
-                ic_issues.append(issue("signature_mismatch", "critical", ev["vc_id"], "Signature mismatch between metadata and VC document", "signature",
-                                       ev["signature"], doc["proof"]["proofValue"]))
-            if not _is_rfc3339(doc["issuanceDate"]):
-                integrity["timestamp_validation"] = False
-                ic_issues.append(issue("invalid_timestamp", "critical", ev["vc_id"], "Invalid timestamp", "issuance_date"))
-            missing = next((name for name, v in (("@context", doc.get("@context")), ("type", doc.get("type")), ("id", doc.get("id")),
-                                                 ("issuer", doc.get("issuer")), ("issuanceDate", doc.get("issuanceDate"))) if not v), None)
-            if missing:
-                integrity["structural_integrity"] = False
-                ic_issues.append(issue("invalid_structure", "critical", ev["vc_id"], "Invalid VC structure: missing %s" % missing))
-            integrity["issues"] += ic_issues
-            score = 100.0
-            if verdict is None and did not in self.keys._index:
-                security["did_authenticity"] = False; score -= 50.0
-                security["issues"].append(issue("did_resolution_failed", "critical", ev["vc_id"], "Failed to resolve issuer DID"))
-            elif not verdict:
-                security["key_validation"] = False; score -= 40.0
-                security["issues"].append(issue("signature_verification_failed", "critical", ev["vc_id"], "Signature verification failed"))
-            if ev["issuer_did"] != doc["issuer"]:
-                tamper.append("issuer_did_inconsistency")
-            if ev["execution_id"] != cs["executionId"]:
-                tamper.append("execution_id_inconsistency")
-            if ev["signature"] != doc["proof"]["proofValue"]:
-                tamper.append("signature_inconsistency")
-            if tamper:
-                score -= 20.0
-                security["tamper_evidence"] += tamper
-                security["issues"].append(issue("tamper_evidence", "warning", ev["vc_id"], "Tamper evidence detected: %s" % tamper))
-            security["security_score"] = min(security["security_score"], score)
-            if "https://www.w3.org/2018/credentials/v1" not in (doc.get("@context") or []):
-                compliance["w3c_compliance"] = False
-                compliance["issues"].append(issue("w3c_compliance_failure", "warning", doc.get("id", ""), "VC does not meet W3C standards"))
-            if not {"VerifiableCredential", "AgentFieldExecutionCredential"} <= set(doc.get("type") or []):
-                compliance["agentfield_standard_compliance"] = False
-                compliance["issues"].append(issue("agentfield_compliance_failure", "warning", doc.get("id", ""),
-                                                  "VC does not meet AgentField standard requirements"))
+        for (ev, doc), verdict in zip(parsed, verdicts):
+            self._audit_component(ev, doc, verdict, integrity, security, compliance)
         if wf_doc is not None:
-            verdict = verdicts[-1]
-            if verdict is None and wf_doc["issuer"] not in self.keys._index:
-                security["did_authenticity"] = False
-                security["issues"].append(issue("workflow_did_resolution_failed", "critical", wf["workflow_vc_id"], "Failed to resolve workflow VC issuer DID"))
-            elif not verdict:
-                security["key_validation"] = False
-                security["issues"].append(issue("workflow_signature_verification_failed", "critical", wf["workflow_vc_id"],
-                                                "Workflow VC signature verification failed"))
-            if not {"VerifiableCredential", "AgentFieldWorkflowCredential"} <= set(wf_doc.get("type") or []):
-                compliance["agentfield_standard_compliance"] = False
-                compliance["issues"].append(issue("workflow_compliance_failure", "warning", wf["workflow_vc_id"],
-                                                  "Workflow VC does not meet AgentField standard requirements"))
-        all_issues = integrity["issues"] + security["issues"] + compliance["issues"]
-        critical += [i for i in all_issues if i["severity"] == "critical"]
-        warnings = [i for i in all_issues if i["severity"] == "warning"]
-        score = max(0.0, ((100.0 - 25.0 * len(critical) - 5.0 * len(warnings)) + security["security_score"]) / 2.0)   # calculateOverallScore
-        return {"valid": not critical, "overall_score": score, "critical_issues": critical, "warnings": warnings, "integrity_checks": integrity,
-                "security_analysis": security, "compliance_checks": compliance,
-                "verification_timestamp": chain.get("verification_timestamp", "")}
+            self._audit_workflow_vc(wf, wf_doc, verdicts[-1], security, compliance)
+        return _comprehensive_result(critical, integrity, security, compliance, chain.get("verification_timestamp", ""))
+
+    # -- the comprehensive audit on the device (afc_vc_audit_stored_batch)
+    def _audit_device(self, kind, docs, columns):
+        """(status, issue mask) per stored document from the device, or all HOST when there is no key set to resolve against."""
+        n = len(docs)
+        ks = self._named_keyset()
+        if ks is None or not n:
+            return np.full(n, _abi.VC_HOST, dtype=np.uint8), np.zeros(n, dtype=np.uint32)
+        return ks.audit_stored(kind, docs, columns)
+
+    def _host_verdicts(self, kind, parsed):
+        """_keyed_verify over (index, parsed document) pairs the device left to the host: the mirror's own re-marshal and verify."""
+        if not parsed:
+            return {}
+        marshal = go_json.vc_document if kind == _abi.DOC_EXECUTION_VC else go_json.workflow_vc_document
+        v = self._keyed_verify([d["issuer"] for _, d in parsed], [marshal(d) for _, d in parsed], [d["proof"]["proofValue"] for _, d in parsed])
+        return {i: x for (i, _), x in zip(parsed, v)}
+
+    def audit_stored_execution_vcs(self, records, verification_timestamp=""):
+        """verify_execution_vc_comprehensive for many ExecutionVC records (e.g. a whole store), one result per record and equal to it.
+        One device call proves each stored document canonical, compares it with the record's columns, applies the timestamp,
+        structure and compliance rules and verifies its signature.  A credential with nothing to report (verified, mask 0) gets the
+        clean result without being parsed here; only documents the device left to the host (HOST), non-zero masks and undecided
+        rules go through the mirror's checks, with the device's signature verdict where it has one."""
+        docs = [_doc_bytes(r["vc_document"]) for r in records]
+        status, issues = self._audit_device(_abi.DOC_EXECUTION_VC, docs, [[r[c] for c in _abi.AUDIT_COLUMNS] for r in records])
+        out = [None] * len(records)
+        host, report = [], []
+        for i, (st, m) in enumerate(zip(status, issues)):
+            if st == _abi.VC_VALID and m == 0:
+                out[i] = _clean_result(verification_timestamp)
+                continue
+            try:
+                doc = _parse_execution_doc(records[i]["vc_document"])
+            except (ValueError, KeyError, TypeError) as ex:
+                out[i] = _parse_error_result(records[i], ex, verification_timestamp)
+                continue
+            (host if st == _abi.VC_HOST else report).append((i, doc))
+        verdicts = self._host_verdicts(_abi.DOC_EXECUTION_VC, host)
+        for i, doc in host + report:
+            verdict = verdicts[i] if i in verdicts else _device_verdict(status[i])
+            integrity, security, compliance = _new_checks()
+            self._audit_component(records[i], doc, verdict, integrity, security, compliance)
+            out[i] = _comprehensive_result([], integrity, security, compliance, verification_timestamp)
+        return out
+
+    def audit_workflow_chains(self, chains):
+        """verify_workflow_vc_comprehensive for many chains (same results, same issue order, same scores): the component documents
+        of all chains go through one device call, the workflow VCs through a second.  Components and workflow VCs with nothing to
+        report contribute nothing; the others go through the mirror's checks as in audit_stored_execution_vcs."""
+        comps = [(c, ev) for c, ch in enumerate(chains) for ev in ch["component_vcs"]]
+        c_status, c_issues = self._audit_device(_abi.DOC_EXECUTION_VC, [_doc_bytes(ev["vc_document"]) for _, ev in comps],
+                                                [[ev[k] for k in _abi.AUDIT_COLUMNS] for _, ev in comps])
+        wfs = [(c, ch["workflow_vc"]) for c, ch in enumerate(chains) if ch.get("workflow_vc") is not None and ch["workflow_vc"].get("vc_document") is not None]
+        w_status, w_issues = self._audit_device(_abi.DOC_WORKFLOW_VC, [_doc_bytes(wf["vc_document"]) for _, wf in wfs], None)
+        per_chain = [{"critical": [], "comps": [], "wf": None} for _ in chains]
+        host_c, host_w = [], []
+        for j, ((c, ev), st, m) in enumerate(zip(comps, c_status, c_issues)):
+            if st == _abi.VC_VALID and m == 0:
+                continue
+            try:
+                doc = _parse_execution_doc(ev["vc_document"])
+            except (ValueError, KeyError, TypeError) as ex:
+                per_chain[c]["critical"].append(_issue("parse_error", "critical", ev["vc_id"], "Failed to parse VC document: %s" % ex))
+                continue
+            per_chain[c]["comps"].append((j, ev, doc))
+            if st == _abi.VC_HOST:
+                host_c.append((j, doc))
+        for j, ((c, wf), st, m) in enumerate(zip(wfs, w_status, w_issues)):
+            if st == _abi.VC_VALID and m == 0:
+                continue
+            try:
+                wf_doc = _parse_workflow_doc(wf["vc_document"])
+            except (ValueError, KeyError, TypeError) as ex:
+                per_chain[c]["critical"].append(_issue("workflow_vc_parse_error", "critical", wf["workflow_vc_id"],
+                                                       "Failed to parse workflow VC document: %s" % ex))
+                continue
+            per_chain[c]["wf"] = (j, wf, wf_doc)
+            if st == _abi.VC_HOST:
+                host_w.append((j, wf_doc))
+        c_verdicts = self._host_verdicts(_abi.DOC_EXECUTION_VC, host_c)
+        w_verdicts = self._host_verdicts(_abi.DOC_WORKFLOW_VC, host_w)
+        out = []
+        for ch, p in zip(chains, per_chain):
+            integrity, security, compliance = _new_checks()
+            for j, ev, doc in p["comps"]:
+                self._audit_component(ev, doc, c_verdicts[j] if j in c_verdicts else _device_verdict(c_status[j]), integrity, security, compliance)
+            if p["wf"] is not None:
+                j, wf, wf_doc = p["wf"]
+                self._audit_workflow_vc(wf, wf_doc, w_verdicts[j] if j in w_verdicts else _device_verdict(w_status[j]), security, compliance)
+            out.append(_comprehensive_result(p["critical"], integrity, security, compliance, ch.get("verification_timestamp", "")))
+        return out
+
+
+def _issue(kind, severity, component, description, field="", expected="", actual=""):
+    """types.VerificationIssue (vc_service.go:880-889)."""
+    return {"type": kind, "severity": severity, "component": component, "field": field, "expected": expected, "actual": actual,
+            "description": description}
+
+
+def _doc_bytes(doc):
+    return doc.encode("utf-8") if isinstance(doc, str) else bytes(doc)
+
+
+def _parse_execution_doc(raw):
+    """What the comprehensive checks read a stored execution VC as (json.Unmarshal into types.VCDocument, numbers as float64)."""
+    doc = json.loads(raw, parse_int=float)
+    doc["credentialSubject"]["audit"]["metadata"] = go_json.unmarshal_numbers(doc["credentialSubject"]["audit"].get("metadata"))
+    doc["credentialSubject"]["execution"].setdefault("errorMessage", "")
+    return doc
+
+
+def _parse_workflow_doc(raw):
+    doc = json.loads(raw, parse_int=float)
+    doc["credentialSubject"]["audit"]["metadata"] = go_json.unmarshal_numbers(doc["credentialSubject"]["audit"].get("metadata"))
+    return doc
+
+
+def _new_checks():
+    """The three running results as performIntegrityChecks / performSecurityAnalysis / performComplianceChecks start them."""
+    integrity = {"metadata_consistency": True, "field_consistency": True, "timestamp_validation": True, "hash_validation": True,
+                 "structural_integrity": True, "issues": []}
+    security = {"signature_strength": "Ed25519", "key_validation": True, "did_authenticity": True, "replay_protection": True,
+                "tamper_evidence": [], "security_score": 100.0, "issues": []}
+    compliance = {"w3c_compliance": True, "agentfield_standard_compliance": True, "audit_trail_integrity": True,
+                  "data_integrity_checks": True, "issues": []}
+    return integrity, security, compliance
+
+
+def _comprehensive_result(critical, integrity, security, compliance, verification_timestamp):
+    """ComprehensiveVCVerificationResult: issues split by severity, calculateOverallScore (vc_service.go:1361-1383)."""
+    all_issues = integrity["issues"] + security["issues"] + compliance["issues"]
+    critical = critical + [i for i in all_issues if i["severity"] == "critical"]
+    warnings = [i for i in all_issues if i["severity"] == "warning"]
+    score = max(0.0, ((100.0 - 25.0 * len(critical) - 5.0 * len(warnings)) + security["security_score"]) / 2.0)
+    return {"valid": not critical, "overall_score": score, "critical_issues": critical, "warnings": warnings, "integrity_checks": integrity,
+            "security_analysis": security, "compliance_checks": compliance, "verification_timestamp": verification_timestamp}
+
+
+def _clean_result(verification_timestamp):
+    """The result of a credential with nothing to report."""
+    return _comprehensive_result([], *_new_checks(), verification_timestamp)
+
+
+def _parse_error_result(record, ex, verification_timestamp):
+    """VerifyExecutionVCComprehensive's early return when json.Unmarshal fails (vc_service.go:966-977): the three checks keep Go's zero values."""
+    return {"valid": False, "overall_score": 0.0,
+            "critical_issues": [_issue("parse_error", "critical", record["vc_id"], "Failed to parse VC document: %s" % ex)], "warnings": [],
+            "integrity_checks": {"metadata_consistency": False, "field_consistency": False, "timestamp_validation": False, "hash_validation": False,
+                                 "structural_integrity": False, "issues": None},
+            "security_analysis": {"signature_strength": "", "key_validation": False, "did_authenticity": False, "replay_protection": False,
+                                  "tamper_evidence": None, "security_score": 0.0, "issues": None},
+            "compliance_checks": {"w3c_compliance": False, "agentfield_standard_compliance": False, "audit_trail_integrity": False,
+                                  "data_integrity_checks": False, "issues": None},
+            "verification_timestamp": verification_timestamp}
+
+
+def _device_verdict(status):
+    """A device status as _keyed_verify's verdict: VALID True, INVALID False, UNRESOLVED / BAD_ENCODING None."""
+    return {_abi.VC_VALID: True, _abi.VC_INVALID: False}.get(int(status))
 
 
 def _vc_response(valid, error="", message="", issuer_did="", issued_at=""):

@@ -105,3 +105,69 @@ func (s *StoredCUDA) VerifyStoredBatch(kind DocKind, docs []json.RawMessage, res
 	}
 	return out, nil
 }
+
+// StoredAuditCUDA audits stored execution VCs on the GPU (afc_vc_audit_stored_batch) against the same named key set.
+// Credentials the device leaves to the host (AFC_VC_HOST) or whose mask holds an undecided bit, and every credential of a
+// batch whose call fails, go through StoredAuditStdlib.
+type StoredAuditCUDA struct{ *StoredCUDA }
+
+func (s StoredAuditCUDA) AuditStoredBatch(vcs []types.ExecutionVC, resolve Resolver) ([]AuditResult, error) {
+	n := len(vcs)
+	if n == 0 {
+		return nil, nil
+	}
+	total, ctotal := 0, 0
+	for i := range vcs {
+		v := &vcs[i]
+		total += len(v.VCDocument)
+		for _, c := range auditColumns(v) {
+			ctotal += len(c)
+		}
+	}
+	buf := C.malloc(C.size_t(total + 1))
+	off := C.malloc(C.size_t(8 * (n + 1)))
+	cols := C.malloc(C.size_t(ctotal + 1))
+	coff := C.malloc(C.size_t(8 * (C.AFC_AUDIT_COLUMNS*n + 1)))
+	status := C.malloc(C.size_t(n))
+	issues := C.malloc(C.size_t(4 * n))
+	for _, p := range []unsafe.Pointer{buf, off, cols, coff, status, issues} {
+		defer C.free(p)
+	}
+	b := unsafe.Slice((*byte)(buf), total+1)
+	o := unsafe.Slice((*uint64)(off), n+1)
+	cb := unsafe.Slice((*byte)(cols), ctotal+1)
+	co := unsafe.Slice((*uint64)(coff), C.AFC_AUDIT_COLUMNS*n+1)
+	pos, cpos, k := 0, 0, 0
+	for i := range vcs {
+		o[i] = uint64(pos)
+		pos += copy(b[pos:], vcs[i].VCDocument)
+		for _, c := range auditColumns(&vcs[i]) {
+			co[k] = uint64(cpos)
+			cpos += copy(cb[cpos:], c)
+			k++
+		}
+	}
+	o[n], co[k] = uint64(pos), uint64(cpos)
+	rc := C.afc_vc_audit_stored_batch(s.ctx, s.ks, C.AFC_DOC_EXECUTION_VC, (*C.uint8_t)(buf), (*C.uint64_t)(off), (*C.uint8_t)(cols),
+		(*C.uint64_t)(coff), C.uint32_t(n), (*C.uint8_t)(status), (*C.uint32_t)(issues))
+	if rc != 0 {
+		observeFallback("audit_stored")
+		return StoredAuditStdlib{}.AuditStoredBatch(vcs, resolve)
+	}
+	st := unsafe.Slice((*byte)(status), n)
+	is := unsafe.Slice((*uint32)(issues), n)
+	out := make([]AuditResult, n)
+	for i := range vcs {
+		if st[i] == C.AFC_VC_HOST || is[i]&(AuditStatusUndecided|AuditTimestampUndecided) != 0 {
+			out[i] = auditStoredOne(&vcs[i], resolve)
+			continue
+		}
+		out[i] = AuditResult{Status: st[i], Issues: is[i]}
+	}
+	return out, nil
+}
+
+// the record's columns in the order of AFC_AUDIT_COLUMNS
+func auditColumns(v *types.ExecutionVC) [10]string {
+	return [10]string{v.IssuerDID, v.ExecutionID, v.WorkflowID, v.SessionID, v.CallerDID, v.TargetDID, v.Status, v.InputHash, v.OutputHash, v.Signature}
+}

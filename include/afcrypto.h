@@ -173,6 +173,52 @@ int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const
 int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                    uint8_t* d_status, uint32_t* d_fields, void* stream);
 
+/* ---- stored credentials audited against their records on the device ---------------------------------------------------------
+ * replaces, per credential, the checks of VCService.VerifyExecutionVCComprehensive (internal/services/vc_service.go:926-1005):
+ * json.Unmarshal, performIntegrityChecks (:1008-1181), performSecurityAnalysis (:1184-1233) and performComplianceChecks
+ * (:1236-1268), and of the per-component loop of VerifyWorkflowVCComprehensive (:1442-1512).  Everything afc_vc_verify_stored_batch
+ * does (status has the same meaning), plus issues[i], a mask of AFC_AUDIT_* bits for the things the credential has to report:
+ *   bits 0-9     the record's column k differs from the document's member (Unmarshal(member) != column; the status column is
+ *                compared after NormalizeExecutionStatus on both sides)
+ *   INVALID_TIMESTAMP   issuanceDate is not RFC 3339           MISSING_*       validateVCStructure: @context / type empty or null,
+ *   NOT_W3C             @context lacks the W3C context                          id / issuer / issuanceDate empty
+ *   NOT_AGENTFIELD      type lacks VerifiableCredential or AgentFieldExecutionCredential (workflow documents:
+ *                       AgentFieldWorkflowCredential, checkWorkflowVCCompliance :1628-1644; the only bit defined for them)
+ *   STATUS_UNDECIDED    the status comparison is left to the caller (non-printable or non-ASCII bytes, or an escape in the document)
+ *   TIMESTAMP_UNDECIDED the timestamp rule is left to the caller (a byte >= 0x80 in issuanceDate)
+ * issues[i] is 0 and meaningless where status[i] is AFC_VC_HOST.  cols / col_off: AFC_AUDIT_COLUMNS byte strings per record, in the
+ * order below, as packed Go strings (column k of record i = cols[col_off[10 i + k] .. col_off[10 i + k + 1]), n * 10 + 1 offsets);
+ * required for execution documents, NULL for workflow documents (else AFC_EINVAL).  The host-buffer call streams chunks through
+ * the same ring as afc_vc_verify_stored_batch and checks that the column offsets never run backwards; the _dev call synchronises
+ * `stream` once to size its scratch. */
+#define AFC_AUDIT_COLUMNS 10   /* issuer_did, execution_id, workflow_id, session_id, caller_did, target_did,
+                                  status, input_hash, output_hash, signature: the ExecutionVC record, pkg/types */
+#define AFC_AUDIT_ISSUER_MISMATCH (1u << 0)
+#define AFC_AUDIT_EXECUTION_ID_MISMATCH (1u << 1)
+#define AFC_AUDIT_WORKFLOW_ID_MISMATCH (1u << 2)
+#define AFC_AUDIT_SESSION_ID_MISMATCH (1u << 3)
+#define AFC_AUDIT_CALLER_DID_MISMATCH (1u << 4)
+#define AFC_AUDIT_TARGET_DID_MISMATCH (1u << 5)
+#define AFC_AUDIT_STATUS_MISMATCH (1u << 6)
+#define AFC_AUDIT_INPUT_HASH_MISMATCH (1u << 7)
+#define AFC_AUDIT_OUTPUT_HASH_MISMATCH (1u << 8)
+#define AFC_AUDIT_SIGNATURE_MISMATCH (1u << 9)
+#define AFC_AUDIT_INVALID_TIMESTAMP (1u << 10)
+#define AFC_AUDIT_MISSING_CONTEXT (1u << 11)
+#define AFC_AUDIT_MISSING_TYPE (1u << 12)
+#define AFC_AUDIT_MISSING_ID (1u << 13)
+#define AFC_AUDIT_MISSING_ISSUER (1u << 14)
+#define AFC_AUDIT_MISSING_ISSUANCE_DATE (1u << 15)
+#define AFC_AUDIT_NOT_W3C (1u << 16)
+#define AFC_AUDIT_NOT_AGENTFIELD (1u << 17)
+#define AFC_AUDIT_STATUS_UNDECIDED (1u << 18)
+#define AFC_AUDIT_TIMESTAMP_UNDECIDED (1u << 19)
+int afc_vc_audit_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                              const uint64_t* col_off /* n*AFC_AUDIT_COLUMNS+1, NULL for workflow docs */, uint32_t n, uint8_t* status,
+                              uint32_t* issues);
+int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
+                                  const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_issues, void* stream);
+
 /* ---- E1/K1: Ed25519 sign, public keys -----------------------------------------------------------
  * replaces ed25519.NewKeyFromSeed + ed25519.Sign in VCService.signVC / signWorkflowVC
  * (internal/services/vc_service.go:434-466, :686-718) and NewKeyFromSeed in

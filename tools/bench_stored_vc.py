@@ -2,7 +2,8 @@
 """Stored execution-VC documents verified from their bytes (afc_vc_verify_stored_batch[_dev]) against the keyed-verify floor.
 Prints one JSON line: documents/s of the device-pointer call with its per-kernel split, of the keyed verify alone over the same
 signing bytes already rendered, and of the host-buffer call; host_fallback and all_expected; the card and its power limit, read
-in the same run.  Needs a CUDA device; writes nothing.
+in the same run.  The audit_stored block does the same for the audit of stored execution VCs against their records
+(afc_vc_audit_stored_batch[_dev]), next to the stored-verify device call on the same documents.  Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R]"""
 import argparse
 import json
@@ -73,6 +74,67 @@ def stored_vc_block(ctx, dev, timed):
             "host_fallback": host_fallback, "all_expected": all_expected}
 
 
+def audit_stored_block(ctx, dev, timed):
+    """Stored execution VCs audited against their records (afc_vc_audit_stored_batch): 2^20 records from 1024 issuers built on the
+    device, 1 % with a corrupted signature, 1 % with one column of the record changed (over all ten columns).  Beside it, the
+    stored-verify device call on the same documents.  all_expected: every status and every mask is exactly the planted damage;
+    host_fallback / undecided count documents and masks the host would have to finish (0 expected)."""
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import canonical as CA
+    from agentfield_b200.identity import KeySet
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_audit_gpu import plant_damage
+    n, K = 1 << 20, 1024
+    rng = np.random.default_rng(0xAF08)
+    cache = afb.ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (6000 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    d_ki = (torch.arange(n, device=dev) % K).to(torch.int32)
+    d_docs, d_doff, _, _, _, d_cols, d_coff = CA.synthetic_stored_vcs_dev(ctx, d_exp, dids, d_ki, n, seed=0xAF08, audit_columns=True)
+    want_st, want_iss = plant_damage(d_docs, d_doff, d_cols, d_coff, n)
+    ks = KeySet([cache.public_key(d) for d in dids], ctx, dids=dids)
+    d_st = torch.empty(n, dtype=torch.uint8, device=dev)
+    d_iss = torch.empty(n, dtype=torch.int32, device=dev)
+    run = lambda: ks.audit_stored_dev(0, d_docs, d_doff, d_cols, d_coff, n, d_st, d_iss)
+    ms_dev = timed(run)
+    all_expected = bool(torch.equal(d_st, want_st)) and bool(torch.equal(d_iss, want_iss))
+    host_fallback = int((d_st == 2).sum())
+    undecided = int(((d_iss & ((1 << 18) | (1 << 19))) != 0).sum())
+    ctx.profile_begin()
+    timed(run, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    d_st2 = torch.empty(n, dtype=torch.uint8, device=dev)
+    verify = lambda: ks.verify_stored_dev(0, d_docs, d_doff, n, d_st2)
+    ms_verify = timed(verify)
+    ctx.profile_begin()
+    timed(verify, reps=3)
+    vkms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    buf, off = d_docs.cpu().numpy(), d_doff.cpu().numpy().view(np.uint64)
+    cbuf, coff = d_cols.cpu().numpy(), d_coff.cpu().numpy().view(np.uint64)
+    st_host = np.empty(n, dtype=np.uint8)
+    iss_host = np.empty(n, dtype=np.uint32)
+    lib, P = afb._abi.load(), afb._abi.ptr
+
+    def host_call():
+        afb._abi.check(lib.afc_vc_audit_stored_batch(ctx.handle, ks.handle, 0, P(buf), P(off), P(cbuf), P(coff), n, P(st_host), P(iss_host)))
+    host_call()
+    t0 = time.perf_counter()
+    for _ in range(3):
+        host_call()
+    ms_host = (time.perf_counter() - t0) / 3 * 1e3
+    all_expected = all_expected and bool((st_host == want_st.cpu().numpy()).all()) and bool((iss_host == want_iss.cpu().numpy().view(np.uint32)).all())
+    ks.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"records": n, "issuers": K, "doc_bytes": int(off[-1]), "column_bytes": int(coff[-1]), "gpu": gpu,
+            "dev_call": {"docs_per_s": n / (ms_dev * 1e-3), "ms": ms_dev, "kernels_ms": kms},
+            "stored_verify_dev_call": {"docs_per_s": n / (ms_verify * 1e-3), "ms": ms_verify, "kernels_ms": vkms,
+                                       "note": "afc_vc_verify_stored_batch_dev on the same documents"},
+            "host_call": {"docs_per_s": n / (ms_host * 1e-3), "ms": ms_host, "note": "documents and columns in pageable host memory, statuses and masks back"},
+            "host_fallback": host_fallback, "undecided": undecided, "all_expected": all_expected}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
@@ -90,7 +152,7 @@ def main():
             fn()
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
-    print(json.dumps({"stored_vc_verify": stored_vc_block(ctx, dev, timed)}), flush=True)
+    print(json.dumps({"stored_vc_verify": stored_vc_block(ctx, dev, timed), "audit_stored": audit_stored_block(ctx, dev, timed)}), flush=True)
     ctx.close()
 
 
