@@ -288,24 +288,84 @@ AFC_HD void store_digest256(uint8_t* out, const uint32_t st[8]) {
 // mad.wide.u32 d, a, ONE, c64 into IMAD.WIDE + IADD3 + IMAD.X, so the ALU pipe keeps its add and the FMA pipe gains two.
 // Rotates as multiplications by 2^(32-n) from the constant bank — two IMAD + two IMAD.HI per 64-bit rotate instead of two SHF —
 // do leave the ALU pipe, but cost more than they free: each further rotate moved made k_ed_hram + verify slower.)
-AFC_OUTLINE void sha512_compress(uint64_t* st, uint64_t* w) {
-    uint64_t a = st[0], b = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
+AFC_HD void sha512_round(uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d, uint64_t& e, uint64_t& f, uint64_t& g, uint64_t& h,
+                         uint64_t kw) {
+    const uint64_t t1 = h + (rotr64(e, 14) ^ rotr64(e, 18) ^ rotr64(e, 41)) + ((e & f) ^ (~e & g)) + kw;
+    const uint64_t t2 = (rotr64(a, 28) ^ rotr64(a, 34) ^ rotr64(a, 39)) + ((a & b) ^ (a & c) ^ (b & c));
+    h = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;
+}
+
+// One compression: returns st + F(st, w[0..15]).  State and block are passed by value in registers: through pointers both live in
+// local memory, and as ONE 192-byte aggregate the calling convention passes them on the stack.  The first 16 rounds, which need no
+// schedule, are peeled; the other 64 stay a rolled loop of 16 so that the ONE out-of-line copy per kernel stays small in the
+// instruction cache.
+struct sha512_st { uint64_t st[8]; };
+struct sha512_blk { uint64_t w[16]; };
+AFC_OUTLINE sha512_st sha512_compress_regs(sha512_st x, sha512_blk blk) {
+    uint64_t a = x.st[0], b = x.st[1], c = x.st[2], d = x.st[3], e = x.st[4], f = x.st[5], g = x.st[6], h = x.st[7];
+    uint64_t w[16];
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+        w[j] = blk.w[j];
+        sha512_round(a, b, c, d, e, f, g, h, AFC_K512[j] + w[j]);
+    }
 #pragma unroll 1
-    for (int r = 0; r < 80; r += 16) {
+    for (int r = 16; r < 80; r += 16) {
 #pragma unroll
         for (int j = 0; j < 16; j++) {
-            if (r > 0) {
-                uint64_t w15 = w[(j + 1) & 15], w2 = w[(j + 14) & 15];
-                uint64_t s0 = rotr64(w15, 1) ^ rotr64(w15, 8) ^ (w15 >> 7);
-                uint64_t s1 = rotr64(w2, 19) ^ rotr64(w2, 61) ^ (w2 >> 6);
-                w[j] = w[j] + s0 + w[(j + 9) & 15] + s1;
-            }
-            uint64_t t1 = h + (rotr64(e, 14) ^ rotr64(e, 18) ^ rotr64(e, 41)) + ((e & f) ^ (~e & g)) + AFC_K512[r + j] + w[j];
-            uint64_t t2 = (rotr64(a, 28) ^ rotr64(a, 34) ^ rotr64(a, 39)) + ((a & b) ^ (a & c) ^ (b & c));
-            h = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;
+            const uint64_t w15 = w[(j + 1) & 15], w2 = w[(j + 14) & 15];
+            const uint64_t s0 = rotr64(w15, 1) ^ rotr64(w15, 8) ^ (w15 >> 7);
+            const uint64_t s1 = rotr64(w2, 19) ^ rotr64(w2, 61) ^ (w2 >> 6);
+            w[j] = w[j] + s0 + w[(j + 9) & 15] + s1;
+            sha512_round(a, b, c, d, e, f, g, h, AFC_K512[r + j] + w[j]);
         }
     }
-    st[0] += a; st[1] += b; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+    sha512_st o;
+    o.st[0] = x.st[0] + a; o.st[1] = x.st[1] + b; o.st[2] = x.st[2] + c; o.st[3] = x.st[3] + d;
+    o.st[4] = x.st[4] + e; o.st[5] = x.st[5] + f; o.st[6] = x.st[6] + g; o.st[7] = x.st[7] + h;
+    return o;
+}
+// 128 message bytes from 16-byte-aligned p as big-endian words
+AFC_HD void sha512_load_block(uint64_t w[16], const uint8_t* p) {
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+        const word4 v = ld_u128(p + 16 * q);
+        w[2 * q] = ((uint64_t)bswap32(v.x) << 32) | bswap32(v.y);
+        w[2 * q + 1] = ((uint64_t)bswap32(v.z) << 32) | bswap32(v.w);
+    }
+}
+
+// The last len < 128 bytes of a message at 16-byte-aligned p, followed by 0x80 and zeros, as big-endian words.  Only 16-byte
+// loads that hold at least one message byte are issued; the bytes they bring from past the end are masked off.  The caller adds
+// the bit length: into w[15] when len < 112, otherwise into a block of its own.
+AFC_HD void sha512_tail_block(uint64_t w[16], const uint8_t* p, uint32_t len) {
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+        word4 v = {0u, 0u, 0u, 0u};
+        if (16u * q < len) v = ld_u128(p + 16 * q);
+        w[2 * q] = ((uint64_t)bswap32(v.x) << 32) | bswap32(v.y);
+        w[2 * q + 1] = ((uint64_t)bswap32(v.z) << 32) | bswap32(v.w);
+    }
+#pragma unroll
+    for (int i = 0; i < 16; i++) {
+        const int rem = (int)len - 8 * i;                      // message bytes in word i, if in 0..7
+        if (rem <= 0) w[i] = rem == 0 ? 0x8000000000000000ull : 0ull;
+        else if (rem < 8) w[i] = (w[i] & (~0ull << (64 - 8 * rem))) | (0x80ull << (56 - 8 * rem));
+    }
+}
+
+// Bytes k..k+3 (k % 4 == 0) of msg followed by 0x80 and zeros, as a big-endian word.  Stateless, so nothing but (msg, len)
+// stays live across a compression; only 4-byte loads that hold at least one message byte are issued.
+AFC_HD uint32_t sha512_padded_word(const uint8_t* msg, uint64_t len, int64_t k) {
+    const int64_t r = (int64_t)len - k;                // message bytes from k on
+    if (r < 0) return 0u;
+    if (r == 0) return 0x80000000u;
+    const uintptr_t a = (uintptr_t)msg + (uint64_t)k;
+    const uint32_t* p = (const uint32_t*)(a & ~(uintptr_t)3);
+    const uint32_t sh = (uint32_t)(a & 3) * 8;
+    const uint32_t lo = ld_u32(p), hi = (sh && (uintptr_t)(p + 1) < a + (uint64_t)r) ? ld_u32(p + 1) : 0u;
+    const uint32_t v = bswap32(funnel_r(lo, hi, sh));
+    return r >= 4 ? v : (v & (0xffffffffu << (32 - 8 * r))) | (0x80000000u >> (8 * r));
 }
 
 // SHA-512( prefix (PW 32-bit words, given as LITTLE-endian-loaded words of the byte string) || msg ).
@@ -314,67 +374,63 @@ AFC_OUTLINE void sha512_compress(uint64_t* st, uint64_t* w) {
 template <int PW>
 AFC_HD void sha512_prefixed(uint32_t digest_le[16], const uint32_t* prefix_le, const uint8_t* msg, uint64_t len) {
     static_assert(PW % 4 == 0 && PW <= 24, "prefix must be whole 16-byte groups and leave room in block 0");
-    uint64_t st[8];
+    sha512_st x;
+    sha512_blk blk;
 #pragma unroll
-    for (int i = 0; i < 8; i++) st[i] = AFC_H512[i];
+    for (int i = 0; i < 8; i++) x.st[i] = AFC_H512[i];
     const uint64_t total = (uint64_t)PW * 4 + len;
     constexpr int M0 = 128 - 4 * PW;                   // message bytes that share block 0 with the prefix
-    bool first_done = false;
     if ((((uintptr_t)msg) & 15) == 0 && len >= (uint64_t)M0) {
-        // lean path: block 0 = prefix || msg[0:M0], then whole 128-byte blocks, all with 128-bit loads
-        uint64_t w[16];
+        // lean path: block 0 = prefix || msg[0:M0], then whole 128-byte blocks, then the padded tail, all with 128-bit loads
 #pragma unroll
-        for (int i = 0; i < PW / 2; i++) w[i] = ((uint64_t)bswap32(prefix_le[2 * i]) << 32) | bswap32(prefix_le[2 * i + 1]);
+        for (int i = 0; i < PW / 2; i++) blk.w[i] = ((uint64_t)bswap32(prefix_le[2 * i]) << 32) | bswap32(prefix_le[2 * i + 1]);
 #pragma unroll
         for (int q = 0; q < M0 / 16; q++) {
-            word4 v = ld_u128(msg + 16 * q);
-            w[PW / 2 + 2 * q] = ((uint64_t)bswap32(v.x) << 32) | bswap32(v.y);
-            w[PW / 2 + 2 * q + 1] = ((uint64_t)bswap32(v.z) << 32) | bswap32(v.w);
+            const word4 v = ld_u128(msg + 16 * q);
+            blk.w[PW / 2 + 2 * q] = ((uint64_t)bswap32(v.x) << 32) | bswap32(v.y);
+            blk.w[PW / 2 + 2 * q + 1] = ((uint64_t)bswap32(v.z) << 32) | bswap32(v.w);
         }
-        sha512_compress(st, w);
+        x = sha512_compress_regs(x, blk);
         msg += M0; len -= M0;
-        first_done = true;
-        uint64_t nfull = len >> 7;
-        for (uint64_t blk = 0; blk < nfull; blk++) {
-#pragma unroll
-            for (int q = 0; q < 8; q++) {
-                word4 v = ld_u128(msg + 16 * q);
-                w[2 * q] = ((uint64_t)bswap32(v.x) << 32) | bswap32(v.y);
-                w[2 * q + 1] = ((uint64_t)bswap32(v.z) << 32) | bswap32(v.w);
-            }
-            sha512_compress(st, w);
+        const uint64_t nfull = len >> 7;
+        for (uint64_t i = 0; i < nfull; i++) {
+            sha512_load_block(blk.w, msg);
+            x = sha512_compress_regs(x, blk);
             msg += 128;
         }
-        len &= 127;
-    }
-    // general path: (the rest of) the message through the byte-granular padded stream
-    PadStream ps; ps.init(msg, len);
-    const uint64_t pending = first_done ? len : total;            // bytes still to absorb, prefix included if not yet done
-    const uint64_t nblk = (pending + 17 + 127) / 128;
-    for (uint64_t blk = 0; blk < nblk; blk++) {
-        uint64_t w[16];
-        if (blk == 0 && !first_done) {
+        const uint32_t tail = (uint32_t)(len & 127);
+        sha512_tail_block(blk.w, msg, tail);
+        if (tail < 112) blk.w[15] = total * 8;
+        x = sha512_compress_regs(x, blk);
+        if (tail >= 112) {
 #pragma unroll
-            for (int i = 0; i < 16; i++) {
-                uint32_t hi, lo;
-                if (2 * i < PW) { hi = bswap32(prefix_le[2 * i]); lo = bswap32(prefix_le[2 * i + 1]); }
-                else { hi = ps.next_be(); lo = ps.next_be(); }
-                w[i] = ((uint64_t)hi << 32) | lo;
-            }
-        } else {
-#pragma unroll 1
-            for (int i = 0; i < 16; i++) {
-                uint32_t hi = ps.next_be(), lo = ps.next_be();
-                w[i] = ((uint64_t)hi << 32) | lo;
-            }
+            for (int i = 0; i < 15; i++) blk.w[i] = 0;
+            blk.w[15] = total * 8;
+            x = sha512_compress_regs(x, blk);
         }
-        if (blk == nblk - 1) { w[14] = 0; w[15] = total * 8; }
-        sha512_compress(st, w);
+    } else {
+        // general path (unaligned or short messages): word by word, padded in registers
+        const uint32_t nblk = (uint32_t)((total + 17 + 127) / 128);
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            if (2 * i < PW) blk.w[i] = ((uint64_t)bswap32(prefix_le[2 * i]) << 32) | bswap32(prefix_le[2 * i + 1]);
+            else blk.w[i] = ((uint64_t)sha512_padded_word(msg, len, 8 * i - 4 * PW) << 32) | sha512_padded_word(msg, len, 8 * i + 4 - 4 * PW);
+        }
+        for (uint32_t bi = 0; bi < nblk; bi++) {
+            if (bi > 0) {
+                const int64_t k0 = 128 * (int64_t)bi - 4 * PW;
+#pragma unroll
+                for (int i = 0; i < 16; i++)
+                    blk.w[i] = ((uint64_t)sha512_padded_word(msg, len, k0 + 8 * i) << 32) | sha512_padded_word(msg, len, k0 + 8 * i + 4);
+            }
+            if (bi == nblk - 1) { blk.w[14] = 0; blk.w[15] = total * 8; }
+            x = sha512_compress_regs(x, blk);
+        }
     }
 #pragma unroll
     for (int i = 0; i < 8; i++) {
-        digest_le[2 * i] = bswap32((uint32_t)(st[i] >> 32));
-        digest_le[2 * i + 1] = bswap32((uint32_t)st[i]);
+        digest_le[2 * i] = bswap32((uint32_t)(x.st[i] >> 32));
+        digest_le[2 * i + 1] = bswap32((uint32_t)x.st[i]);
     }
 }
 

@@ -967,8 +967,9 @@ template <bool CT, class F>
 __device__ __forceinline__ void base_mult(ge_p3& h, const uint32_t* a, const ge_precomp* tab) {
     if (CT) ge_scalarmult_base_ct<F>(h, a, tab); else ge_scalarmult_base<F>(h, a, tab);
 }
+// (4 CTAs per SM, <= 128 registers: left alone, ptxas spends 163 on the in-register SHA-512 and a CTA per SM is lost)
 template <bool CT>
-__global__ void __launch_bounds__(ED_THREADS)
+__global__ void __launch_bounds__(ED_THREADS, 4)
 k_ed_sign(const ge_precomp* __restrict__ comb_in, const uint8_t* __restrict__ keys, const uint32_t* __restrict__ key_index, uint32_t n_keys,
           const uint8_t* __restrict__ msgs, const uint64_t* __restrict__ off, uint32_t n, uint32_t T, int G, uint8_t* __restrict__ sigs) {
     const ge_precomp* comb = stage_ct_table<CT>(comb_in);

@@ -394,15 +394,16 @@ __global__ void k_microbench_hash(int which, uint32_t iters, uint32_t* sink) {
         }
         if (st[0] == 0x12345678u) sink[0] = st[1];
     } else {
-        uint64_t st[8], w[16];
+        sha512_st x;
+        sha512_blk b;
 #pragma unroll
-        for (int i = 0; i < 8; i++) st[i] = seed + i;
+        for (int i = 0; i < 8; i++) x.st[i] = seed + i;
         for (uint32_t it = 0; it < iters; it++) {
 #pragma unroll
-            for (int i = 0; i < 16; i++) w[i] = st[i & 7] ^ (it + i);
-            sha512_compress(st, w);
+            for (int i = 0; i < 16; i++) b.w[i] = x.st[i & 7] ^ (it + i);
+            x = sha512_compress_regs(x, b);
         }
-        if (st[0] == 0x12345678u) sink[0] = (uint32_t)st[1];
+        if (x.st[0] == 0x12345678u) sink[0] = (uint32_t)x.st[1];
     }
 }
 
