@@ -75,6 +75,8 @@ SYMBOLS = {
     "afc_keyset_new_named": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.POINTER(vp)]),
     "afc_vc_verify_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_verify_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
+    "afc_vc_verify_json_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp]),
+    "afc_vc_verify_json_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_vc_audit_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_audit_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),

@@ -91,6 +91,16 @@ cudaError_t vc_emit(const void* schema, const uint8_t* docs, const uint64_t* doc
                     cudaStream_t s, LaunchLog* lg);
 cudaError_t vc_fold(uint8_t* status, const uint8_t* ok, uint32_t n, cudaStream_t s, LaunchLog* lg);
 
+// ---- k_vcjson.cu: credential documents in any JSON spelling (afc_vcjson.cuh).  schema: a VcjSchema on the device (vcj_schema_bytes()).
+size_t vcj_schema_bytes();
+int vcj_schema_host(int doc_kind, void* out);          // builds the host copy of a schema; -1 for an unknown kind
+// the outputs of vc_parse; len_out[i] = length of the re-marshalled signing message (0 unless candidate)
+cudaError_t vcj_parse(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint8_t* dids, const uint32_t* did_off,
+                      const uint32_t* slots, uint32_t slot_mask, uint8_t* status, uint64_t* len_out, uint8_t* sigs, uint32_t* key_index,
+                      uint32_t* fields, cudaStream_t s, LaunchLog* lg);
+cudaError_t vcj_emit(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint64_t* msg_off, uint8_t* msgs,
+                     cudaStream_t s, LaunchLog* lg);
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

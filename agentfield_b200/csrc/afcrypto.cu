@@ -129,6 +129,7 @@ struct afc_keyset {
     uint32_t* d_slots = nullptr;   // slot_mask + 1 entries, 0xffffffff = empty
     uint32_t slot_mask = 0;
     uint8_t* d_schemas = nullptr;  // 2 x launch::vc_schema_bytes(): execution VC, workflow VC
+    uint8_t* d_vcj_schemas = nullptr;  // 2 x launch::vcj_schema_bytes(): the same for documents in any spelling (afc_vcjson.cuh)
 };
 
 struct afc_merkle_tree {
@@ -285,7 +286,7 @@ cudaError_t h2d(Slot& sl, void* dst, const void* src, size_t bytes, bool pinned,
 
 inline bool aligned16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED, OP_VC_AUDIT };
+enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED, OP_VC_AUDIT, OP_VC_JSON };
 
 struct BatchArgs {
     Op op;
@@ -311,10 +312,11 @@ size_t vc_scratch_bytes(uint32_t n, uint64_t doc_bytes, uint32_t n_keys, bool au
 // docs + doc_off[i] is document i (absolute offsets); the signing messages of a batch are never longer than its documents
 // (D[0:p] plus the zero-proof text, which is no longer than the proof object it replaces), so doc_bytes bounds their buffer.
 // With `issues` (the audit) the parse also captures each document and k_vc_crosscheck compares it with its record's columns; the
-// scratch area then needs vc_scratch_bytes(..., true).
+// scratch area then needs vc_scratch_bytes(..., true).  With `json` (afc_vc_verify_json_batch) documents in any spelling are read and
+// re-marshalled by k_vcj_parse / k_vcj_emit, which decline a message longer than its document, so the same bound holds.
 cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
                               uint64_t doc_bytes, uint8_t* status, uint32_t* fields, uint8_t* scratch, cudaStream_t st, launch::LaunchLog* lg,
-                              uint32_t* issues = nullptr, const uint8_t* cols = nullptr, const uint64_t* col_off = nullptr) {
+                              uint32_t* issues = nullptr, const uint8_t* cols = nullptr, const uint64_t* col_off = nullptr, bool json = false) {
     if (n == 0) return cudaSuccess;
     uint8_t* p = scratch;
     auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
@@ -326,8 +328,12 @@ cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, cons
     uint64_t* scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n));
     uint32_t* kscr = (uint32_t*)take((size_t)n * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, n));
     const void* schema = ks->d_schemas + (size_t)kind * launch::vc_schema_bytes();
+    const void* jschema = ks->d_vcj_schemas + (size_t)kind * launch::vcj_schema_bytes();
     cudaError_t e;
-    if (issues) {
+    if (json) {
+        e = launch::vcj_parse(jschema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
+                              kidx, fields, st, lg);
+    } else if (issues) {
         uint32_t* caps = (uint32_t*)take(launch::vc_capture_bytes(n));
         e = launch::vc_parse_capture(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
                                      kidx, caps, st, lg);
@@ -337,7 +343,8 @@ cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, cons
                              kidx, fields, st, lg);
     }
     if (e == cudaSuccess) e = launch::offsets_from_lengths(msg_off, n, scan, st, lg);
-    if (e == cudaSuccess) e = launch::vc_emit(schema, docs, doc_off, n, msg_off, msgs, st, lg);
+    if (e == cudaSuccess) e = json ? launch::vcj_emit(jschema, docs, doc_off, n, msg_off, msgs, st, lg)
+                                   : launch::vc_emit(schema, docs, doc_off, n, msg_off, msgs, st, lg);
     if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, kidx, sigs, msgs, msg_off, n, ok,
                                                             kscr, kscr + (size_t)n * 8, st, lg);
     if (e == cudaSuccess) e = launch::vc_fold(status, ok, n, st, lg);
@@ -427,7 +434,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
             CK(sl.koff.reserve((size_t)(cnt + 1) * 4));
         }
         if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index) CK(sl.koff.reserve((size_t)cnt * 4));
-        if (A.op == OP_VC_STORED) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys)));
+        if (A.op == OP_VC_STORED || A.op == OP_VC_JSON) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys)));
         if (A.op == OP_VC_AUDIT) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys, true)));
         uint64_t cbase = 0, cbytes = 0;             // audit: this chunk's columns (slot buffers a: bytes, koff: offsets)
         if (A.col_off) {
@@ -478,8 +485,9 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
             break;
         }
         case OP_VC_STORED:
+        case OP_VC_JSON:
             e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, A.out2 ? (uint32_t*)sl.b.p : nullptr, sl.vc.p,
-                                  sl.stream, lc);
+                                  sl.stream, lc, nullptr, nullptr, nullptr, A.op == OP_VC_JSON);
             break;
         case OP_VC_AUDIT: {
             const uint8_t* d_cols = nullptr; const uint64_t* d_coff = nullptr;
@@ -1003,7 +1011,7 @@ void afc_keyset_free(afc_keyset* ks) {
     if (ks->d_pks) cudaFree(ks->d_pks);
     if (ks->d_valid) cudaFree(ks->d_valid);
     if (ks->d_tabs) cudaFree(ks->d_tabs);
-    void* named[] = {ks->d_dids, ks->d_did_off, ks->d_slots, ks->d_schemas};
+    void* named[] = {ks->d_dids, ks->d_did_off, ks->d_slots, ks->d_schemas, ks->d_vcj_schemas};
     for (void* p : named) if (p) cudaFree(p);
     delete ks;
 }
@@ -1067,17 +1075,22 @@ int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, 
     ks->slot_mask = cap - 1;
     const size_t sb = launch::vc_schema_bytes();
     std::vector<uint8_t> schemas(2 * sb);
-    if (launch::vc_schema_host(0, schemas.data()) != 0 || launch::vc_schema_host(1, schemas.data() + sb) != 0) {
+    const size_t jb = launch::vcj_schema_bytes();
+    std::vector<uint8_t> jschemas(2 * jb);
+    if (launch::vc_schema_host(0, schemas.data()) != 0 || launch::vc_schema_host(1, schemas.data() + sb) != 0 ||
+        launch::vcj_schema_host(0, jschemas.data()) != 0 || launch::vcj_schema_host(1, jschemas.data() + jb) != 0) {
         afc_keyset_free(ks); *out = nullptr; return AFC_EINVAL;
     }
     cudaError_t e = cudaMalloc((void**)&ks->d_dids, total + 4);
     if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_did_off, ((size_t)n_keys + 1) * 4);
     if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_slots, (size_t)cap * 4);
     if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_schemas, 2 * sb);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&ks->d_vcj_schemas, 2 * jb);
     if (e == cudaSuccess && total) e = cudaMemcpy(ks->d_dids, dids + base, total, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(ks->d_did_off, off.data(), ((size_t)n_keys + 1) * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(ks->d_slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(ks->d_schemas, schemas.data(), 2 * sb, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(ks->d_vcj_schemas, jschemas.data(), 2 * jb, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
         set_err(ctx, e, "afc_keyset_new_named");
         afc_keyset_free(ks); *out = nullptr;
@@ -1100,8 +1113,9 @@ int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const
     A.out = status; A.out_item = 1; A.out2 = (uint8_t*)fields; A.out2_item = fields ? 16 : 0;
     return run_host_batch(ctx, A);
 }
-int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
-                                   uint8_t* d_status, uint32_t* d_fields, void* stream) {
+// the _dev form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
+static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n, uint8_t* d_status,
+                         uint32_t* d_fields, void* stream, bool json) {
     int rc = vc_stored_check(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status);
     if (rc != AFC_OK || n == 0) return rc;
     if (d_fields && !aligned16(d_fields)) return AFC_EINVAL;
@@ -1115,10 +1129,29 @@ int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, c
     if (ends[1] < ends[0]) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys), st));
-    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, d_fields, scratch, st, lc);
+    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, d_fields, scratch, st, lc, nullptr,
+                                      nullptr, nullptr, json);
     cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;
+}
+int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
+                                   uint8_t* d_status, uint32_t* d_fields, void* stream) {
+    return vc_verify_dev(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, stream, false);
+}
+
+// documents in any JSON spelling: the arguments, statuses and fields of afc_vc_verify_stored_batch
+int afc_vc_verify_json_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                             uint8_t* status, uint32_t* fields) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
+    if (rc != AFC_OK) return rc;
+    BatchArgs A{}; A.op = OP_VC_JSON; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
+    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)fields; A.out2_item = fields ? 16 : 0;
+    return run_host_batch(ctx, A);
+}
+int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
+                                 uint8_t* d_status, uint32_t* d_fields, void* stream) {
+    return vc_verify_dev(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, stream, true);
 }
 
 // audit: the arguments of afc_vc_verify_stored_batch, plus columns exactly for execution documents

@@ -162,6 +162,27 @@ class KeySet:
         buf, off = pack(docs)
         return self.verify_stored_packed(doc_kind, buf, off)
 
+    def verify_json_packed(self, doc_kind, buf, off, fields=True):
+        """afc_vc_verify_json_batch: verify_stored_packed for documents in any JSON spelling (request bodies, files), re-marshalled on
+        the device.  Same statuses and fields (spans into each input document)."""
+        n = len(off) - 1
+        st = np.empty(n, dtype=np.uint8)
+        fl = np.empty((n, 4), dtype=np.uint32) if fields else None
+        _abi.check(self._lib.afc_vc_verify_json_batch(self.ctx.handle, self.handle, doc_kind, _abi.ptr(buf), _abi.ptr(off), n, _abi.ptr(st),
+                                                      _abi.ptr(fl)), self.ctx.handle)
+        return st, fl
+
+    def verify_json_dev(self, doc_kind, d_docs, d_off, n, d_status, d_fields=None, stream=None):
+        _abi.check(self._lib.afc_vc_verify_json_batch_dev(self.ctx.handle, self.handle, doc_kind, _abi.ptr(d_docs), _abi.ptr(d_off), n,
+                                                          _abi.ptr(d_status), _abi.ptr(d_fields), self.ctx._stream(stream)), self.ctx.handle)
+
+    def verify_json(self, doc_kind, docs):
+        """Host convenience: a list of documents in any JSON spelling (bytes) -> (statuses, fields)."""
+        if not docs:
+            return np.zeros(0, dtype=np.uint8), np.zeros((0, 4), dtype=np.uint32)
+        buf, off = pack(docs)
+        return self.verify_json_packed(doc_kind, buf, off)
+
     def audit_stored_packed(self, doc_kind, buf, off, cols=None, col_off=None):
         """afc_vc_audit_stored_batch: n stored documents (packed bytes + n+1 offsets) and, for execution documents, their records'
         _abi.AUDIT_COLUMNS columns (packed bytes + n*10+1 offsets) -> (status uint8 [n], issues uint32 [n] of _abi.AUDIT_* bits)."""

@@ -296,12 +296,25 @@ class VCService:
             self._stored_keyset_dids = dids
         return self._stored_keyset
 
-    def _verify_stored(self, kind, stored_docs):
+    # -- documents in any JSON spelling verified on the device (afc_vc_verify_json_batch)
+    def verify_vc_json_batch(self, raw_docs):
+        """VerifyVC(json.RawMessage) (vc_service.go:242-289) for many execution-VC documents as clients send them: request bodies of
+        POST /api/v1/did/verify and files given to `af vc verify`, in any JSON spelling.  Returns what verify_stored_vc_batch returns;
+        the spellings real clients produce are re-marshalled and verified on the GPU, only the others here."""
+        return self._verify_stored(_abi.DOC_EXECUTION_VC, raw_docs, json_spelling=True)
+
+    def verify_workflow_vc_json_batch(self, raw_docs):
+        """The same for workflow-VC documents (verifyWorkflowVCSignature, vc_service.go:1589-1625)."""
+        return self._verify_stored(_abi.DOC_WORKFLOW_VC, raw_docs, json_spelling=True)
+
+    def _verify_stored(self, kind, stored_docs, json_spelling=False):
+        """json_spelling: the device call re-marshals documents in any spelling (afc_vc_verify_json_batch); it declines invalid UTF-8,
+        so the spans of the documents it accepts decode exactly as Go decodes them."""
         docs = [bytes(d) for d in stored_docs]
         n = len(docs)
         ks = self._named_keyset()
         if ks is not None and n:
-            status, fields = ks.verify_stored(kind, docs)
+            status, fields = (ks.verify_json if json_spelling else ks.verify_stored)(kind, docs)
         else:
             status, fields = np.full(n, _abi.VC_HOST, dtype=np.uint8), np.zeros((n, 4), dtype=np.uint32)
         out = [None] * n

@@ -24,8 +24,11 @@ type Resolver func(did string) (ed25519.PublicKey, error)
 
 // StoredVerifier verifies stored credential documents from their bytes and answers exactly what VCService.VerifyVC
 // (internal/services/vc_service.go:242-289) answers for each: parse, resolve the issuer, decode the signature, verify.
+// VerifyStoredBatch is for documents as the control plane stores them (json.Marshal's form); VerifyJSONBatch for documents in
+// any JSON spelling (request bodies, files).  Both answer the same; they differ in which documents the GPU form can take.
 type StoredVerifier interface {
 	VerifyStoredBatch(kind DocKind, docs []json.RawMessage, resolve Resolver) ([]types.VCVerificationResponse, error)
+	VerifyJSONBatch(kind DocKind, docs []json.RawMessage, resolve Resolver) ([]types.VCVerificationResponse, error)
 }
 
 // StoredStdlib is the reference's own path, one document at a time: Unmarshal, zero the proof, Marshal, Verify.
@@ -37,6 +40,12 @@ func (StoredStdlib) VerifyStoredBatch(kind DocKind, docs []json.RawMessage, reso
 		out[i] = verifyStoredOne(kind, d, resolve)
 	}
 	return out, nil
+}
+
+// VerifyJSONBatch is VerifyVC for documents as clients send them, in any JSON spelling; the stdlib path is the same
+// Unmarshal -> Marshal -> Verify, which does not depend on the spelling.
+func (StoredStdlib) VerifyJSONBatch(kind DocKind, docs []json.RawMessage, resolve Resolver) ([]types.VCVerificationResponse, error) {
+	return StoredStdlib{}.VerifyStoredBatch(kind, docs, resolve)
 }
 
 func verifyStoredOne(kind DocKind, doc json.RawMessage, resolve Resolver) types.VCVerificationResponse {

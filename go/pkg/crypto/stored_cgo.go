@@ -57,6 +57,17 @@ func NewStoredCUDA(c *CUDA, issuers map[string]ed25519.PublicKey) (*StoredCUDA, 
 func (s *StoredCUDA) Close() { C.afc_keyset_free(s.ks) }
 
 func (s *StoredCUDA) VerifyStoredBatch(kind DocKind, docs []json.RawMessage, resolve Resolver) ([]types.VCVerificationResponse, error) {
+	return s.verifyBatch(kind, docs, resolve, false)
+}
+
+// VerifyJSONBatch is VerifyVC for documents as clients send them (request bodies of POST /api/v1/did/verify, files given to
+// `af vc verify`), in any JSON spelling: the device re-marshals them (afc_vc_verify_json_batch).  Documents it leaves to the
+// host go through verifyStoredOne, which handles any spelling.
+func (s *StoredCUDA) VerifyJSONBatch(kind DocKind, docs []json.RawMessage, resolve Resolver) ([]types.VCVerificationResponse, error) {
+	return s.verifyBatch(kind, docs, resolve, true)
+}
+
+func (s *StoredCUDA) verifyBatch(kind DocKind, docs []json.RawMessage, resolve Resolver, anySpelling bool) ([]types.VCVerificationResponse, error) {
 	n := len(docs)
 	if n == 0 {
 		return nil, nil
@@ -81,10 +92,20 @@ func (s *StoredCUDA) VerifyStoredBatch(kind DocKind, docs []json.RawMessage, res
 		pos += copy(b[pos:], d)
 	}
 	o[n] = uint64(pos)
-	rc := C.afc_vc_verify_stored_batch(s.ctx, s.ks, C.int(kind), (*C.uint8_t)(buf), (*C.uint64_t)(off), C.uint32_t(n),
-		(*C.uint8_t)(status), (*C.uint32_t)(fields))
+	var rc C.int
+	if anySpelling {
+		rc = C.afc_vc_verify_json_batch(s.ctx, s.ks, C.int(kind), (*C.uint8_t)(buf), (*C.uint64_t)(off), C.uint32_t(n),
+			(*C.uint8_t)(status), (*C.uint32_t)(fields))
+	} else {
+		rc = C.afc_vc_verify_stored_batch(s.ctx, s.ks, C.int(kind), (*C.uint8_t)(buf), (*C.uint64_t)(off), C.uint32_t(n),
+			(*C.uint8_t)(status), (*C.uint32_t)(fields))
+	}
 	if rc != 0 {
-		observeFallback("verify_stored")
+		if anySpelling {
+			observeFallback("verify_json")
+		} else {
+			observeFallback("verify_stored")
+		}
 		return StoredStdlib{}.VerifyStoredBatch(kind, docs, resolve)
 	}
 	st := unsafe.Slice((*byte)(status), n)

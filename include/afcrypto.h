@@ -173,6 +173,25 @@ int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const
 int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                    uint8_t* d_status, uint32_t* d_fields, void* stream);
 
+/* ---- credential documents in any JSON spelling verified on the device ------------------------------------------------------
+ * VerifyVC for documents that arrive from outside: request bodies of POST /api/v1/did/verify (internal/handlers/did_handlers.go:97-111)
+ * and files given to `af vc verify` (internal/cli/vc.go:159), as the Python SDK (json.dumps), the web UI (JSON.stringify, also
+ * pretty-printed) or any other client spells them.  The device reads each document, writes Go's canonical text of it (what
+ * json.Marshal(json.Unmarshal(D)) writes, with the zero proof) and verifies that.  Arguments, statuses, fields (spans into the input
+ * document), chunking and errors are those of afc_vc_verify_stored_batch; a bad kind or NULL is AFC_EINVAL, a key set without DIDs
+ * AFC_ESTATE.  Accepted: whitespace between tokens; every JSON string escape (backslash-u in either case, surrogate pairs), each
+ * character re-escaped with Go's rules; int members -?(0|[1-9][0-9]*) up to 18 digits (-0 is 0); metadata values that are strings,
+ * true / false / null, integers of up to 15 digits (-0 kept) and arrays / objects up to 8 deep, keys without backslashes in strictly
+ * increasing byte order; "errorMessage":"" and "endTime":null (omitted), "endTime":"" (written).  AFC_VC_HOST (the caller runs
+ * Unmarshal -> Marshal -> Verify itself) for: member order other than the struct's, missing, unknown, duplicate, re-cased or escaped
+ * member names, null for a string, anything that is not JSON (BOM, NaN, trailing commas, raw control bytes, leading zeros),
+ * fractions, exponents and longer integers, unsorted or duplicate metadata keys, depth beyond 8, a backslash in issuer or
+ * proofValue, raw invalid UTF-8, lone surrogate escapes, and a canonical message longer than the document. */
+int afc_vc_verify_json_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                             uint8_t* status, uint32_t* fields);
+int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
+                                 uint8_t* d_status, uint32_t* d_fields, void* stream);
+
 /* ---- stored credentials audited against their records on the device ---------------------------------------------------------
  * replaces, per credential, the checks of VCService.VerifyExecutionVCComprehensive (internal/services/vc_service.go:926-1005):
  * json.Unmarshal, performIntegrityChecks (:1008-1181), performSecurityAnalysis (:1184-1233) and performComplianceChecks

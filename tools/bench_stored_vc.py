@@ -3,7 +3,9 @@
 Prints one JSON line: documents/s of the device-pointer call with its per-kernel split, of the keyed verify alone over the same
 signing bytes already rendered, and of the host-buffer call; host_fallback and all_expected; the card and its power limit, read
 in the same run.  The audit_stored block does the same for the audit of stored execution VCs against their records
-(afc_vc_audit_stored_batch[_dev]), next to the stored-verify device call on the same documents.  Needs a CUDA device; writes nothing.
+(afc_vc_audit_stored_batch[_dev]), next to the stored-verify device call on the same documents.  The verify_json block measures
+documents in three client spellings (afc_vc_verify_json_batch_dev) next to the stored-verify call on the canonical form.  Needs a
+CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R]"""
 import argparse
 import json
@@ -135,11 +137,49 @@ def audit_stored_block(ctx, dev, timed):
             "host_fallback": host_fallback, "undecided": undecided, "all_expected": all_expected}
 
 
+def verify_json_block(ctx, dev, timed):
+    """Documents in any JSON spelling re-marshalled on the device (afc_vc_verify_json_batch): 2^20 execution VCs from 1024 issuers,
+    1 % with a corrupted signature, in three spellings: the canonical bytes, json.dumps(doc, indent=2, ensure_ascii=False) (the shape
+    of JSON.stringify(doc, null, 2)) and json.dumps(doc) (what requests sends).  2^16 distinct documents are built on the device,
+    re-spelled on the host with every number token kept, tiled to 2^20, then corrupted.  Beside them, the stored-verify call on the
+    canonical form.  host_fallback must be 0 and all_expected true for every spelling."""
+    import torch
+    from agentfield_b200.respell import respelled_stored_vcs_dev
+    n, K = 1 << 20, 1024
+    out = {"docs": n, "issuers": K}
+    for name, how in (("canonical", None), ("indent2_no_ascii", "js_pretty"), ("dumps", "dumps")):
+        d_docs, d_off, ks, want = respelled_stored_vcs_dev(ctx, dev, n, K, 0xAF09, how)
+        d_st = torch.empty(n, dtype=torch.uint8, device=dev)
+        run = lambda: ks.verify_json_dev(0, d_docs, d_off, n, d_st)
+        ms = timed(run)
+        r = {"bytes": int(d_off[-1]), "docs_per_s": n / (ms * 1e-3), "ms": ms, "host_fallback": int((d_st == 2).sum()),
+             "all_expected": bool(torch.equal(d_st, want))}
+        ctx.profile_begin()
+        timed(run, reps=3)
+        r["kernels_ms"] = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+        if how is None:
+            d_st2 = torch.empty(n, dtype=torch.uint8, device=dev)
+            stored = lambda: ks.verify_stored_dev(0, d_docs, d_off, n, d_st2)
+            ms_s = timed(stored)
+            ctx.profile_begin()
+            timed(stored, reps=3)
+            out["stored_dev_call"] = {"docs_per_s": n / (ms_s * 1e-3), "ms": ms_s, "all_expected": bool(torch.equal(d_st2, want)),
+                                      "kernels_ms": {k: v["avg_ms"] for k, v in ctx.profile_end().items()},
+                                      "note": "afc_vc_verify_stored_batch_dev on the canonical documents"}
+        out[name] = r
+        ks.close()
+        del d_docs, d_off
+    out["gpu"] = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                capture_output=True, text=True).stdout.strip()
+    return out
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json"], default=None, help="run one block")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     ctx = afb.Context(0)
@@ -152,7 +192,8 @@ def main():
             fn()
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
-    print(json.dumps({"stored_vc_verify": stored_vc_block(ctx, dev, timed), "audit_stored": audit_stored_block(ctx, dev, timed)}), flush=True)
+    blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block}
+    print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
 
