@@ -19,6 +19,9 @@ AUDIT_COLUMNS = ("issuer_did", "execution_id", "workflow_id", "session_id", "cal
 AUDIT_INVALID_TIMESTAMP, AUDIT_MISSING_CONTEXT, AUDIT_MISSING_TYPE, AUDIT_MISSING_ID = 1 << 10, 1 << 11, 1 << 12, 1 << 13
 AUDIT_MISSING_ISSUER, AUDIT_MISSING_ISSUANCE_DATE, AUDIT_NOT_W3C, AUDIT_NOT_AGENTFIELD = 1 << 14, 1 << 15, 1 << 16, 1 << 17
 AUDIT_STATUS_UNDECIDED, AUDIT_TIMESTAMP_UNDECIDED = 1 << 18, 1 << 19
+ISSUE_COLUMNS = ("vc_id", "caller_did", "issuance_date", "execution_id", "workflow_id", "session_id", "caller_type", "agent_node_did",
+                 "target_did", "function_name", "timestamp", "status", "error_message", "proof_created")
+ISSUE_HASH_DATA = 1
 MERKLE_STATE_BYTES = 8 + 64 * 32
 SHA256_STATE_BYTES = 108
 
@@ -79,6 +82,11 @@ SYMBOLS = {
     "afc_vc_verify_json_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_vc_audit_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_audit_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp, vp]),
+    "afc_vc_issue_bound": (C.c_uint64, [vp, C.c_uint32]),
+    "afc_vc_issue_execution_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, vp, vp,
+                                               vp]),
+    "afc_vc_issue_execution_batch_dev": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, vp,
+                                                   vp, vp, vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),
     "afc_merkle_free": (None, [vp]),
     "afc_merkle_append": (C.c_int, [vp, vp, vp, C.c_uint32, vp, u64p]),

@@ -229,3 +229,35 @@ def synthetic_stored_vcs_dev(ctx, d_expanded, dids, d_key_index, n, seed=0, str_
     # issuer, executionId, workflowId, sessionId, caller.did, target.did, status, inputHash, outputHash, proofValue
     d_cols, d_col_off = packed([cols[k] for k in (3, 5, 6, 7, 8, 11, 18, 14, 15, 27)])
     return d_docs, d_doff, d_msgs, d_moff, d_sigs, d_cols, d_col_off
+
+
+def synthetic_issue_requests(dids, n, seed=0, payload_bytes=(64, 2048), nil_frac=0.1, err_frac=0.01, long_frac=0.0, long_bytes=256 << 10):
+    """n GenerateExecutionVC requests (the dicts of services.VCService.generate_execution_vc_batch) of realistic shape: issuers drawn
+    from `dids` in turn, UUID-like ids, RFC 3339 times, input and output payloads of payload_bytes[0]..payload_bytes[1] bytes (uniform,
+    seeded; nil_frac of them nil), err_frac of the requests with an error message that needs escaping (a third of those longer than
+    500 bytes, cut inside a rune), and long_frac of the payloads long_bytes long.  The payloads are views of one random buffer."""
+    rng = np.random.default_rng(seed)
+    lo, hi = payload_bytes
+    lens = rng.integers(lo, hi + 1, 2 * n)
+    lens[rng.random(2 * n) < long_frac] = long_bytes
+    nil = rng.random(2 * n) < nil_frac
+    starts = rng.integers(0, 4096, 2 * n)
+    pool = memoryview(rng.integers(0, 256, int(lens.max()) + 4096, dtype=np.uint8).tobytes())
+    errs = np.flatnonzero(rng.random(n) < err_frac)
+    err_text = {}
+    for j, i in enumerate(errs):
+        base = 'tool "fetch" failed: <status 502> & retry\n\tline 2   ' + "é中\U0001F600" * int(rng.integers(1, 8))
+        err_text[int(i)] = base * (40 if j % 3 == 0 else 1)
+    statuses = ("succeeded", "failed", "running", "completed", "timeout")
+    out = []
+    for i in range(n):
+        did = dids[i % len(dids)]
+        p = [None if nil[2 * i + k] else pool[int(starts[2 * i + k]):int(starts[2 * i + k] + lens[2 * i + k])] for k in (0, 1)]
+        out.append({"vc_id": "%08x-4e7a-4b1c-9d2e-%012x" % (i, i * 2654435761 % (1 << 48)), "caller_did": did,
+                    "issuance_date": "2026-09-21T06:%02d:%02dZ" % (i // 60 % 60, i % 60), "execution_id": "exec_%016x" % i,
+                    "workflow_id": "wf_%08x" % (i // 16), "session_id": "sess_%06x" % (i // 256), "caller_type": "agent",
+                    "agent_node_did": dids[(i + 1) % len(dids)], "target_did": dids[(i + 7) % len(dids)], "function_name": "tool.fetch_%d" % (i % 97),
+                    "input": p[0], "output": p[1], "status": statuses[i % len(statuses)], "error_message": err_text.get(i, ""),
+                    "duration_ms": int(rng.integers(0, 10 ** 7)), "timestamp": "2026-09-21T05:59:%02d.%06dZ" % (i % 60, i % 1000000),
+                    "proof_created": "2026-09-21T06:00:01Z"})
+    return out

@@ -101,6 +101,21 @@ cudaError_t vcj_parse(const void* schema, const uint8_t* docs, const uint64_t* d
 cudaError_t vcj_emit(const void* schema, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, const uint64_t* msg_off, uint8_t* msgs,
                      cudaStream_t s, LaunchLog* lg);
 
+// ---- k_vcissue.cu: execution credentials issued on the device (afc_vcissue.cuh).  col_off: 14 absolute offsets per credential + 1;
+// hashes: 2 x 43 characters per credential (input, output), nullptr without HashSensitiveData
+// payload j of 2n (input i = 2i, output i = 2i + 1) -> hashData characters at hashes + 43 j
+cudaError_t vci_hashdata(const uint8_t* payloads, const uint64_t* payload_off, const uint8_t* nil, uint32_t m, uint8_t* hashes, cudaStream_t s,
+                         LaunchLog* lg);
+// the signing-message and stored-document length of each credential (write them to off + 1 for offsets_from_lengths)
+cudaError_t vci_sizes(const uint8_t* cols, const uint64_t* col_off, const int64_t* duration, const uint8_t* hashes, uint32_t n, uint64_t* msg_len,
+                      uint64_t* doc_len, cudaStream_t s, LaunchLog* lg);
+// both byte strings of each credential; the stored document's proofValue is a placeholder until vci_proof
+cudaError_t vci_fill(const uint8_t* cols, const uint64_t* col_off, const int64_t* duration, const uint8_t* hashes, uint32_t n, const uint64_t* msg_off,
+                     uint8_t* msgs, const uint64_t* doc_off, uint8_t* docs, cudaStream_t s, LaunchLog* lg);
+// sigs: n x 64, 16-byte aligned -> 86 characters into each stored document and into proof_values (n x 86)
+cudaError_t vci_proof(const uint8_t* sigs, uint32_t n, const uint64_t* doc_off, uint8_t* docs, uint8_t* proof_values, cudaStream_t s, LaunchLog* lg);
+uint64_t vci_literal_bytes();          // constant text of both document forms together
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

@@ -367,6 +367,16 @@ struct LaneDrain {
     ~LaneDrain() { if (armed) for (int w = 0; w < kSlots; w++) cudaStreamSynchronize(lane.slot[w].stream); }
 };
 
+// AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments (read once per process)
+uint32_t max_chunk_items() {
+    static const uint32_t v = [] { const char* e = getenv("AFC_CHUNK_ITEMS"); uint32_t x = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return x ? x : kChunkItems; }();
+    return v;
+}
+uint32_t min_chunk_items() {
+    static const uint32_t v = [] { const char* e = getenv("AFC_MIN_CHUNK_ITEMS"); uint32_t x = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return x ? x : kMinChunkItems; }();
+    return v;
+}
+
 int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
     if (A.n == 0) return AFC_OK;
     if (A.koff && !monotone(A.koff, A.n)) return AFC_EINVAL;
@@ -382,9 +392,7 @@ int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
     const bool pin_cols = A.cols ? is_pinned(A.cols) : true, pin_coff = A.col_off ? is_pinned(A.col_off) : true;
     const uint32_t C = AFC_AUDIT_COLUMNS;
     CallLog lc(ctx, 12 * (int)(A.n / kChunkItems + 8) + 8);
-    // AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments
-    static const uint32_t max_chunk = [] { const char* e = getenv("AFC_CHUNK_ITEMS"); uint32_t v = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return v ? v : kChunkItems; }();
-    static const uint32_t min_chunk = [] { const char* e = getenv("AFC_MIN_CHUNK_ITEMS"); uint32_t v = e ? (uint32_t)strtoul(e, nullptr, 10) : 0; return v ? v : kMinChunkItems; }();
+    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
     uint32_t i0 = 0;
     int which = 0;
     struct Pending { uint32_t i0, cnt; bool active; } pend[kSlots] = {};
@@ -1191,6 +1199,247 @@ int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, co
     cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;
+}
+
+// ---------------------------------------------------------------------------------- issuing execution credentials
+// Bounds from the column bytes alone (so that the _dev call needs nothing but the two ends of col_off): each credential's constant
+// text, four digests, a 20-character int64, the 86 proofValue characters and the errorMessage member's frame and suffix, plus at
+// most 6 bytes per column byte (backslash-u 00XX, or backslash-u fffd for an invalid byte) for each of its at most 3 appearances in the stored document
+// (caller_did: issuer, caller.did, verificationMethod) and 2 in the signing message.
+static uint64_t issue_fixed_bytes() { return launch::vci_literal_bytes() + 4 * 43 + 20 + 86 + 32; }
+static uint64_t issue_doc_bound(uint32_t n, uint64_t col_bytes) { return (uint64_t)n * issue_fixed_bytes() + 18 * col_bytes; }
+static uint64_t issue_msg_bound(uint32_t n, uint64_t col_bytes) { return (uint64_t)n * issue_fixed_bytes() + 12 * col_bytes; }
+
+uint64_t afc_vc_issue_bound(const uint64_t* col_off, uint32_t n) {
+    if (!col_off || n == 0) return 0;
+    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_ISSUE_COLUMNS];
+    return issue_doc_bound(n, b >= a ? b - a : 0);
+}
+
+// per-call device scratch: signing messages and their offsets, signatures, scan tiles
+struct IssueScratch { uint8_t* msgs; uint64_t* msg_off; uint8_t* sigs; uint64_t* scan; };
+static size_t issue_scratch_bytes(uint32_t n, uint64_t col_bytes) {
+    return vc_align(issue_msg_bound(n, col_bytes) + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) +
+           vc_align(launch::json_scan_scratch_bytes(n));
+}
+static IssueScratch issue_scratch(uint8_t* p, uint32_t n, uint64_t col_bytes) {
+    IssueScratch s;
+    s.msgs = p; p += vc_align(issue_msg_bound(n, col_bytes) + 64);
+    s.msg_off = (uint64_t*)p; p += vc_align(((size_t)n + 1) * 8);
+    s.sigs = p; p += vc_align((size_t)n * 64);
+    s.scan = (uint64_t*)p;
+    return s;
+}
+// hashData, both lengths, both scans: doc_off is complete when this has run
+static cudaError_t issue_sizes(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* pay, const uint64_t* pay_off,
+                               const uint8_t* nil, uint8_t* hashes, uint32_t n, uint64_t* doc_off, const IssueScratch& S, cudaStream_t st,
+                               launch::LaunchLog* lg) {
+    cudaError_t e = hashes ? launch::vci_hashdata(pay, pay_off, nil, 2 * n, hashes, st, lg) : cudaSuccess;
+    if (e == cudaSuccess) e = launch::vci_sizes(cols, col_off, dur, hashes, n, S.msg_off + 1, doc_off + 1, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(S.msg_off, n, S.scan, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(doc_off, n, S.scan, st, lg);
+    return e;
+}
+// both byte strings, the signatures, the proofValues
+static cudaError_t issue_finish(afc_ctx* ctx, const uint8_t* d_exp, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                const uint64_t* col_off, const int64_t* dur, const uint8_t* hashes, uint32_t n, uint8_t* docs, const uint64_t* doc_off,
+                                uint8_t* pv, const IssueScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = launch::vci_fill(cols, col_off, dur, hashes, n, S.msg_off, S.msgs, doc_off, docs, st, lg);
+    if (e == cudaSuccess) e = launch::ed_sign_expanded_batch(ctx->comb, afc_internal_sign_table(ctx), d_exp, n_keys, key_index, S.msgs, S.msg_off, n,
+                                                             S.sigs, st, lg);
+    if (e == cudaSuccess) e = launch::vci_proof(S.sigs, n, doc_off, docs, pv, st, lg);
+    return e;
+}
+static int issue_check(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                       const uint64_t* col_off, const int64_t* duration_ms, const uint8_t* payloads, const uint64_t* payload_off,
+                       const uint8_t* payload_nil, uint32_t flags, uint32_t n, afc_merkle* log, const uint8_t* docs, const uint64_t* doc_off,
+                       const uint8_t* hashes, const uint8_t* proof_values) {
+    if (!ctx || !col_off || !doc_off || (flags & ~(uint32_t)AFC_ISSUE_HASH_DATA)) return AFC_EINVAL;
+    if (log && log->ctx != ctx) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!expanded96 || n_keys == 0 || !key_index || !cols || !duration_ms || !docs || !proof_values) return AFC_EINVAL;
+    if ((flags & AFC_ISSUE_HASH_DATA) && (!hashes || !payloads || !payload_off || !payload_nil)) return AFC_EINVAL;
+    return AFC_OK;
+}
+
+int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                     const uint64_t* d_col_off, const int64_t* d_duration_ms, const uint8_t* d_payloads,
+                                     const uint64_t* d_payload_off, const uint8_t* d_payload_nil, uint32_t flags, uint32_t n, afc_merkle* log,
+                                     uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off, uint8_t* d_hashes, uint8_t* d_proof_values,
+                                     void* stream) {
+    int rc = issue_check(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_duration_ms, d_payloads, d_payload_off, d_payload_nil, flags,
+                         n, log, d_docs, d_doc_off, d_hashes, d_proof_values);
+    if (rc != AFC_OK || n == 0) return rc;
+    if (!aligned16(d_expanded96)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t ends[2];                       // the column bytes bound the documents: read them once (one synchronisation)
+    CK(cudaMemcpyAsync(&ends[0], d_col_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[1], d_col_off + (size_t)n * AFC_ISSUE_COLUMNS, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ends[1] < ends[0] || docs_cap < issue_doc_bound(n, ends[1] - ends[0])) return AFC_EINVAL;
+    const uint64_t cb = ends[1] - ends[0];
+    uint8_t* hashes = (flags & AFC_ISSUE_HASH_DATA) ? d_hashes : nullptr;
+    {
+        CallLog lc(ctx);
+        uint8_t* scratch = nullptr;
+        CK(cudaMallocAsync((void**)&scratch, issue_scratch_bytes(n, cb), st));
+        const IssueScratch S = issue_scratch(scratch, n, cb);
+        cudaError_t e = issue_sizes(d_cols, d_col_off, d_duration_ms, d_payloads, d_payload_off, d_payload_nil, hashes, n, d_doc_off, S, st, lc);
+        if (e == cudaSuccess) e = issue_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_duration_ms, hashes, n, d_docs, d_doc_off,
+                                               d_proof_values, S, st, lc);
+        cudaFreeAsync(scratch, st);
+        CK(e);
+    }
+    return log ? afc_merkle_append_dev(log, d_docs, d_doc_off, n, stream) : AFC_OK;
+}
+
+// The host-buffer call: chunks of credentials through the lane's ring.  A chunk's documents land at their final offsets, so its
+// stream is synchronised once after the sizes pass to learn where the chunk ends (the next chunk's copies are enqueued after that).
+static int issue_host_run(afc_ctx* ctx, const uint8_t* d_keys, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
+                          const int64_t* dur, const uint8_t* pay, const uint64_t* pay_off, const uint8_t* nil, bool hash, uint32_t n, afc_merkle* log,
+                          uint8_t* docs, uint64_t* doc_off, uint8_t* hashes, uint8_t* pv) {
+    const uint32_t C = AFC_ISSUE_COLUMNS;
+    LaneGuard lg(ctx);
+    Lane& lane = lg.lane();
+    LaneDrain drain_on_exit(lane);
+    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_dur = is_pinned(dur), pin_ki = is_pinned(key_index);
+    const bool pin_pay = hash ? is_pinned(pay) : true, pin_poff = hash ? is_pinned(pay_off) : true, pin_nil = hash ? is_pinned(nil) : true;
+    const bool pin_docs = is_pinned(docs), pin_h = hash ? is_pinned(hashes) : true, pin_pv = is_pinned(pv);
+    CallLog lc(ctx);
+    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
+    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
+    auto drain = [&](int w) -> int {
+        Pending& p = pend[w];
+        if (!p.active) return AFC_OK;
+        Slot& sl = lane.slot[w];
+        CK(cudaStreamSynchronize(sl.stream));
+        const uint8_t* h = sl.h_out.p;
+        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
+        for (uint32_t j = 0; j < p.cnt; j++) doc_off[p.i0 + j] = p.base + rel[j];
+        if (!pin_h) { memcpy(hashes + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
+        if (!pin_pv) { memcpy(pv + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
+        if (!pin_docs) memcpy(docs + p.base, h, p.bytes);
+        p.active = false;
+        return AFC_OK;
+    };
+    uint32_t i0 = 0;
+    uint64_t base = 0;
+    int which = 0;
+    while (i0 < n) {
+        const uint32_t left = n - i0;
+        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
+        if (limit < min_chunk) limit = min_chunk;
+        if (limit > max_chunk) limit = max_chunk;
+        uint32_t i1 = i0;
+        const uint64_t cbase = col_off[(size_t)i0 * C], pbase = hash ? pay_off[2 * (size_t)i0] : 0;
+        while (i1 < n && i1 - i0 < limit) {
+            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (hash ? pay_off[2 * (size_t)(i1 + 1)] - pbase : 0);
+            if (bytes > kChunkBytes && i1 != i0) break;
+            i1++;
+        }
+        const uint32_t cnt = i1 - i0;
+        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, pbytes = hash ? pay_off[2 * (size_t)i1] - pbase : 0;
+        Slot& sl = lane.slot[which];
+        int rc = drain(which);
+        if (rc != AFC_OK) return rc;
+        const uint64_t dbound = issue_doc_bound(cnt, cbytes);
+        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 8, (size_t)cnt * 4, pbytes + 32, ((size_t)2 * cnt + 1) * 8,
+                             (size_t)2 * cnt, dbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 86, (size_t)cnt * 86, issue_scratch_bytes(cnt, cbytes)};
+        size_t total = 0;
+        for (size_t b : sz) total += vc_align(b);
+        CK(sl.vc.reserve(total));
+        uint8_t* q[12];
+        {
+            uint8_t* p = sl.vc.p;
+            for (int k = 0; k < 12; k++) { q[k] = p; p += vc_align(sz[k]); }
+        }
+        size_t bounce = 0;
+        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_dur ? 0 : (size_t)cnt * 8,
+                                   pin_ki ? 0 : (size_t)cnt * 4, pin_pay ? 0 : pbytes, pin_poff ? 0 : ((size_t)2 * cnt + 1) * 8, pin_nil ? 0 : (size_t)2 * cnt};
+        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
+        CK(sl.h_in.reserve(bounce + 256, ctx));
+        CK(sl.h_out2.reserve(8, ctx));
+        size_t used = 0;
+        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
+        const uint64_t* d_coff = (const uint64_t*)q[1];
+        const int64_t* d_dur = (const int64_t*)q[2];
+        const uint32_t* d_ki = (const uint32_t*)q[3];
+        uint8_t* d_pay = q[4] + (pbase & 15) - pbase;
+        const uint64_t* d_poff = (const uint64_t*)q[5];
+        const uint8_t* d_nil = q[6];
+        uint8_t* d_docs = q[7];
+        uint64_t* d_doff = (uint64_t*)q[8];
+        uint8_t* d_h = hash ? q[9] : nullptr;
+        uint8_t* d_pv = q[10];
+        const IssueScratch S = issue_scratch(q[11], cnt, cbytes);
+        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
+        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
+        CK(h2d(sl, q[2], dur + i0, (size_t)cnt * 8, pin_dur, &used));
+        CK(h2d(sl, q[3], key_index + i0, (size_t)cnt * 4, pin_ki, &used));
+        if (hash) {
+            CK(h2d(sl, q[4] + (pbase & 15), pay + pbase, pbytes, pin_pay, &used));
+            CK(h2d(sl, q[5], pay_off + 2 * (size_t)i0, ((size_t)2 * cnt + 1) * 8, pin_poff, &used));
+            CK(h2d(sl, q[6], nil + 2 * (size_t)i0, (size_t)2 * cnt, pin_nil, &used));
+        }
+        CK(issue_sizes(d_cols, d_coff, d_dur, d_pay, d_poff, d_nil, d_h, cnt, d_doff, S, sl.stream, lc));
+        CK(cudaMemcpyAsync(sl.h_out2.p, d_doff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
+        CK(cudaStreamSynchronize(sl.stream));
+        uint64_t bytes;
+        memcpy(&bytes, sl.h_out2.p, 8);
+        CK(issue_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_dur, d_h, cnt, d_docs, d_doff, d_pv, S, sl.stream, lc));
+        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_h ? 0 : vc_align((size_t)cnt * 86)) + (pin_pv ? 0 : vc_align((size_t)cnt * 86)) +
+                            (pin_docs ? 0 : bytes) + 256, ctx));
+        uint8_t* h = sl.h_out.p;
+        CK(cudaMemcpyAsync(h, d_doff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
+        h += vc_align(((size_t)cnt + 1) * 8);
+        if (hash) {
+            CK(cudaMemcpyAsync(pin_h ? hashes + (size_t)i0 * 86 : h, d_h, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
+            if (!pin_h) h += vc_align((size_t)cnt * 86);
+        }
+        CK(cudaMemcpyAsync(pin_pv ? pv + (size_t)i0 * 86 : h, d_pv, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_pv) h += vc_align((size_t)cnt * 86);
+        CK(cudaMemcpyAsync(pin_docs ? docs + base : h, d_docs, bytes, cudaMemcpyDeviceToHost, sl.stream));
+        if (log) { rc = afc_merkle_append_dev(log, d_docs, d_doff, cnt, sl.stream); if (rc != AFC_OK) return rc; }
+        pend[which] = {i0, cnt, base, bytes, true};
+        base += bytes;
+        which = (which + 1) % kSlots;
+        i0 = i1;
+    }
+    for (int w = 0; w < kSlots; w++) {      // oldest first
+        int rc = drain((which + w) % kSlots);
+        if (rc != AFC_OK) return rc;
+    }
+    drain_on_exit.armed = false;
+    doc_off[n] = base;
+    return AFC_OK;
+}
+
+int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                 const uint64_t* col_off, const int64_t* duration_ms, const uint8_t* payloads, const uint64_t* payload_off,
+                                 const uint8_t* payload_nil, uint32_t flags, uint32_t n, afc_merkle* log, uint8_t* docs, uint64_t docs_cap,
+                                 uint64_t* doc_off, uint8_t* hashes, uint8_t* proof_values) {
+    int rc = issue_check(ctx, expanded96, n_keys, key_index, cols, col_off, duration_ms, payloads, payload_off, payload_nil, flags, n, log, docs,
+                         doc_off, hashes, proof_values);
+    if (rc != AFC_OK) return rc;
+    if (n == 0) { doc_off[0] = 0; return AFC_OK; }
+    const bool hash = (flags & AFC_ISSUE_HASH_DATA) != 0;
+    for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
+    uint64_t bad = 0;
+    for (size_t k = 0; k < (size_t)n * AFC_ISSUE_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
+    if (hash) for (size_t k = 0; k < (size_t)2 * n; k++) bad |= (uint64_t)(payload_off[k + 1] < payload_off[k]);
+    if (bad || docs_cap < afc_vc_issue_bound(col_off, n)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    uint8_t* d_keys = nullptr;
+    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
+    cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        rc = issue_host_run(ctx, d_keys, n_keys, key_index, cols, col_off, duration_ms, payloads, payload_off, payload_nil, hash, n, log, docs, doc_off,
+                            hashes, proof_values);
+    } else { set_err(ctx, e, "cudaMemcpy(expanded keys)"); rc = AFC_ECUDA; }
+    cudaMemset(d_keys, 0, (size_t)n_keys * 96);       // expanded private keys do not outlive the call on the device
+    cudaFree(d_keys);
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------- Merkle log

@@ -66,6 +66,94 @@ class ExpandedKeys:
         torch.cuda.synchronize(dev)
         return [bytes(s) for s in d_sigs.cpu().numpy()]
 
+    def key_index(self, dids):
+        return np.fromiter((self._index[d] for d in dids), dtype=np.uint32, count=len(dids))
+
+    def _issue_bound(self, n, col_bytes):
+        """afc_vc_issue_bound for n requests of col_bytes column bytes in all (the bound is a sum over requests)."""
+        lib = _abi.load()
+        one = np.zeros(len(_abi.ISSUE_COLUMNS) + 1, dtype=np.uint64)
+        fixed = lib.afc_vc_issue_bound(_abi.ptr(one), 1)
+        one[-1] = col_bytes
+        return lib.afc_vc_issue_bound(_abi.ptr(one), 1) + (n - 1) * fixed if n else 0
+
+    def issue_dev(self, d_key_index, d_cols, d_col_off, d_duration, d_payloads, d_payload_off, d_payload_nil, n, hash_data=True, log=None,
+                  stream=None, d_expanded=None):
+        """afc_vc_issue_execution_batch_dev: n GenerateExecutionVC requests on the device.  d_key_index: int32 [n] into this cache (or
+        into d_expanded, K x 96); d_cols / d_col_off: uint8 columns and int64 [n*14+1] absolute offsets (_abi.ISSUE_COLUMNS order);
+        d_duration: int64 [n]; d_payloads / d_payload_off (int64 [2n+1]) / d_payload_nil (uint8 [2n]): input i then output i, read only
+        with hash_data; log: an audit.Auditor that receives the stored documents.  Returns (d_docs uint8, d_doc_off int64 [n+1],
+        d_hashes uint8 [n, 86] or None, d_proof_values uint8 [n, 86])."""
+        import torch
+        dev = d_col_off.device
+        if d_expanded is None:
+            d_expanded = torch.from_numpy(self._expanded).to(dev)
+        ncols = len(_abi.ISSUE_COLUMNS)
+        col_bytes = int(d_col_off[n * ncols]) - int(d_col_off[0]) if n else 0
+        cap = self._issue_bound(n, col_bytes)
+        d_docs = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        d_doc_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_hashes = torch.empty((n, 86), dtype=torch.uint8, device=dev) if hash_data else None
+        d_pv = torch.empty((n, 86), dtype=torch.uint8, device=dev)
+        lib = _abi.load()
+        _abi.check(lib.afc_vc_issue_execution_batch_dev(self.ctx.handle, _abi.ptr(d_expanded), d_expanded.shape[0], _abi.ptr(d_key_index),
+                                                        _abi.ptr(d_cols), _abi.ptr(d_col_off), _abi.ptr(d_duration), _abi.ptr(d_payloads),
+                                                        _abi.ptr(d_payload_off), _abi.ptr(d_payload_nil), _abi.ISSUE_HASH_DATA if hash_data else 0, n,
+                                                        log.handle if log is not None else None, _abi.ptr(d_docs), cap, _abi.ptr(d_doc_off),
+                                                        _abi.ptr(d_hashes), _abi.ptr(d_pv), self.ctx._stream(stream)), self.ctx.handle)
+        total = int(d_doc_off[n]) if n else 0
+        return d_docs[:total], d_doc_off, d_hashes, d_pv
+
+    def issue_packed(self, key_index, cols, col_off, duration, payloads, payload_off, payload_nil, hash_data=True, log=None, expanded=None):
+        """afc_vc_issue_execution_batch on host arrays (the layout of issue_dev).  Returns (docs uint8, doc_off uint64 [n+1], hashes
+        uint8 [n, 86] or None, proof_values uint8 [n, 86])."""
+        n = len(key_index)
+        exp = self._expanded if expanded is None else expanded
+        cap = _abi.load().afc_vc_issue_bound(_abi.ptr(col_off), n)
+        docs = np.empty(max(cap, 1), dtype=np.uint8)
+        doc_off = np.zeros(n + 1, dtype=np.uint64)
+        hashes = np.empty((n, 86), dtype=np.uint8) if hash_data else None
+        pv = np.empty((n, 86), dtype=np.uint8)
+        _abi.check(_abi.load().afc_vc_issue_execution_batch(self.ctx.handle, _abi.ptr(exp), exp.shape[0], _abi.ptr(key_index), _abi.ptr(cols),
+                                                            _abi.ptr(col_off), _abi.ptr(duration), _abi.ptr(payloads), _abi.ptr(payload_off),
+                                                            _abi.ptr(payload_nil), _abi.ISSUE_HASH_DATA if hash_data else 0, n,
+                                                            log.handle if log is not None else None, _abi.ptr(docs), cap, _abi.ptr(doc_off),
+                                                            _abi.ptr(hashes), _abi.ptr(pv)), self.ctx.handle)
+        return docs[:int(doc_off[n])], doc_off, hashes, pv
+
+    @staticmethod
+    def pack_issue_requests(requests):
+        """GenerateExecutionVC requests (the dicts of services.VCService.generate_execution_vc_batch) -> (cols, col_off, duration, payloads,
+        payload_off, payload_nil) host arrays.  Strings are UTF-8 with lone surrogates kept as their three bytes; bytes pass as they are."""
+        defaults = {"caller_type": "agent", "target_did": "", "function_name": "", "error_message": ""}
+
+        def col(r, k):
+            v = r.get(k) if k in defaults else r[k]
+            v = defaults[k] if v is None else v
+            return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+        flat = [col(r, k) for r in requests for k in _abi.ISSUE_COLUMNS]
+        cols, col_off = pack(flat)
+        duration = np.fromiter((int(r["duration_ms"]) for r in requests), dtype=np.int64, count=len(requests))
+        pl = [(r.get("input"), r.get("output")) for r in requests]
+        payloads, payload_off = pack([b"" if p is None else p for io in pl for p in io])
+        payload_nil = np.fromiter((p is None for io in pl for p in io), dtype=np.uint8, count=2 * len(requests))
+        return cols, col_off, duration, payloads, payload_off, payload_nil
+
+    def issue(self, requests, hash_data=True, log=None):
+        """GenerateExecutionVC for many requests in one host-buffer call: [{"vc_document": bytes, "signature": str, "input_hash": str,
+        "output_hash": str}]."""
+        n = len(requests)
+        if n == 0:
+            return []
+        ki = self.key_index([r["caller_did"] for r in requests])
+        docs, off, hashes, pv = self.issue_packed(ki, *self.pack_issue_requests(requests), hash_data=hash_data, log=log)
+        buf = docs.tobytes()
+        out = []
+        for i in range(n):
+            ih, oh = (hashes[i, :43].tobytes().decode(), hashes[i, 43:].tobytes().decode()) if hash_data else ("", "")
+            out.append({"vc_document": buf[int(off[i]):int(off[i + 1])], "signature": pv[i].tobytes().decode(), "input_hash": ih, "output_hash": oh})
+        return out
+
 
 class KeySet:
     """afc_keyset: issuer public keys with device-resident verification tables (384 KB per key).  With `dids` (one per key) the

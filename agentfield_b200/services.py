@@ -13,7 +13,7 @@
 Same names (snake_cased) and behaviour; each takes a BATCH (the natural seam is the loop in
 VerifyWorkflowVCComprehensive, vc_service.go:1442-1512, or a linger queue in front of one-per-request calls) and does
 every hash / signature on the GPU through the C ABI.  The canonical JSON bytes come from go_json.py on the host or, with
-canonical_on_device=True, from the device template (canonical.py): values -> documents -> signatures without a host round trip.
+canonical_on_device=True, from the device: GenerateExecutionVC's hashes, documents and signatures in one call (afc_vc_issue_execution_batch).
 """
 import base64
 import json
@@ -106,7 +106,6 @@ class VCService:
         self.store = store                                        # vc_store.ExecutionVCStore: the issued batch is persisted in ONE transaction
         self.hash_sensitive_data = hash_sensitive_data
         self.canonical_on_device = canonical_on_device
-        self._templates = None
         self._keyset = None
         self._keyset_dids = None
 
@@ -117,13 +116,19 @@ class VCService:
         return [_b64url(d) for d in Hasher(self.ctx).sha256_batch(datas)]
 
     # -- E1 / D1
-    def generate_execution_vc_batch(self, requests):
+    def generate_execution_vc_batch(self, requests, log=None):
         """requests: dicts with execution_id, workflow_id, session_id, caller_did, target_did, agent_node_did, caller_type,
         function_name, input (bytes|None), output (bytes|None), status, error_message (str|None), duration_ms, timestamp,
-        vc_id, issuance_date, proof_created.  Returns [{"vc_document": bytes, "signature": str, "input_hash", "output_hash"}]."""
+        vc_id, issuance_date, proof_created.  Returns [{"vc_document": bytes, "signature": str, "input_hash", "output_hash"}].
+        With canonical_on_device the hashes, documents and signatures come from one device call (ExpandedKeys.issue).  log: an
+        audit.Auditor that receives the stored documents, in batch order."""
         n = len(requests)
-        hashes = self.hash_data_batch([marshal_data_or_null(r.get("input")) for r in requests] +
-                                      [marshal_data_or_null(r.get("output")) for r in requests])
+        issued = self.keys.issue(requests, self.hash_sensitive_data, log) if self.canonical_on_device and n else None
+        if issued is None:
+            hashes = self.hash_data_batch([marshal_data_or_null(r.get("input")) for r in requests] +
+                                          [marshal_data_or_null(r.get("output")) for r in requests])
+        else:
+            hashes = [v["input_hash"] for v in issued] + [v["output_hash"] for v in issued]
         docs, msgs = [], []
         for i, r in enumerate(requests):
             ih, oh = hashes[i], hashes[n + i]
@@ -142,27 +147,20 @@ class VCService:
                 },
             }
             docs.append(doc)
-            if not self.canonical_on_device:
+            if issued is None:
                 msgs.append(go_json.vc_document(doc))                                    # zero-valued proof: what signVC signs
-        dids = [r["caller_did"] for r in requests]
-        if self.canonical_on_device and n:
-            import torch
-            from . import canonical
-            if self._templates is None:
-                self._templates = (canonical.vc_document_template(False, self.ctx), canonical.vc_document_template(True, self.ctx))
-            t0, t1 = self._templates
-            dev = torch.device("cuda", self.ctx.device)
-            fields, off = t0.pack_values([canonical.vc_document_values(d) for d in docs])
-            d_msgs, d_off = t0.fill_dev(torch.from_numpy(fields).to(dev), torch.from_numpy(off.view(np.int64)).to(dev), n)
-            sigs = self.keys.sign_dev(dids, d_msgs, d_off, n)                            # documents never leave the device
+        if issued is None:
+            pvs = [_b64url(sig) for sig in self.keys.sign_batch([r["caller_did"] for r in requests], msgs)]      # one GPU batch
         else:
-            sigs = self.keys.sign_batch(dids, msgs)                                      # one GPU batch
+            pvs = [v["signature"] for v in issued]
         proofs = [{"type": "Ed25519Signature2020", "created": r["proof_created"], "verificationMethod": "%s#key-1" % r["caller_did"],
-                   "proofPurpose": "assertionMethod", "proofValue": _b64url(sig)} for r, sig in zip(requests, sigs)]
-        if self.canonical_on_device and n:
-            stored = self._templates[1].fill([canonical.vc_document_values(d, p) for d, p in zip(docs, proofs)])
-        else:
+                   "proofPurpose": "assertionMethod", "proofValue": pv} for r, pv in zip(requests, pvs)]
+        if issued is None:
             stored = [go_json.vc_document(d, p) for d, p in zip(docs, proofs)]
+            if log is not None and stored:
+                log.append(stored)
+        else:
+            stored = [v["vc_document"] for v in issued]
         out = []
         for doc, proof, vc_bytes in zip(docs, proofs, stored):
             out.append({"vc_document": vc_bytes, "signature": proof["proofValue"],

@@ -300,6 +300,45 @@ int afc_merkle_load(afc_merkle* m, const uint8_t* state);
 int afc_merkle_leaf_hashes_dev(afc_ctx* ctx, const uint8_t* d_leaves, const uint64_t* d_leaf_off, uint32_t n,
                                uint8_t* d_out32, void* stream);
 
+/* ---- E1: issuing execution credentials in one call: GenerateExecutionVC (internal/services/vc_service.go:138-239) for n requests.
+ * For request i the call writes exactly what the reference computes and stores:
+ *   docs[doc_off[i] .. doc_off[i+1])   the stored vc_document: json.Marshal(createVCDocument(...)) with the signed proof
+ *   proof_values[86 i .. 86 i + 86)     the signature (proofValue, base64url without padding)
+ *   hashes[86 i .. 86 i + 43), [86 i + 43 .. 86 i + 86)   input_hash and output_hash (hashData: SHA-256 of json.Marshal([]byte),
+ *                                       base64url without padding), with AFC_ISSUE_HASH_DATA only (without it both are "")
+ * and, with a log, appends the n stored documents (leaf = document bytes) in order, through afc_merkle_append_dev on the call's stream.
+ * Inputs:
+ *   expanded96 / n_keys / key_index   the issuers' expanded keys (afc_ed25519_expand_batch) and each request's key; signing is constant
+ *                                     time unless afc_sign_configure says otherwise
+ *   cols / col_off                    AFC_ISSUE_COLUMNS byte strings per request, in the order below (column k of request i =
+ *                                     cols[col_off[14 i + k] .. col_off[14 i + k + 1]), n * 14 + 1 absolute offsets).  The VC id,
+ *                                     issuanceDate, the proof's created and timestamp are the caller's (the reference reads a clock or
+ *                                     makes up an id); error_message is the untruncated message ("" = none)
+ *   duration_ms                       n Go ints
+ *   payloads / payload_off / payload_nil   2n payloads, input i then output i (payload_off: 2n + 1 absolute offsets; payload_nil[j] != 0
+ *                                     for a nil []byte, which hashes as null); read with AFC_ISSUE_HASH_DATA only
+ * docs_cap must be at least afc_vc_issue_bound(col_off, n), a bound computed from col_off[0] and col_off[14 n] alone and additive over
+ * requests (else AFC_EINVAL, before any work), so a call never fails half-way for lack of room.  Other AFC_EINVAL: a NULL pointer, hashes NULL with
+ * AFC_ISSUE_HASH_DATA, unknown flags, n_keys == 0, a log of another context; in the host-buffer call also key_index[i] >= n_keys and
+ * offsets that run backwards.  The _dev call cannot inspect its index array without a sync: an index >= n_keys signs with key 0.
+ * The host-buffer call streams chunks through the context's staging ring and writes every document at its final offset; the expanded
+ * keys it stages are wiped from the device when it returns.  The _dev call synchronises `stream` once, to read the two ends of
+ * col_off; expanded96 must be 16-byte aligned.  n = 0 writes doc_off[0] = 0 in the host-buffer call and nothing in the _dev call. */
+#define AFC_ISSUE_COLUMNS 14  /* vc_id, caller_did, issuance_date, execution_id, workflow_id, session_id, caller_type,
+                                 agent_node_did, target_did, function_name, timestamp, status, error_message, proof_created */
+#define AFC_ISSUE_HASH_DATA 1 /* flags: VCRequirements.HashSensitiveData */
+uint64_t afc_vc_issue_bound(const uint64_t* col_off, uint32_t n);
+int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                 const uint64_t* col_off /* n*14+1 */, const int64_t* duration_ms, const uint8_t* payloads,
+                                 const uint64_t* payload_off /* 2n+1 */, const uint8_t* payload_nil /* 2n */, uint32_t flags, uint32_t n,
+                                 afc_merkle* log /* NULL: no append */, uint8_t* docs, uint64_t docs_cap, uint64_t* doc_off /* n+1 */,
+                                 uint8_t* hashes /* n x 2 x 43 */, uint8_t* proof_values /* n x 86 */);
+int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                     const uint64_t* d_col_off, const int64_t* d_duration_ms, const uint8_t* d_payloads,
+                                     const uint64_t* d_payload_off, const uint8_t* d_payload_nil, uint32_t flags, uint32_t n, afc_merkle* log,
+                                     uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off, uint8_t* d_hashes, uint8_t* d_proof_values,
+                                     void* stream);
+
 /* ---- N4: audit proofs for bulk offline verification (`af vc verify`, internal/cli/vc.go:159-331; export bundles,
  * internal/handlers/ui/did.go:533-865) ------------------------------------------------------------------------
  * afc_merkle_tree materialises every level over a fixed set of leaf hashes (device memory, ~2n x 32 B) so that RFC 6962

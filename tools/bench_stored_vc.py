@@ -4,9 +4,10 @@ Prints one JSON line: documents/s of the device-pointer call with its per-kernel
 signing bytes already rendered, and of the host-buffer call; host_fallback and all_expected; the card and its power limit, read
 in the same run.  The audit_stored block does the same for the audit of stored execution VCs against their records
 (afc_vc_audit_stored_batch[_dev]), next to the stored-verify device call on the same documents.  The verify_json block measures
-documents in three client spellings (afc_vc_verify_json_batch_dev) next to the stored-verify call on the canonical form.  Needs a
+documents in three client spellings (afc_vc_verify_json_batch_dev) next to the stored-verify call on the canonical form.  The
+issue_execution block measures execution credentials issued in one call (afc_vc_issue_execution_batch[_dev]).  Needs a
 CUDA device; writes nothing.
-usage: python tools/bench_stored_vc.py [--reps R]"""
+usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
 import json
 import os
@@ -174,12 +175,173 @@ def verify_json_block(ctx, dev, timed):
     return out
 
 
+def issue_execution_block(ctx, dev, timed):
+    """Execution credentials issued on the device (afc_vc_issue_execution_batch): 2^20 requests from 1024 issuers (55-character DIDs,
+    RFC 3339 times), input and output payloads of 64-2048 B (uniform, seeded; 10 % nil), 1 % with an error message that needs escaping
+    (a third of those past 500 bytes), constant-time signing.  Next to it, the same device work done the way the service did it before:
+    SHA-256 over the pre-encoded payload text, the template fill without proof, expanded-key signing, base64url, the fill with proof.
+    Also the host-buffer call (2^18 requests, pinned buffers), the _dev call appending to a log, and a tail variant where 0.1 % of the
+    payloads are 256 KiB.  Every hash and every signature is checked (hashlib; afc_vc_verify_stored_batch), and 2000 sampled documents
+    byte for byte against the host mirror, before timing."""
+    import base64
+    import hashlib
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import canonical as CA, go_json, services
+    from agentfield_b200.identity import KeySet
+    n, K = 1 << 20, 1024
+    rng = np.random.default_rng(0xAF1E)
+    cache = afb.ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (8000 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    t = lambda a: torch.from_numpy(a).to(dev)
+
+    def upload(reqs):
+        cols, coff, dur, pay, poff, nil = cache.pack_issue_requests(reqs)
+        ki = cache.key_index([r["caller_did"] for r in reqs])
+        return dict(d_key_index=t(ki.view(np.int32)), d_cols=t(cols), d_col_off=t(coff.view(np.int64)), d_duration=t(dur), d_payloads=t(pay),
+                    d_payload_off=t(poff.view(np.int64)), d_payload_nil=t(nil), n=len(reqs), d_expanded=d_exp), (cols, coff, dur, pay, poff, nil, ki)
+    reqs = CA.synthetic_issue_requests(dids, n, seed=0xAF1E)
+    D, H = upload(reqs)
+    pay_bytes = int(H[4][-1])
+    d_docs, d_off, d_h, d_pv = cache.issue_dev(**D)
+    torch.cuda.synchronize()
+    # checks: every hash (hashlib), every document (verify), 2000 documents byte for byte (host mirror)
+    h = d_h.cpu().numpy()
+    hashes_ok = True
+    for i, r in enumerate(reqs):
+        for k, d in ((0, r["input"]), (1, r["output"])):
+            m = services.marshal_data_or_null(None if d is None else bytes(d))
+            hashes_ok &= h[i, 43 * k:43 * k + 43].tobytes() == base64.urlsafe_b64encode(hashlib.sha256(m).digest()).rstrip(b"=")
+    ks = KeySet([cache.public_key(d) for d in dids], ctx, dids=dids)
+    d_st = torch.empty(n, dtype=torch.uint8, device=dev)
+    ks.verify_stored_dev(0, d_docs, d_off, n, d_st)
+    verify_ok = bool((d_st == 1).all())
+    ks.close()
+    docs_host, off_host, pv = d_docs.cpu().numpy().tobytes(), d_off.cpu().numpy(), d_pv.cpu().numpy()
+    sample = rng.choice(n, 2000, replace=False)
+    svc = services.VCService(cache, canonical_on_device=False)
+    mirror = svc.generate_execution_vc_batch([reqs[int(i)] for i in sample])
+    sample_ok = all(m["vc_document"] == docs_host[int(off_host[i]):int(off_host[i + 1])] and m["signature"] == pv[i].tobytes().decode()
+                    for m, i in zip(mirror, sample))
+    all_expected = bool(hashes_ok and verify_ok and sample_ok)
+    run = lambda: cache.issue_dev(**D)
+    ms_dev = timed(run)
+    ctx.profile_begin()
+    timed(run, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    total_bytes = int(off_host[-1])
+    # the same device work the way the service did it before: hash pre-encoded text, fill, sign, base64url, fill again
+    text = [services.marshal_data_or_null(None if r[k] is None else bytes(r[k])) for r in reqs for k in ("input", "output")]
+    tbuf, toff = afb.crypto.pack(text)
+    del text
+    d_tbuf, d_toff = t(tbuf), t(toff.view(np.int64))
+    d_dig = torch.empty((2 * n, 32), dtype=torch.uint8, device=dev)
+    t0, t1 = CA.vc_document_template(False, ctx), CA.vc_document_template(True, ctx)
+    ctxlist, typelist = go_json.string_list(["https://www.w3.org/2018/credentials/v1", "https://agentfield.example.com/contexts/execution/v1"]).encode(), \
+        go_json.string_list(["VerifiableCredential", "AgentFieldExecutionCredential"]).encode()
+    md = b'{"agentfield_version":"1.0.0","vc_version":"1.0"}'
+    u = lambda s: s.encode("utf-8", "surrogatepass")
+    v0, v1 = [], []
+    for i, r in enumerate(reqs):
+        ih, oh = h[i, :43].tobytes(), h[i, 43:].tobytes()
+        em = go_json.truncate_error_message(r["error_message"])
+        row = [ctxlist, typelist, b"urn:agentfield:vc:" + u(r["vc_id"]), u(r["caller_did"]), u(r["issuance_date"]), u(r["execution_id"]),
+               u(r["workflow_id"]), u(r["session_id"]), u(r["caller_did"]), u(r["caller_type"]), u(r["agent_node_did"]), u(r["target_did"]),
+               u(r["agent_node_did"]), u(r["function_name"]), ih, oh, u(r["timestamp"]), b"%d" % r["duration_ms"], u(r["status"]),
+               (b',"errorMessage":' + go_json.any_string(em).encode("utf-8")) if em else b"", ih, oh, md]
+        v0.append(row)
+        v1.append(row + [b"Ed25519Signature2020", u(r["proof_created"]), u(r["caller_did"]) + b"#key-1", b"assertionMethod", pv[i].tobytes()])
+    f0, o0 = t0.pack_values(v0)
+    f1, o1 = t1.pack_values(v1)
+    del v0, v1
+    d_f0, d_o0, d_f1, d_o1 = t(f0), t(o0.view(np.int64)), t(f1), t(o1.view(np.int64))
+    d_sigs = torch.empty((n, 64), dtype=torch.uint8, device=dev)
+    d_pv2 = torch.empty((n, 86), dtype=torch.uint8, device=dev)
+    ms_sha = timed(lambda: ctx.sha256_dev(d_tbuf, d_toff, 2 * n, d_dig))
+    ms_fill0 = timed(lambda: t0.fill_dev(d_f0, d_o0, n))
+    d_msgs, d_moff = t0.fill_dev(d_f0, d_o0, n)
+    ms_sign = timed(lambda: ctx.sign_expanded_dev(d_exp, D["d_key_index"], d_msgs, d_moff, n, d_sigs))
+    ms_b64 = timed(lambda: ctx.b64url_encode_dev(d_sigs, 64, n, d_pv2))
+    ms_fill1 = timed(lambda: t1.fill_dev(d_f1, d_o1, n))
+    d_docs1, _ = t1.fill_dev(d_f1, d_o1, n)
+    pieces_same = bool(torch.equal(d_pv2, d_pv)) and bool(torch.equal(d_docs1, d_docs))
+    del d_tbuf, d_toff, d_dig, d_f0, d_o0, d_f1, d_o1, d_msgs, d_moff, d_docs1, tbuf, f0, f1
+    # the _dev call appending to a log
+    aud = afb.Auditor(ctx)
+    ms_log = timed(lambda: cache.issue_dev(**D, log=aud))
+    aud.close()
+    del d_docs, d_off, d_h, d_pv
+    # the host-buffer call, pinned buffers, 2^18 requests
+    nh = 1 << 18
+    cols, coff, dur, pay, poff, nil, ki = H
+    cut_c, cut_p = int(coff[nh * 14]), int(poff[2 * nh])
+
+    def pin(a):
+        p = torch.empty(a.shape, dtype=torch.from_numpy(a[:0]).dtype, pin_memory=True).numpy()
+        p[...] = a
+        return p
+    hin = [pin(cols[:cut_c]), pin(coff[:nh * 14 + 1]), pin(dur[:nh]), pin(pay[:cut_p]), pin(poff[:2 * nh + 1]), pin(nil[:2 * nh])]
+    lib, P = afb._abi.load(), afb._abi.ptr
+    cap = lib.afc_vc_issue_bound(P(hin[1]), nh)
+    hdocs = torch.empty(cap, dtype=torch.uint8, pin_memory=True).numpy()
+    hoff = torch.empty(nh + 1, dtype=torch.int64, pin_memory=True).numpy()
+    hh = torch.empty((nh, 86), dtype=torch.uint8, pin_memory=True).numpy()
+    hpv = torch.empty((nh, 86), dtype=torch.uint8, pin_memory=True).numpy()
+    hki = pin(ki[:nh])
+
+    def host_call():
+        afb._abi.check(lib.afc_vc_issue_execution_batch(ctx.handle, P(cache._expanded), K, P(hki), P(hin[0]), P(hin[1]), P(hin[2]), P(hin[3]),
+                                                        P(hin[4]), P(hin[5]), afb._abi.ISSUE_HASH_DATA, nh, None, P(hdocs), cap, P(hoff), P(hh),
+                                                        P(hpv)), ctx.handle)
+    host_call()
+    host_same = hoff[nh] == off_host[nh] and hdocs[:hoff[nh]].tobytes() == docs_host[:int(off_host[nh])] and (hpv == pv[:nh]).all() and \
+        (hh == h[:nh]).all()
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        host_call()
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    del hin, hdocs, hoff, hh, hpv, hki, H, D
+    torch.cuda.empty_cache()
+    # tail: 0.1 % of the payloads are 256 KiB
+    treqs = CA.synthetic_issue_requests(dids, n, seed=0xAF1F, long_frac=0.001)
+    TD, _ = upload(treqs)
+    long_n = sum((r["input"] is not None and len(r["input"]) == 256 << 10) + (r["output"] is not None and len(r["output"]) == 256 << 10) for r in treqs)
+    d_docs, d_off, d_h, d_pv = cache.issue_dev(**TD)
+    torch.cuda.synchronize()
+    th = d_h.cpu().numpy()
+    tail_ok = True
+    for i in range(0, n, 97):
+        r = treqs[i]
+        for k, d in ((0, r["input"]), (1, r["output"])):
+            m = services.marshal_data_or_null(None if d is None else bytes(d))
+            tail_ok &= th[i, 43 * k:43 * k + 43].tobytes() == base64.urlsafe_b64encode(hashlib.sha256(m).digest()).rstrip(b"=")
+    del d_docs, d_off, d_h, d_pv
+    ms_tail = timed(lambda: cache.issue_dev(**TD))
+    ctx.profile_begin()
+    timed(lambda: cache.issue_dev(**TD), reps=3)
+    tkms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    old = ms_sha + ms_fill0 + ms_sign + ms_b64 + ms_fill1
+    return {"requests": n, "issuers": K, "payload_bytes": pay_bytes, "doc_bytes": total_bytes, "gpu": gpu,
+            "all_expected": all_expected, "hashes_ok": bool(hashes_ok), "verify_ok": verify_ok, "sample_ok": bool(sample_ok),
+            "dev_call": {"vcs_per_s": n / (ms_dev * 1e-3), "ms": ms_dev, "kernels_ms": kms},
+            "pieces": {"ms": old, "vcs_per_s": n / (old * 1e-3), "sha256_ms": ms_sha, "fill_ms": ms_fill0, "sign_ms": ms_sign, "b64url_ms": ms_b64,
+                       "fill_proof_ms": ms_fill1, "same_bytes": pieces_same,
+                       "note": "afc_sha256_batch_dev over pre-encoded text, two template fills, expanded-key signing, base64url; host work not counted"},
+            "dev_call_with_log": {"vcs_per_s": n / (ms_log * 1e-3), "ms": ms_log},
+            "host_call": {"requests": nh, "vcs_per_s": nh / (ms_host * 1e-3), "ms": ms_host, "same_as_dev": bool(host_same),
+                          "note": "every buffer pinned"},
+            "tail": {"long_payloads": int(long_n), "vcs_per_s": n / (ms_tail * 1e-3), "ms": ms_tail, "kernels_ms": tkms, "hashes_ok": bool(tail_ok)}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json"], default=None, help="run one block")
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution"], default=None, help="run one block")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     ctx = afb.Context(0)
@@ -192,7 +354,8 @@ def main():
             fn()
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
-    blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block}
+    blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
+              "issue_execution": issue_execution_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
