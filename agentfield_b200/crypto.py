@@ -140,6 +140,19 @@ class Context:
                                                    _abi.ptr(out)), self.handle)
         return out
 
+    def webhook_sign_packed(self, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off):
+        """afc_webhook_sign_batch over packed inputs (include/afcrypto.h) -> (bodies, body_off, headers n x 71, status)."""
+        n = len(result_off) - 1
+        cap = int(self._lib.afc_webhook_bound(_abi.ptr(col_off), _abi.ptr(result_off), n))
+        bodies = np.empty(max(cap, 1), dtype=np.uint8)
+        body_off = np.zeros(n + 1, dtype=np.uint64)
+        headers = np.zeros((n, _abi.WEBHOOK_HEADER_CHARS), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.uint8)
+        _abi.check(self._lib.afc_webhook_sign_batch(self.handle, _abi.ptr(cols), _abi.ptr(col_off), _abi.ptr(duration_ms), _abi.ptr(flags),
+                                                    _abi.ptr(results), _abi.ptr(result_off), _abi.ptr(secrets), _abi.ptr(secret_off), n,
+                                                    _abi.ptr(bodies), cap, _abi.ptr(body_off), _abi.ptr(headers), _abi.ptr(status)), self.handle)
+        return bodies[:int(body_off[-1])], body_off, headers, status
+
     def verify_packed(self, pks, sigs, buf, off, out=None):
         n = len(off) - 1
         if out is None:
@@ -191,6 +204,13 @@ class Context:
     def hmac_sha256_dev(self, d_keys, d_koff, d_msgs, d_off, n, d_out, stream=None):
         _abi.check(self._lib.afc_hmac_sha256_batch_dev(self.handle, _abi.ptr(d_keys), _abi.ptr(d_koff), _abi.ptr(d_msgs), _abi.ptr(d_off), n,
                                                        _abi.ptr(d_out), self._stream(stream)), self.handle)
+
+    def webhook_sign_dev(self, d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies, bodies_cap,
+                         d_body_off, d_headers, d_status, stream=None):
+        _abi.check(self._lib.afc_webhook_sign_batch_dev(self.handle, _abi.ptr(d_cols), _abi.ptr(d_col_off), _abi.ptr(d_duration_ms), _abi.ptr(d_flags),
+                                                        _abi.ptr(d_results), _abi.ptr(d_result_off), _abi.ptr(d_secrets), _abi.ptr(d_secret_off), n,
+                                                        _abi.ptr(d_bodies), int(bodies_cap), _abi.ptr(d_body_off), _abi.ptr(d_headers),
+                                                        _abi.ptr(d_status), self._stream(stream)), self.handle)
 
     def verify_dev(self, d_pks, d_sigs, d_msgs, d_off, n, d_ok, stream=None):
         _abi.check(self._lib.afc_ed25519_verify_batch_dev(self.handle, _abi.ptr(d_pks), _abi.ptr(d_sigs), _abi.ptr(d_msgs), _abi.ptr(d_off), n,

@@ -116,6 +116,20 @@ cudaError_t vci_fill(const uint8_t* cols, const uint64_t* col_off, const int64_t
 cudaError_t vci_proof(const uint8_t* sigs, uint32_t n, const uint64_t* doc_off, uint8_t* docs, uint8_t* proof_values, cudaStream_t s, LaunchLog* lg);
 uint64_t vci_literal_bytes();          // constant text of both document forms together
 
+// ---- k_webhook.cu: webhook deliveries built and signed on the device (afc_webhook.cuh).  col_off: 8 absolute offsets per delivery + 1;
+// result_off: n + 1 absolute offsets; tape: (result_off[n] - result_off[0]) / 2 + 1 entries; plan: n bytes kept between the passes
+// each body's length (0 for a WH_HOST delivery; write them to body_off + 1 for offsets_from_lengths) and its status
+cudaError_t wh_sizes(const uint8_t* cols, const uint64_t* col_off, const int64_t* duration, const uint8_t* flags, const uint8_t* results,
+                     const uint64_t* result_off, uint32_t n, uint32_t* tape, uint8_t* plan, uint64_t* body_len, uint8_t* status, cudaStream_t s,
+                     LaunchLog* lg);
+cudaError_t wh_emit(const uint8_t* cols, const uint64_t* col_off, const int64_t* duration, const uint8_t* flags, const uint8_t* results,
+                    const uint64_t* result_off, uint32_t n, uint32_t* tape, const uint8_t* plan, const uint64_t* body_off, uint8_t* bodies,
+                    cudaStream_t s, LaunchLog* lg);
+// secret_off: n + 1 absolute uint32 offsets; mac: n x 32 scratch -> n x 71 header characters
+cudaError_t wh_sign(const uint8_t* secrets, const uint32_t* secret_off, const uint8_t* flags, const uint8_t* status, const uint8_t* bodies,
+                    const uint64_t* body_off, uint32_t n, uint8_t* mac, uint8_t* headers, cudaStream_t s, LaunchLog* lg);
+uint64_t wh_fixed_bytes();             // the constant text a body can hold at most
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

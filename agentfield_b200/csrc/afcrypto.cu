@@ -1442,6 +1442,225 @@ int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32
     return rc;
 }
 
+// ---------------------------------------------------------------------------------- webhook deliveries
+// Bound from the byte counts alone: each delivery's constant text plus at most 6 bytes per column and result byte (a byte escaped as
+// backslash-u 00XX or fffd; a number token grows at most 21 / 4 times, 1e20 -> 100000000000000000000).
+static uint64_t wh_bound(uint32_t n, uint64_t bytes) { return (uint64_t)n * launch::wh_fixed_bytes() + 6 * bytes; }
+
+uint64_t afc_webhook_bound(const uint64_t* col_off, const uint64_t* result_off, uint32_t n) {
+    if (!col_off || !result_off || n == 0) return 0;
+    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_WEBHOOK_COLUMNS], c = result_off[0], d = result_off[n];
+    return wh_bound(n, (b >= a ? b - a : 0) + (d >= c ? d - c : 0));
+}
+
+// per-call device scratch: the result tapes, the plans, the HMACs, scan tiles
+struct WebhookScratch { uint32_t* tape; uint8_t* plan; uint8_t* mac; uint64_t* scan; };
+static size_t wh_scratch_bytes(uint32_t n, uint64_t result_bytes) {
+    return vc_align((result_bytes / 2 + 1) * 4) + vc_align(n) + vc_align((size_t)n * 32) + vc_align(launch::json_scan_scratch_bytes(n));
+}
+static WebhookScratch wh_scratch(uint8_t* p, uint32_t n, uint64_t result_bytes) {
+    WebhookScratch s;
+    s.tape = (uint32_t*)p; p += vc_align((result_bytes / 2 + 1) * 4);
+    s.plan = p; p += vc_align(n);
+    s.mac = p; p += vc_align((size_t)n * 32);
+    s.scan = (uint64_t*)p;
+    return s;
+}
+static cudaError_t wh_enqueue(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
+                              const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, uint64_t* body_off,
+                              uint8_t* headers, uint8_t* status, const WebhookScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = launch::wh_sizes(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off + 1, status, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(body_off, n, S.scan, st, lg);
+    if (e == cudaSuccess) e = launch::wh_emit(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off, bodies, st, lg);
+    if (e == cudaSuccess) e = launch::wh_sign(sec, sec_off, flags, status, bodies, body_off, n, S.mac, headers, st, lg);
+    return e;
+}
+static int wh_check(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
+                    const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, const uint8_t* bodies, const uint64_t* body_off,
+                    const uint8_t* headers, const uint8_t* status) {
+    if (!ctx || !col_off || !res_off || !sec_off || !body_off) return AFC_EINVAL;
+    if (n && (!cols || !dur || !flags || !bodies || !headers || !status)) return AFC_EINVAL;
+    return AFC_OK;
+}
+
+int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64_t* d_col_off, const int64_t* d_duration_ms, const uint8_t* d_flags,
+                               const uint8_t* d_results, const uint64_t* d_result_off, const uint8_t* d_secrets, const uint32_t* d_secret_off,
+                               uint32_t n, uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_headers, uint8_t* d_status,
+                               void* stream) {
+    int rc = wh_check(ctx, d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies, d_body_off,
+                      d_headers, d_status);
+    if (rc != AFC_OK || n == 0) return rc;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t ends[4];                       // the column and result bytes bound the bodies and size the tapes: one synchronisation
+    CK(cudaMemcpyAsync(&ends[0], d_col_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[1], d_col_off + (size_t)n * AFC_WEBHOOK_COLUMNS, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[2], d_result_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ends[3], d_result_off + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ends[1] < ends[0] || ends[3] < ends[2] || bodies_cap < wh_bound(n, (ends[1] - ends[0]) + (ends[3] - ends[2]))) return AFC_EINVAL;
+    if ((!d_results && ends[3] != ends[2]) || !d_secrets) return AFC_EINVAL;
+    const uint64_t rb = ends[3] - ends[2];
+    CallLog lc(ctx);
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, wh_scratch_bytes(n, rb), st));
+    cudaError_t e = wh_enqueue(d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies, d_body_off,
+                               d_headers, d_status, wh_scratch(scratch, n, rb), st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+// The host-buffer call: chunks of deliveries through the lane's ring, as issue_host_run does.  A chunk's stream is synchronised once
+// after the sizes pass to learn where its bodies end.  Staged secrets are wiped from the device slot after each chunk's headers and
+// from the pinned bounce buffer once the chunk is drained (or the call returns early).
+static int wh_host_run(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
+                       const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, uint64_t* body_off,
+                       uint8_t* headers, uint8_t* status) {
+    const uint32_t C = AFC_WEBHOOK_COLUMNS;
+    LaneGuard lg(ctx);
+    Lane& lane = lg.lane();
+    struct SecretBounce { uint8_t* p = nullptr; size_t bytes = 0; } bounce_sec[kSlots];
+    struct WipeOnExit {                     // runs after LaneDrain (declared before it): no copy still reads the bounce buffers
+        SecretBounce* b;
+        ~WipeOnExit() { for (int w = 0; w < kSlots; w++) if (b[w].bytes) memset(b[w].p, 0, b[w].bytes); }
+    } wipe{bounce_sec};
+    LaneDrain drain_on_exit(lane);
+    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_dur = is_pinned(dur), pin_fl = is_pinned(flags);
+    const bool pin_res = is_pinned(res), pin_roff = is_pinned(res_off), pin_sec = is_pinned(sec), pin_soff = is_pinned(sec_off);
+    const bool pin_bodies = is_pinned(bodies), pin_h = is_pinned(headers), pin_st = is_pinned(status);
+    CallLog lc(ctx);
+    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
+    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
+    auto drain = [&](int w) -> int {
+        Pending& p = pend[w];
+        if (!p.active) return AFC_OK;
+        Slot& sl = lane.slot[w];
+        CK(cudaStreamSynchronize(sl.stream));
+        if (bounce_sec[w].bytes) { memset(bounce_sec[w].p, 0, bounce_sec[w].bytes); bounce_sec[w].bytes = 0; }
+        const uint8_t* h = sl.h_out.p;
+        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
+        for (uint32_t j = 0; j < p.cnt; j++) body_off[p.i0 + j] = p.base + rel[j];
+        if (!pin_h) { memcpy(headers + (size_t)p.i0 * 71, h, (size_t)p.cnt * 71); h += vc_align((size_t)p.cnt * 71); }
+        if (!pin_st) { memcpy(status + p.i0, h, p.cnt); h += vc_align(p.cnt); }
+        if (!pin_bodies) memcpy(bodies + p.base, h, p.bytes);
+        p.active = false;
+        return AFC_OK;
+    };
+    uint32_t i0 = 0;
+    uint64_t base = 0;
+    int which = 0;
+    while (i0 < n) {
+        const uint32_t left = n - i0;
+        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
+        if (limit < min_chunk) limit = min_chunk;
+        if (limit > max_chunk) limit = max_chunk;
+        uint32_t i1 = i0;
+        const uint64_t cbase = col_off[(size_t)i0 * C], rbase = res_off[i0];
+        while (i1 < n && i1 - i0 < limit) {
+            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (res_off[i1 + 1] - rbase);
+            if (bytes > kChunkBytes && i1 != i0) break;
+            i1++;
+        }
+        const uint32_t cnt = i1 - i0;
+        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, rbytes = res_off[i1] - rbase;
+        const uint64_t kbase = sec_off[i0], kbytes = sec_off[i1] - kbase;
+        Slot& sl = lane.slot[which];
+        int rc = drain(which);
+        if (rc != AFC_OK) return rc;
+        const uint64_t bbound = wh_bound(cnt, cbytes + rbytes);
+        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 8, (size_t)cnt, rbytes + 32, ((size_t)cnt + 1) * 8,
+                             kbytes + 32, ((size_t)cnt + 1) * 4, bbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 71, (size_t)cnt,
+                             wh_scratch_bytes(cnt, rbytes)};
+        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
+        size_t total = 0;
+        for (size_t b : sz) total += vc_align(b);
+        CK(sl.vc.reserve(total));
+        uint8_t* q[NB];
+        {
+            uint8_t* p = sl.vc.p;
+            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
+        }
+        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_dur ? 0 : (size_t)cnt * 8, pin_fl ? 0 : (size_t)cnt,
+                                   pin_res ? 0 : rbytes, pin_roff ? 0 : ((size_t)cnt + 1) * 8, pin_sec ? 0 : kbytes, pin_soff ? 0 : ((size_t)cnt + 1) * 4};
+        size_t bounce = 0;
+        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
+        CK(sl.h_in.reserve(bounce + 256, ctx));
+        CK(sl.h_out2.reserve(8, ctx));
+        size_t used = 0;
+        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
+        const uint64_t* d_coff = (const uint64_t*)q[1];
+        const int64_t* d_dur = (const int64_t*)q[2];
+        const uint8_t* d_fl = q[3];
+        uint8_t* d_res = q[4] + (rbase & 15) - rbase;
+        const uint64_t* d_roff = (const uint64_t*)q[5];
+        uint8_t* d_sec = q[6] + (kbase & 3) - kbase;
+        const uint32_t* d_soff = (const uint32_t*)q[7];
+        uint8_t* d_bodies = q[8];
+        uint64_t* d_boff = (uint64_t*)q[9];
+        uint8_t* d_h = q[10];
+        uint8_t* d_st = q[11];
+        const WebhookScratch S = wh_scratch(q[12], cnt, rbytes);
+        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
+        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
+        CK(h2d(sl, q[2], dur + i0, (size_t)cnt * 8, pin_dur, &used));
+        CK(h2d(sl, q[3], flags + i0, cnt, pin_fl, &used));
+        CK(h2d(sl, q[4] + (rbase & 15), res + rbase, rbytes, pin_res, &used));
+        CK(h2d(sl, q[5], res_off + i0, ((size_t)cnt + 1) * 8, pin_roff, &used));
+        if (!pin_sec && kbytes) bounce_sec[which] = {sl.h_in.p + used, (size_t)kbytes};
+        CK(h2d(sl, q[6] + (kbase & 3), sec + kbase, kbytes, pin_sec, &used));
+        CK(h2d(sl, q[7], sec_off + i0, ((size_t)cnt + 1) * 4, pin_soff, &used));
+        CK(launch::wh_sizes(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff + 1, d_st, sl.stream, lc));
+        CK(launch::offsets_from_lengths(d_boff, cnt, S.scan, sl.stream, lc));
+        CK(cudaMemcpyAsync(sl.h_out2.p, d_boff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
+        CK(cudaStreamSynchronize(sl.stream));
+        uint64_t bytes;
+        memcpy(&bytes, sl.h_out2.p, 8);
+        CK(launch::wh_emit(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff, d_bodies, sl.stream, lc));
+        CK(launch::wh_sign(d_sec, d_soff, d_fl, d_st, d_bodies, d_boff, cnt, S.mac, d_h, sl.stream, lc));
+        if (kbytes) CK(cudaMemsetAsync(q[6], 0, kbytes + 32, sl.stream));          // secrets do not stay behind in the staging slot
+        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_h ? 0 : vc_align((size_t)cnt * 71)) + (pin_st ? 0 : vc_align(cnt)) +
+                            (pin_bodies ? 0 : bytes) + 256, ctx));
+        uint8_t* h = sl.h_out.p;
+        CK(cudaMemcpyAsync(h, d_boff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
+        h += vc_align(((size_t)cnt + 1) * 8);
+        CK(cudaMemcpyAsync(pin_h ? headers + (size_t)i0 * 71 : h, d_h, (size_t)cnt * 71, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_h) h += vc_align((size_t)cnt * 71);
+        CK(cudaMemcpyAsync(pin_st ? status + i0 : h, d_st, cnt, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_st) h += vc_align(cnt);
+        if (bytes) CK(cudaMemcpyAsync(pin_bodies ? bodies + base : h, d_bodies, bytes, cudaMemcpyDeviceToHost, sl.stream));
+        pend[which] = {i0, cnt, base, bytes, true};
+        base += bytes;
+        which = (which + 1) % kSlots;
+        i0 = i1;
+    }
+    for (int w = 0; w < kSlots; w++) {      // oldest first
+        int rc = drain((which + w) % kSlots);
+        if (rc != AFC_OK) return rc;
+    }
+    drain_on_exit.armed = false;
+    body_off[n] = base;
+    return AFC_OK;
+}
+
+int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* duration_ms, const uint8_t* flags,
+                           const uint8_t* results, const uint64_t* result_off, const uint8_t* secrets, const uint32_t* secret_off, uint32_t n,
+                           uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off, uint8_t* headers, uint8_t* status) {
+    int rc = wh_check(ctx, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off, n, bodies, body_off, headers, status);
+    if (rc != AFC_OK) return rc;
+    if (n == 0) { body_off[0] = 0; return AFC_OK; }
+    uint64_t bad = 0;
+    for (size_t k = 0; k < (size_t)n * AFC_WEBHOOK_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
+    for (uint32_t i = 0; i < n; i++) {
+        bad |= (uint64_t)(result_off[i + 1] < result_off[i]) | (uint64_t)(secret_off[i + 1] < secret_off[i]);
+        bad |= (uint64_t)(flags[i] & ~(uint32_t)(AFC_WEBHOOK_HAS_DURATION | AFC_WEBHOOK_HAS_ERROR_MESSAGE | AFC_WEBHOOK_HAS_SECRET));
+    }
+    if (bad || bodies_cap < afc_webhook_bound(col_off, result_off, n)) return AFC_EINVAL;
+    if ((!results && result_off[n] != result_off[0]) || (!secrets && secret_off[n] != secret_off[0])) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    return wh_host_run(ctx, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off, n, bodies, body_off, headers, status);
+}
+
 // ---------------------------------------------------------------------------------- Merkle log
 int afc_merkle_new(afc_ctx* ctx, afc_merkle** out) {
     if (!ctx || !out) return AFC_EINVAL;

@@ -203,3 +203,94 @@ def webhook_payload(p) -> bytes:
         parts.append('"error_message":' + string(p["error_message"]))
     parts.append('"timestamp":' + string(p["timestamp"]))
     return ("{" + ",".join(parts) + "}").encode("utf-8")
+
+
+def go_utf8(raw: bytes) -> str:
+    """A Go string's bytes as Python text the way Go's decoder reads them: valid UTF-8 as itself, every byte utf8.DecodeRune rejects as
+    U+FFFD, one per byte."""
+    out, i = [], 0
+    while i < len(raw):
+        b = raw[i]
+        if b < 0x80:
+            out.append(chr(b)); i += 1
+            continue
+        n = 2 if 0xC2 <= b <= 0xDF else 3 if 0xE0 <= b <= 0xEF else 4 if 0xF0 <= b <= 0xF4 else 0
+        try:
+            if n == 0:
+                raise UnicodeDecodeError("utf-8", raw, i, i + 1, "lead")
+            out.append(raw[i:i + n].decode("utf-8")); i += n
+        except UnicodeDecodeError:
+            out.append("�"); i += 1
+    return "".join(out)
+
+
+def _no_surrogates(v):
+    """Lone surrogate escapes decode to U+FFFD in Go; a key that becomes equal to another one then overwrites it (last wins)."""
+    if isinstance(v, str):
+        return "".join("�" if 0xD800 <= ord(c) <= 0xDFFF else c for c in v)
+    if isinstance(v, dict):
+        out = {}
+        for k, x in v.items():
+            out[_no_surrogates(k)] = _no_surrogates(x)
+        return out
+    if isinstance(v, list):
+        return [_no_surrogates(x) for x in v]
+    return v
+
+
+def _go_float(text):
+    x = float(text)
+    if math.isinf(x):
+        raise ValueError("json: cannot unmarshal number %s into a float64" % text)    # strconv.ParseFloat range error
+    return x
+
+
+def _reject_constant(name):
+    raise ValueError("invalid character in JSON: %s" % name)                            # NaN / Infinity are not JSON
+
+
+def decode_execution_payload(raw):
+    """decodeExecutionPayload (internal/services/webhook_dispatcher.go:459-468) with Go's rules, not Python's: None for empty raw (nil);
+    the decoded interface{} value (numbers float64, None for null) when json.Unmarshal accepts raw; otherwise the bytes of raw (the
+    Go string(raw)).  Unmarshal rejects invalid syntax (NaN and Infinity included) and numbers out of float64 range."""
+    import json
+    raw = bytes(raw or b"")
+    if not raw:
+        return None
+    try:
+        v = json.loads(go_utf8(raw), parse_float=_go_float, parse_int=_go_float, parse_constant=_reject_constant)
+    except ValueError:
+        return raw
+    return _no_surrogates(v)
+
+
+def webhook_event(status) -> str:
+    """determineWebhookEvent (webhook_dispatcher.go:450-457)."""
+    from .services import normalize_execution_status
+    s = go_utf8(status) if isinstance(status, (bytes, bytearray)) else status
+    return "execution.completed" if normalize_execution_status(s) == "succeeded" else "execution.failed"
+
+
+def build_webhook_payload(record) -> bytes:
+    """json.Marshal(buildPayload(exec, determineWebhookEvent(exec.Status))) (webhook_dispatcher.go:296-299, 394-419).  record: execution_id,
+    run_id, status, node_id, reasoner_id, target_type, timestamp (str or bytes); duration_ms (int or None); result (the raw stored
+    ResultPayload, bytes; None or b"" = nil); error_message (str, bytes or None)."""
+    def col(k):
+        v = record[k]
+        return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+    event = webhook_event(record["status"])
+    parts = ['"event":' + string(event), '"execution_id":' + string_bytes(col("execution_id")), '"workflow_id":' + string_bytes(col("run_id")),
+             '"status":' + string_bytes(col("status")), '"target":' + string_bytes(col("node_id") + b"." + col("reasoner_id")),
+             '"type":' + string_bytes(col("target_type"))]
+    if record.get("duration_ms") is not None:
+        parts.append('"duration_ms":%d' % int(record["duration_ms"]))
+    if event == "execution.completed":
+        r = decode_execution_payload(record.get("result"))
+        if isinstance(r, bytes):
+            parts.append('"result":' + string_bytes(r))
+        elif r is not None:
+            parts.append('"result":' + value(r))
+    elif record.get("error_message") is not None:
+        parts.append('"error_message":' + string_bytes(col("error_message")))
+    parts.append('"timestamp":' + string_bytes(col("timestamp")))
+    return ("{" + ",".join(parts) + "}").encode("utf-8")

@@ -21,7 +21,7 @@ import json
 import numpy as np
 
 from . import _abi, go_json
-from .crypto import Hasher, MAC, default_context, pack
+from .crypto import Hasher, MAC, default_context, pack, pack32
 from .identity import ExpandedKeys, KeySet
 
 
@@ -95,6 +95,60 @@ def generate_webhook_signature_batch(secrets, bodies, ctx=None):
     """generateWebhookSignature for many deliveries: "sha256=" + hex(HMAC-SHA256(secret, body))."""
     tags = MAC(ctx or default_context()).hmac_sha256_batch([s.encode() if isinstance(s, str) else s for s in secrets], bodies)
     return ["sha256=" + t.hex() for t in tags]
+
+
+def _wh_bytes(v):
+    return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+
+
+def pack_webhook_deliveries(records):
+    """The packed inputs of afc_webhook_sign_batch (include/afcrypto.h) for records as build_webhook_payload takes them, plus an
+    optional "secret" (str or bytes; None = the webhook has none)."""
+    cols, flags, dur, results, secrets = [], [], [], [], []
+    for r in records:
+        cols += [_wh_bytes(r[k]) if k != "error_message" else _wh_bytes(r.get(k) or b"") for k in _abi.WEBHOOK_COLUMNS]
+        f = 0
+        if r.get("duration_ms") is not None:
+            f |= _abi.WEBHOOK_HAS_DURATION
+        if r.get("error_message") is not None:
+            f |= _abi.WEBHOOK_HAS_ERROR_MESSAGE
+        if r.get("secret") is not None:
+            f |= _abi.WEBHOOK_HAS_SECRET
+        flags.append(f)
+        dur.append(int(r["duration_ms"]) if r.get("duration_ms") is not None else 0)
+        results.append(bytes(r.get("result") or b""))
+        secrets.append(_wh_bytes(r["secret"]) if r.get("secret") is not None else b"")
+    cb, co = pack(cols)
+    rb, ro = pack(results)
+    sb, so = pack32(secrets)
+    return cb, co, np.array(dur, dtype=np.int64), np.array(flags, dtype=np.uint8), rb, ro, sb, so
+
+
+def sign_webhook_delivery_host(record):
+    """One delivery built on the host (the AFC_WEBHOOK_HOST path): {"body", "header"}."""
+    import hashlib
+    import hmac
+    body = go_json.build_webhook_payload(record)
+    sec = record.get("secret")
+    return {"body": body, "header": None if sec is None else "sha256=" + hmac.new(_wh_bytes(sec), body, hashlib.sha256).hexdigest()}
+
+
+def sign_webhook_deliveries_batch(records, ctx=None):
+    """determineWebhookEvent + buildPayload + json.Marshal + generateWebhookSignature (webhook_dispatcher.go:294-320) for many
+    deliveries in one device call: [{"body": bytes, "header": str | None}].  Deliveries the device declines (AFC_WEBHOOK_HOST) are
+    built by the host mirror."""
+    if not records:
+        return []
+    ctx = ctx or default_context()
+    bodies, off, headers, status = ctx.webhook_sign_packed(*pack_webhook_deliveries(records))
+    out = []
+    for i, r in enumerate(records):
+        if status[i] == _abi.WEBHOOK_HOST:
+            out.append(sign_webhook_delivery_host(r))
+            continue
+        out.append({"body": bytes(bodies[int(off[i]):int(off[i + 1])]),
+                    "header": headers[i].tobytes().decode() if r.get("secret") is not None else None})
+    return out
 
 
 class VCService:

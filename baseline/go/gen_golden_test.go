@@ -387,6 +387,48 @@ func TestPinGolden(t *testing.T) {
 		m.Write(body)
 		check(t, "go_cases.json", c.ExecutionId, "header", "sha256="+hex.EncodeToString(m.Sum(nil)), c.ExpectHeader)
 	}
+	// ---------------- webhook_cases.json: whole deliveries, buildPayload + determineWebhookEvent + decodeExecutionPayload
+	// (internal/services/webhook_dispatcher.go:394-468) restated with the reference's own types and stdlib calls
+	var wc []struct {
+		ExecutionId  string  `json:"execution_id"`
+		RunId        string  `json:"run_id"`
+		Status       string  `json:"status"`
+		NodeId       string  `json:"node_id"`
+		ReasonerId   string  `json:"reasoner_id"`
+		TargetType   string  `json:"target_type"`
+		Timestamp    string  `json:"timestamp"`
+		Result       string  `json:"result"`
+		DurationMs   *int64  `json:"duration_ms"`
+		ErrorMessage *string `json:"error_message"`
+		Secret       *string `json:"secret"`
+		ExpectBody   string  `json:"expect_body"`
+		ExpectHeader *string `json:"expect_header"`
+	}
+	load(t, "webhook_cases.json", &wc)
+	for _, c := range wc {
+		p := types.ExecutionWebhookPayload{Event: types.WebhookEventExecutionFailed, ExecutionID: c.ExecutionId, RunID: c.RunId, Status: c.Status,
+			Target: c.NodeId + "." + c.ReasonerId, TargetType: c.TargetType, DurationMS: c.DurationMs, Timestamp: c.Timestamp}
+		if types.NormalizeExecutionStatus(c.Status) == string(types.ExecutionStatusSucceeded) {
+			p.Event = types.WebhookEventExecutionCompleted
+			if raw := []byte(c.Result); len(raw) > 0 {
+				var v interface{}
+				if err := json.Unmarshal(raw, &v); err == nil {
+					p.Result = v
+				} else {
+					p.Result = string(raw)
+				}
+			}
+		} else {
+			p.ErrorMessage = c.ErrorMessage
+		}
+		body, _ := json.Marshal(p)
+		check(t, "webhook_cases.json", c.ExecutionId, "body", string(body), c.ExpectBody)
+		if c.Secret != nil && c.ExpectHeader != nil {
+			m := hmac.New(sha256.New, []byte(*c.Secret))
+			m.Write(body)
+			check(t, "webhook_cases.json", c.ExecutionId, "header", "sha256="+hex.EncodeToString(m.Sum(nil)), *c.ExpectHeader)
+		}
+	}
 	// ---------------- write go_pinned.json
 	doc := map[string]interface{}{"go": runtime.Version(), "failed": t.Failed(), "entries": out}
 	b, _ := json.MarshalIndent(doc, "", " ")

@@ -339,6 +339,49 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
                                      uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off, uint8_t* d_hashes, uint8_t* d_proof_values,
                                      void* stream);
 
+/* ---- W2: execution webhook deliveries built and signed in one call: determineWebhookEvent + buildPayload + json.Marshal +
+ * generateWebhookSignature (internal/services/webhook_dispatcher.go:294-320, 394-474) for n deliveries.  For delivery i:
+ *   bodies[body_off[i] .. body_off[i+1])   the request body json.Marshal(types.ExecutionWebhookPayload), the result member being
+ *                                        json.Marshal(json.Unmarshal(raw)) (map keys sorted, numbers as float64, strings re-escaped)
+ *                                        or, for raw the JSON grammar rejects, the string(raw)
+ *   headers[71 i .. 71 i + 71)           the X-AgentField-Signature value "sha256=" + hex(HMAC-SHA256(secret, body)) with
+ *                                        AFC_WEBHOOK_HAS_SECRET, 71 zero bytes without
+ *   status[i]                            AFC_WEBHOOK_BUILT, or AFC_WEBHOOK_HOST: a zero-length body and a zeroed header; the caller
+ *                                        builds that delivery itself.  HOST: a status that is not printable ASCII (the event rule), and a
+ *                                        result the device does not re-marshal exactly (duplicate or escaped keys, invalid UTF-8 or lone
+ *                                        surrogate escapes, nesting beyond 32 levels, numbers outside the normal float64 range, an
+ *                                        Eisel-Lemire give-up)
+ * Inputs:
+ *   cols / col_off     AFC_WEBHOOK_COLUMNS byte strings per delivery in the order below, n * 8 + 1 absolute offsets.  target_type is the
+ *                      caller's resolveTargetType; timestamp is the caller's RFC 3339 text (CompletedAt, or now)
+ *   duration_ms        n int64, read with AFC_WEBHOOK_HAS_DURATION (else the member is omitted; 0 is written)
+ *   flags              n bytes of AFC_WEBHOOK_HAS_*; error_message is written for the failed event with AFC_WEBHOOK_HAS_ERROR_MESSAGE only
+ *   results / result_off   the stored ResultPayload of each delivery, n + 1 absolute offsets (empty = nil)
+ *   secrets / secret_off   the webhook secrets, n + 1 absolute uint32 offsets (read with AFC_WEBHOOK_HAS_SECRET only; any length)
+ * results and secrets may be NULL in the host-buffer call when their offsets span no bytes (results also in the _dev call).
+ * bodies_cap must be at least afc_webhook_bound(col_off, result_off, n), computed from the two ends of both offset arrays alone and
+ * additive over deliveries (else AFC_EINVAL before any work).  Other AFC_EINVAL: a NULL pointer, unknown flag bits (host-buffer call),
+ * offsets that run backwards (host-buffer call).  The host-buffer call streams chunks through the context's staging ring, writes every
+ * body at its final offset and wipes the staged secrets from the device slot and the pinned bounce buffer when it returns.  The _dev
+ * call synchronises `stream` once, to read the ends of col_off and result_off.  n = 0 writes body_off[0] = 0 in the host-buffer call
+ * and nothing in the _dev call. */
+#define AFC_WEBHOOK_COLUMNS 8   /* execution_id, run_id, status, node_id, reasoner_id, target_type, timestamp, error_message */
+#define AFC_WEBHOOK_HAS_DURATION 1
+#define AFC_WEBHOOK_HAS_ERROR_MESSAGE 2
+#define AFC_WEBHOOK_HAS_SECRET 4
+#define AFC_WEBHOOK_BUILT 0
+#define AFC_WEBHOOK_HOST 1
+#define AFC_WEBHOOK_HEADER_CHARS 71
+uint64_t afc_webhook_bound(const uint64_t* col_off, const uint64_t* result_off, uint32_t n);
+int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off /* n*8+1 */, const int64_t* duration_ms, const uint8_t* flags,
+                           const uint8_t* results, const uint64_t* result_off /* n+1 */, const uint8_t* secrets, const uint32_t* secret_off /* n+1 */,
+                           uint32_t n, uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off /* n+1 */, uint8_t* headers /* n x 71 */,
+                           uint8_t* status /* n */);
+int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64_t* d_col_off, const int64_t* d_duration_ms, const uint8_t* d_flags,
+                               const uint8_t* d_results, const uint64_t* d_result_off, const uint8_t* d_secrets, const uint32_t* d_secret_off,
+                               uint32_t n, uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_headers, uint8_t* d_status,
+                               void* stream);
+
 /* ---- N4: audit proofs for bulk offline verification (`af vc verify`, internal/cli/vc.go:159-331; export bundles,
  * internal/handlers/ui/did.go:533-865) ------------------------------------------------------------------------
  * afc_merkle_tree materialises every level over a fixed set of leaf hashes (device memory, ~2n x 32 B) so that RFC 6962

@@ -5,8 +5,9 @@ signing bytes already rendered, and of the host-buffer call; host_fallback and a
 in the same run.  The audit_stored block does the same for the audit of stored execution VCs against their records
 (afc_vc_audit_stored_batch[_dev]), next to the stored-verify device call on the same documents.  The verify_json block measures
 documents in three client spellings (afc_vc_verify_json_batch_dev) next to the stored-verify call on the canonical form.  The
-issue_execution block measures execution credentials issued in one call (afc_vc_issue_execution_batch[_dev]).  Needs a
-CUDA device; writes nothing.
+issue_execution block measures execution credentials issued in one call (afc_vc_issue_execution_batch[_dev]).  The webhook block
+measures webhook deliveries built and signed in one call (afc_webhook_sign_batch[_dev]) next to HMAC alone over the same bodies.
+Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
 import json
@@ -336,12 +337,131 @@ def issue_execution_block(ctx, dev, timed):
             "tail": {"long_payloads": int(long_n), "vcs_per_s": n / (ms_tail * 1e-3), "ms": ms_tail, "kernels_ms": tkms, "hashes_ok": bool(tail_ok)}}
 
 
+def webhook_results(count, seed):
+    """Agent results as the Python SDK stores them: json.dumps default spelling of nested objects of 100 B - 4 KB, keys in insertion
+    (unsorted) order, 17-digit floats, non-ASCII text as \\u escapes in values."""
+    import random
+    rng = random.Random(seed)
+
+    def val(depth):
+        k = rng.random()
+        if depth < 3 and k < 0.2:
+            return {"k%02d_%s" % (rng.randrange(100), rng.choice(["score", "label", "items", "meta"])): val(depth + 1) for _ in range(rng.randrange(1, 6))}
+        if depth < 3 and k < 0.3:
+            return [val(depth + 1) for _ in range(rng.randrange(1, 5))]
+        if k < 0.55:
+            return rng.random() * 10.0 ** rng.randrange(-5, 8)
+        if k < 0.65:
+            return rng.randrange(-10 ** 9, 10 ** 9)
+        if k < 0.9:
+            return "".join(rng.choice("abcdefghij <>&é中😀\n") for _ in range(rng.randrange(4, 40)))
+        return rng.choice([True, False, None])
+    out = []
+    while len(out) < count:
+        target = int(100 * 40 ** rng.random())                  # 100 B - 4 KB, log-uniform
+        d = {}
+        while len(json.dumps(d)) < target:
+            d["field_%d_%s" % (rng.randrange(1000), rng.choice(["answer", "score", "trace"]))] = val(0)
+        out.append(json.dumps(d).encode())
+    return out
+
+
+def webhook_block(ctx, dev, timed):
+    """afc_webhook_sign_batch_dev over 2^20 deliveries: results drawn from 4096 seeded texts, 10 % failed deliveries with error messages,
+    10 % without a secret, 1 % planted AFC_WEBHOOK_HOST (a status with a non-ASCII space)."""
+    import random
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import go_json, services
+    n = 1 << 20
+    texts = webhook_results(4096, 0xAF20)
+    rng = random.Random(0xAF21)
+    base = []
+    for i in range(4096):
+        failed = i % 10 == 3
+        base.append(dict(execution_id="exec_%07d" % i, run_id="run_%05d" % (i // 7), status="failed" if failed else "succeeded", node_id="agent-%d" % (i % 97),
+                         reasoner_id="reasoner_%d" % (i % 13), target_type="reasoner", timestamp="2026-09-21T06:%02d:%02dZ" % (i // 60 % 60, i % 60),
+                         duration_ms=rng.randrange(0, 10 ** 6), result=texts[i], error_message="step %d failed: <timeout> & retry" % i if failed else None,
+                         secret=None if i % 10 == 7 else "whsec_%032x" % rng.getrandbits(128)))
+    recs = []
+    planted = 0
+    for i in range(n):
+        r = base[i % 4096]
+        if i % 100 == 51:
+            r = dict(r, status="done\x85")
+            planted += 1
+        recs.append(r)
+    packed = services.pack_webhook_deliveries(recs)
+    cb, co, dur, fl, rb, ro, sb, so = packed
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    lib, P = afb._abi.load(), afb._abi.ptr
+    cap = int(lib.afc_webhook_bound(P(co), P(ro), n))
+    D = [t(cb), t(co.view(np.int64)), t(dur), t(fl), t(rb), t(ro.view(np.int64)), t(sb), t(so.view(np.int32))]
+    d_bodies = torch.empty(cap, dtype=torch.uint8, device=dev)
+    d_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+    d_h = torch.empty((n, 71), dtype=torch.uint8, device=dev)
+    d_st = torch.empty(n, dtype=torch.uint8, device=dev)
+
+    def dev_call():
+        ctx.webhook_sign_dev(*D, n, d_bodies, cap, d_off, d_h, d_st)
+    dev_call()
+    torch.cuda.synchronize()
+    st = d_st.cpu().numpy()
+    off = d_off.cpu().numpy().view(np.uint64)
+    host_fallback = int((st == afb._abi.WEBHOOK_HOST).sum())
+    bodies = d_bodies[:int(off[-1])].cpu().numpy()
+    srng = random.Random(3)
+    sample_ok = all(st[i] == afb._abi.WEBHOOK_HOST or bodies[int(off[i]):int(off[i + 1])].tobytes() == go_json.build_webhook_payload(recs[i])
+                    for i in srng.sample(range(n), 2000))
+    ms_dev = timed(dev_call)
+    ctx.profile_begin()
+    timed(dev_call, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    # the floor: HMAC alone over the same bodies, built beforehand
+    d_sec, d_soff = D[6], D[7]
+    d_mac = torch.empty((n, 32), dtype=torch.uint8, device=dev)
+    ms_hmac = timed(lambda: ctx.hmac_sha256_dev(d_sec, d_soff, d_bodies, d_off, n, d_mac))
+    body_bytes = int(off[-1])
+    del d_bodies, d_h, d_mac, D
+    torch.cuda.empty_cache()
+    # the host-buffer call from pinned memory
+    nh = 1 << 18
+
+    def pin(a):
+        p_ = torch.empty(a.shape, dtype=torch.from_numpy(a[:0]).dtype, pin_memory=True).numpy()
+        p_[...] = a
+        return p_
+    hp = services.pack_webhook_deliveries(recs[:nh])
+    hin = [pin(a) for a in hp]
+    hcap = int(lib.afc_webhook_bound(P(hin[1]), P(hin[5]), nh))
+    hb = torch.empty(hcap, dtype=torch.uint8, pin_memory=True).numpy()
+    hoff = torch.empty(nh + 1, dtype=torch.int64, pin_memory=True).numpy()
+    hh = torch.empty((nh, 71), dtype=torch.uint8, pin_memory=True).numpy()
+    hs = torch.empty(nh, dtype=torch.uint8, pin_memory=True).numpy()
+
+    def host_call():
+        afb._abi.check(lib.afc_webhook_sign_batch(ctx.handle, *[P(a) for a in hin], nh, P(hb), hcap, P(hoff), P(hh), P(hs)), ctx.handle)
+    host_call()
+    host_same = int(hoff[nh]) == int(off[nh]) and hb[:int(hoff[nh])].tobytes() == bodies[:int(off[nh])].tobytes()
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        host_call()
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"deliveries": n, "result_bytes": int(ro[-1]), "body_bytes": body_bytes, "gpu": gpu, "planted_host": planted, "host_fallback": host_fallback,
+            "sample_ok": bool(sample_ok), "dev_call": {"deliveries_per_s": n / (ms_dev * 1e-3), "ms": ms_dev, "kernels_ms": kms},
+            "hmac_floor": {"deliveries_per_s": n / (ms_hmac * 1e-3), "ms": ms_hmac, "note": "afc_hmac_sha256_batch_dev over the bodies, built beforehand"},
+            "host_call": {"deliveries": nh, "deliveries_per_s": nh / (ms_host * 1e-3), "ms": ms_host, "same_as_dev": bool(host_same),
+                          "note": "every buffer pinned"}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution"], default=None, help="run one block")
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook"], default=None, help="run one block")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     ctx = afb.Context(0)
@@ -355,7 +475,7 @@ def main():
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
-              "issue_execution": issue_execution_block}
+              "issue_execution": issue_execution_block, "webhook": webhook_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
