@@ -22,6 +22,9 @@ AUDIT_STATUS_UNDECIDED, AUDIT_TIMESTAMP_UNDECIDED = 1 << 18, 1 << 19
 ISSUE_COLUMNS = ("vc_id", "caller_did", "issuance_date", "execution_id", "workflow_id", "session_id", "caller_type", "agent_node_did",
                  "target_did", "function_name", "timestamp", "status", "error_message", "proof_created")
 ISSUE_HASH_DATA = 1
+WORKFLOW_COLUMNS = ("workflow_id", "session_id", "issuer_did", "vc_id", "issuance_date", "snapshot_time", "proof_created")
+WORKFLOW_RECORD_COLUMNS = ("vc_id", "status")
+WORKFLOW_BUILT, WORKFLOW_HOST = 0, 1
 WEBHOOK_COLUMNS = ("execution_id", "run_id", "status", "node_id", "reasoner_id", "target_type", "timestamp", "error_message")
 WEBHOOK_HAS_DURATION, WEBHOOK_HAS_ERROR_MESSAGE, WEBHOOK_HAS_SECRET = 1, 2, 4
 WEBHOOK_BUILT, WEBHOOK_HOST = 0, 1
@@ -91,6 +94,9 @@ SYMBOLS = {
                                                vp]),
     "afc_vc_issue_execution_batch_dev": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp, C.c_uint64, vp,
                                                    vp, vp, vp]),
+    "afc_vc_workflow_bound": (C.c_uint64, [vp, vp, vp, C.c_uint32]),
+    "afc_vc_issue_workflow_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),
+    "afc_vc_issue_workflow_batch_dev": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, vp]),
     "afc_webhook_bound": (C.c_uint64, [vp, vp, C.c_uint32]),
     "afc_webhook_sign_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_sign_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),

@@ -130,6 +130,33 @@ cudaError_t wh_sign(const uint8_t* secrets, const uint32_t* secret_off, const ui
                     const uint64_t* body_off, uint32_t n, uint8_t* mac, uint8_t* headers, cudaStream_t s, LaunchLog* lg);
 uint64_t wh_fixed_bytes();             // the constant text a body can hold at most
 
+// ---- k_vcworkflow.cu: workflow credentials issued on the device (afc_vcworkflow.cuh).  col_off: 7 absolute offsets per workflow + 1;
+// rec_off: n + 1 absolute record indices; rec_col_off (2 per record + 1) and created_at (2 per record) are indexed by absolute record;
+// the batch's m = rec_off[n] - rec_off[0] records have per-record scratch cls (m bytes) and id lengths / offsets (m + 1 entries);
+// arr: 2 per workflow (where its componentVcIds array starts, its length)
+// out: col_off[0], col_off[7 n], rec_off[0], rec_off[n], rec_col_off[2 rec_off[0]], rec_col_off[2 rec_off[n]] (one thread)
+cudaError_t vcw_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s,
+                     LaunchLog* lg);
+// each record's class and escaped-id length (write them to id_off + 1 for offsets_from_lengths)
+cudaError_t vcw_records(const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created_at, const uint64_t* rec_off, uint32_t m,
+                        uint8_t* cls, uint64_t* id_len, cudaStream_t s, LaunchLog* lg);
+// each workflow's summary and state, and its signing-message and stored-document length (0 for VCW_HOST; write them to off + 1)
+cudaError_t vcw_sizes(const uint8_t* cols, const uint64_t* col_off, const uint64_t* rec_off, const int64_t* created_at, const uint8_t* cls,
+                      const uint64_t* id_len, uint32_t n, uint64_t* msg_len, uint64_t* doc_len, uint64_t* arr, uint32_t* summary, uint8_t* state,
+                      cudaStream_t s, LaunchLog* lg);
+// both byte strings of each workflow's credential around its componentVcIds array; the proofValue is a placeholder until vcw_proof
+cudaError_t vcw_fill(const uint8_t* cols, const uint64_t* col_off, const uint64_t* rec_off, const int64_t* created_at, const uint32_t* summary,
+                     const uint8_t* state, const uint64_t* arr, uint32_t n, const uint64_t* msg_off, uint8_t* msgs, const uint64_t* doc_off,
+                     uint8_t* docs, cudaStream_t s, LaunchLog* lg);
+// every record's id into both byte strings (id_off: the scanned id lengths)
+cudaError_t vcw_ids(const uint8_t* rec_cols, const uint64_t* rec_col_off, const uint64_t* rec_off, uint32_t n, uint32_t m, const uint8_t* state,
+                    const uint64_t* arr, const uint64_t* id_off, const uint64_t* msg_off, uint8_t* msgs, const uint64_t* doc_off, uint8_t* docs,
+                    cudaStream_t s, LaunchLog* lg);
+// sigs: n x 64, 16-byte aligned -> 86 characters into each built document and into proof_values (zeros for VCW_HOST)
+cudaError_t vcw_proof(const uint8_t* sigs, const uint8_t* state, uint32_t n, const uint64_t* doc_off, uint8_t* docs, uint8_t* proof_values,
+                      cudaStream_t s, LaunchLog* lg);
+uint64_t vcw_literal_bytes();          // constant text of both document forms together
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

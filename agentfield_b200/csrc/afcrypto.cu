@@ -1442,6 +1442,268 @@ int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32
     return rc;
 }
 
+// ---------------------------------------------------------------------------------- issuing workflow credentials
+// Bounds from the three offset arrays' ends alone: each workflow's constant text, three counts of at most 10 digits, the longest status
+// name, startTime, the endTime member, the array's brackets and the 86 proofValue characters; at most 6 bytes per column byte for each of
+// its at most 4 appearances in the stored document (issuer_did: issuer, orchestrator.did and agentNodeDid, verificationMethod), and per
+// record its escaped id in quotes with a comma.  The signing message never holds more than the stored document.
+static uint64_t wf_fixed_bytes() { return launch::vcw_literal_bytes() + 3 * 10 + 9 + 20 + 33 + 2 + 86; }
+static uint64_t wf_doc_bound(uint32_t n, uint64_t col_bytes, uint64_t records, uint64_t rec_bytes) {
+    return (uint64_t)n * wf_fixed_bytes() + 24 * col_bytes + 6 * rec_bytes + 3 * records;
+}
+
+uint64_t afc_vc_workflow_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n) {
+    if (!col_off || !rec_off || !rec_col_off || n == 0) return 0;
+    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_WORKFLOW_COLUMNS], r0 = rec_off[0], r1 = rec_off[n];
+    if (r1 < r0) return wf_doc_bound(n, b >= a ? b - a : 0, 0, 0);
+    const uint64_t c = rec_col_off[2 * r0], d = rec_col_off[2 * r1];
+    return wf_doc_bound(n, b >= a ? b - a : 0, r1 - r0, d >= c ? d - c : 0);
+}
+
+// per-call device scratch: signing messages and their offsets, signatures, scan tiles, record classes, record id offsets, array places
+struct WorkflowScratch { uint8_t* msgs; uint64_t* msg_off; uint8_t* sigs; uint64_t* scan; uint8_t* cls; uint64_t* id_off; uint64_t* arr; };
+static size_t wf_scratch_bytes(uint32_t n, uint32_t m, uint64_t msg_bound) {
+    return vc_align(msg_bound + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) + vc_align(launch::json_scan_scratch_bytes(n > m ? n : m)) +
+           vc_align(m) + vc_align(((size_t)m + 1) * 8) + vc_align((size_t)n * 16);
+}
+static WorkflowScratch wf_scratch(uint8_t* p, uint32_t n, uint32_t m, uint64_t msg_bound) {
+    WorkflowScratch s;
+    s.msgs = p; p += vc_align(msg_bound + 64);
+    s.msg_off = (uint64_t*)p; p += vc_align(((size_t)n + 1) * 8);
+    s.sigs = p; p += vc_align((size_t)n * 64);
+    s.scan = (uint64_t*)p; p += vc_align(launch::json_scan_scratch_bytes(n > m ? n : m));
+    s.cls = p; p += vc_align(m);
+    s.id_off = (uint64_t*)p; p += vc_align(((size_t)m + 1) * 8);
+    s.arr = (uint64_t*)p;
+    return s;
+}
+// records, plans and both lengths, the three scans: doc_off is complete when this has run
+static cudaError_t wf_sizes(const uint8_t* cols, const uint64_t* col_off, const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off,
+                            const int64_t* created, uint32_t n, uint32_t m, uint64_t* doc_off, uint32_t* summary, uint8_t* state,
+                            const WorkflowScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = launch::vcw_records(rec_cols, rec_col_off, created, rec_off, m, S.cls, S.id_off + 1, st, lg);
+    if (e == cudaSuccess) e = launch::vcw_sizes(cols, col_off, rec_off, created, S.cls, S.id_off + 1, n, S.msg_off + 1, doc_off + 1, S.arr, summary,
+                                                state, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(S.msg_off, n, S.scan, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(doc_off, n, S.scan, st, lg);
+    if (e == cudaSuccess && m) e = launch::offsets_from_lengths(S.id_off, m, S.scan, st, lg);
+    return e;
+}
+// both byte strings, the signatures, the proofValues
+static cudaError_t wf_finish(afc_ctx* ctx, const uint8_t* d_exp, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
+                             const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created, uint32_t n, uint32_t m,
+                             uint8_t* docs, const uint64_t* doc_off, uint8_t* pv, const uint8_t* state, const uint32_t* summary, const WorkflowScratch& S,
+                             cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = launch::vcw_fill(cols, col_off, rec_off, created, summary, state, S.arr, n, S.msg_off, S.msgs, doc_off, docs, st, lg);
+    if (e == cudaSuccess) e = launch::vcw_ids(rec_cols, rec_col_off, rec_off, n, m, state, S.arr, S.id_off, S.msg_off, S.msgs, doc_off, docs, st, lg);
+    if (e == cudaSuccess) e = launch::ed_sign_expanded_batch(ctx->comb, afc_internal_sign_table(ctx), d_exp, n_keys, key_index, S.msgs, S.msg_off, n,
+                                                             S.sigs, st, lg);
+    if (e == cudaSuccess) e = launch::vcw_proof(S.sigs, state, n, doc_off, docs, pv, st, lg);
+    return e;
+}
+static int wf_check(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
+                    const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n, const uint8_t* docs, const uint64_t* doc_off,
+                    const uint8_t* proof_values, const uint8_t* state, const uint32_t* summary) {
+    if (!ctx || !col_off || !rec_off || !rec_col_off || !doc_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!expanded96 || n_keys == 0 || !key_index || !cols || !docs || !proof_values || !state || !summary) return AFC_EINVAL;
+    return AFC_OK;
+}
+
+int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                    const uint64_t* d_col_off, const uint64_t* d_rec_off, const uint8_t* d_rec_cols, const uint64_t* d_rec_col_off,
+                                    const int64_t* d_created_at, uint32_t n, uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off,
+                                    uint8_t* d_proof_values, uint8_t* d_state, uint32_t* d_summary, void* stream) {
+    int rc = wf_check(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_col_off, n, d_docs, d_doc_off, d_proof_values,
+                      d_state, d_summary);
+    if (rc != AFC_OK || n == 0) return rc;
+    if (!aligned16(d_expanded96)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[6];                       // the ends of the three offset arrays bound the documents: gathered by one thread, read once
+    {
+        uint64_t* d_ends = nullptr;
+        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
+        cudaError_t e = launch::vcw_ends(d_col_off, d_rec_off, d_rec_col_off, n, d_ends, st, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(d_ends, st);
+        CK(e);
+        CK(cudaStreamSynchronize(st));
+    }
+    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] > 0xffffffffull) return AFC_EINVAL;
+    const uint32_t m = (uint32_t)(ends[3] - ends[2]);
+    if (m && (!d_rec_cols || !d_created_at)) return AFC_EINVAL;
+    const uint64_t bound = wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4]);
+    if (docs_cap < bound) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, wf_scratch_bytes(n, m, bound), st));
+    const WorkflowScratch S = wf_scratch(scratch, n, m, bound);
+    cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, d_doc_off, d_summary, d_state, S, st, lc);
+    if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m,
+                                        d_docs, d_doc_off, d_proof_values, d_state, d_summary, S, st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+// The host-buffer call: chunks of whole workflows through the lane's ring, as issue_host_run does.  A chunk's records travel with it
+// (the kernels index them by absolute record, so the staged record arrays are addressed from a shifted base); a workflow larger than a
+// chunk's byte budget goes alone.
+static int wf_host_run(afc_ctx* ctx, const uint8_t* d_keys, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
+                       const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created, uint32_t n, uint8_t* docs,
+                       uint64_t* doc_off, uint8_t* pv, uint8_t* state, uint32_t* summary) {
+    const uint32_t C = AFC_WORKFLOW_COLUMNS;
+    LaneGuard lg(ctx);
+    Lane& lane = lg.lane();
+    LaneDrain drain_on_exit(lane);
+    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_ki = is_pinned(key_index), pin_roff = is_pinned(rec_off);
+    const bool pin_rcols = is_pinned(rec_cols), pin_rcoff = is_pinned(rec_col_off), pin_cr = is_pinned(created);
+    const bool pin_docs = is_pinned(docs), pin_pv = is_pinned(pv), pin_st = is_pinned(state), pin_sum = is_pinned(summary);
+    CallLog lc(ctx);
+    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
+    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
+    auto drain = [&](int w) -> int {
+        Pending& p = pend[w];
+        if (!p.active) return AFC_OK;
+        Slot& sl = lane.slot[w];
+        CK(cudaStreamSynchronize(sl.stream));
+        const uint8_t* h = sl.h_out.p;
+        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
+        for (uint32_t j = 0; j < p.cnt; j++) doc_off[p.i0 + j] = p.base + rel[j];
+        if (!pin_pv) { memcpy(pv + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
+        if (!pin_st) { memcpy(state + p.i0, h, p.cnt); h += vc_align(p.cnt); }
+        if (!pin_sum) { memcpy(summary + (size_t)p.i0 * 4, h, (size_t)p.cnt * 16); h += vc_align((size_t)p.cnt * 16); }
+        if (!pin_docs) memcpy(docs + p.base, h, p.bytes);
+        p.active = false;
+        return AFC_OK;
+    };
+    uint32_t i0 = 0;
+    uint64_t base = 0;
+    int which = 0;
+    while (i0 < n) {
+        const uint32_t left = n - i0;
+        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
+        if (limit < min_chunk) limit = min_chunk;
+        if (limit > max_chunk) limit = max_chunk;
+        uint32_t i1 = i0;
+        const uint64_t cbase = col_off[(size_t)i0 * C], r0 = rec_off[i0], rbase = rec_col_off[2 * r0];
+        while (i1 < n && i1 - i0 < limit) {
+            const uint64_t r = rec_off[i1 + 1];
+            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (rec_col_off[2 * r] - rbase) + 32 * (r - r0);
+            if (bytes > kChunkBytes && i1 != i0) break;
+            i1++;
+        }
+        const uint32_t cnt = i1 - i0;
+        const uint64_t r1 = rec_off[i1];
+        const uint32_t m = (uint32_t)(r1 - r0);
+        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, rbytes = rec_col_off[2 * r1] - rbase;
+        Slot& sl = lane.slot[which];
+        int rc = drain(which);
+        if (rc != AFC_OK) return rc;
+        const uint64_t dbound = wf_doc_bound(cnt, cbytes, m, rbytes);
+        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 4, ((size_t)cnt + 1) * 8, rbytes + 32, ((size_t)2 * m + 1) * 8,
+                             (size_t)m * 16, dbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 86, (size_t)cnt, (size_t)cnt * 16,
+                             wf_scratch_bytes(cnt, m, dbound)};
+        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
+        size_t total = 0;
+        for (size_t b : sz) total += vc_align(b);
+        CK(sl.vc.reserve(total));
+        uint8_t* q[NB];
+        {
+            uint8_t* p = sl.vc.p;
+            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
+        }
+        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_ki ? 0 : (size_t)cnt * 4,
+                                   pin_roff ? 0 : ((size_t)cnt + 1) * 8, pin_rcols ? 0 : rbytes, pin_rcoff ? 0 : ((size_t)2 * m + 1) * 8,
+                                   pin_cr ? 0 : (size_t)m * 16};
+        size_t bounce = 0;
+        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
+        CK(sl.h_in.reserve(bounce + 256, ctx));
+        CK(sl.h_out2.reserve(8, ctx));
+        size_t used = 0;
+        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
+        const uint64_t* d_coff = (const uint64_t*)q[1];
+        const uint32_t* d_ki = (const uint32_t*)q[2];
+        const uint64_t* d_roff = (const uint64_t*)q[3];
+        uint8_t* d_rcols = q[4] + (rbase & 15) - rbase;
+        const uint64_t* d_rcoff = (const uint64_t*)q[5] - 2 * r0;     // absolute record indices stay valid
+        const int64_t* d_cr = (const int64_t*)q[6] - 2 * r0;
+        uint8_t* d_docs = q[7];
+        uint64_t* d_doff = (uint64_t*)q[8];
+        uint8_t* d_pv = q[9];
+        uint8_t* d_st = q[10];
+        uint32_t* d_sum = (uint32_t*)q[11];
+        const WorkflowScratch S = wf_scratch(q[12], cnt, m, dbound);
+        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
+        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
+        CK(h2d(sl, q[2], key_index + i0, (size_t)cnt * 4, pin_ki, &used));
+        CK(h2d(sl, q[3], rec_off + i0, ((size_t)cnt + 1) * 8, pin_roff, &used));
+        if (m) {
+            CK(h2d(sl, q[4] + (rbase & 15), rec_cols + rbase, rbytes, pin_rcols, &used));
+            CK(h2d(sl, q[5], rec_col_off + 2 * r0, ((size_t)2 * m + 1) * 8, pin_rcoff, &used));
+            CK(h2d(sl, q[6], created + 2 * r0, (size_t)m * 16, pin_cr, &used));
+        }
+        CK(wf_sizes(d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_doff, d_sum, d_st, S, sl.stream, lc));
+        CK(cudaMemcpyAsync(sl.h_out2.p, d_doff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
+        CK(cudaStreamSynchronize(sl.stream));
+        uint64_t bytes;
+        memcpy(&bytes, sl.h_out2.p, 8);
+        CK(wf_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_docs, d_doff, d_pv, d_st, d_sum, S, sl.stream, lc));
+        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_pv ? 0 : vc_align((size_t)cnt * 86)) + (pin_st ? 0 : vc_align(cnt)) +
+                            (pin_sum ? 0 : vc_align((size_t)cnt * 16)) + (pin_docs ? 0 : bytes) + 256, ctx));
+        uint8_t* h = sl.h_out.p;
+        CK(cudaMemcpyAsync(h, d_doff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
+        h += vc_align(((size_t)cnt + 1) * 8);
+        CK(cudaMemcpyAsync(pin_pv ? pv + (size_t)i0 * 86 : h, d_pv, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_pv) h += vc_align((size_t)cnt * 86);
+        CK(cudaMemcpyAsync(pin_st ? state + i0 : h, d_st, cnt, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_st) h += vc_align(cnt);
+        CK(cudaMemcpyAsync(pin_sum ? (void*)(summary + (size_t)i0 * 4) : (void*)h, d_sum, (size_t)cnt * 16, cudaMemcpyDeviceToHost, sl.stream));
+        if (!pin_sum) h += vc_align((size_t)cnt * 16);
+        if (bytes) CK(cudaMemcpyAsync(pin_docs ? docs + base : h, d_docs, bytes, cudaMemcpyDeviceToHost, sl.stream));
+        pend[which] = {i0, cnt, base, bytes, true};
+        base += bytes;
+        which = (which + 1) % kSlots;
+        i0 = i1;
+    }
+    for (int w = 0; w < kSlots; w++) {      // oldest first
+        int rc = drain((which + w) % kSlots);
+        if (rc != AFC_OK) return rc;
+    }
+    drain_on_exit.armed = false;
+    doc_off[n] = base;
+    return AFC_OK;
+}
+
+int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                const uint64_t* col_off, const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off,
+                                const int64_t* created_at, uint32_t n, uint8_t* docs, uint64_t docs_cap, uint64_t* doc_off, uint8_t* proof_values,
+                                uint8_t* state, uint32_t* summary) {
+    int rc = wf_check(ctx, expanded96, n_keys, key_index, cols, col_off, rec_off, rec_col_off, n, docs, doc_off, proof_values, state, summary);
+    if (rc != AFC_OK) return rc;
+    if (n == 0) { doc_off[0] = 0; return AFC_OK; }
+    for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
+    uint64_t bad = 0;
+    for (size_t k = 0; k < (size_t)n * AFC_WORKFLOW_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
+    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(rec_off[i + 1] < rec_off[i]) | (uint64_t)(rec_off[i + 1] - rec_off[i] > 0xffffffffull);
+    if (bad) return AFC_EINVAL;
+    for (uint64_t k = 2 * rec_off[0]; k < 2 * rec_off[n]; k++) bad |= (uint64_t)(rec_col_off[k + 1] < rec_col_off[k]);
+    if (bad || docs_cap < afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n)) return AFC_EINVAL;
+    if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    uint8_t* d_keys = nullptr;
+    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
+    cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        rc = wf_host_run(ctx, d_keys, n_keys, key_index, cols, col_off, rec_off, rec_cols, rec_col_off, created_at, n, docs, doc_off, proof_values, state,
+                         summary);
+    } else { set_err(ctx, e, "cudaMemcpy(expanded keys)"); rc = AFC_ECUDA; }
+    cudaMemset(d_keys, 0, (size_t)n_keys * 96);       // expanded private keys do not outlive the call on the device
+    cudaFree(d_keys);
+    return rc;
+}
+
 // ---------------------------------------------------------------------------------- webhook deliveries
 // Bound from the byte counts alone: each delivery's constant text plus at most 6 bytes per column and result byte (a byte escaped as
 // backslash-u 00XX or fffd; a number token grows at most 21 / 4 times, 1e20 -> 100000000000000000000).

@@ -14,6 +14,7 @@ Derivation follows the reference exactly: seed' = SHA-256(masterSeed || path), d
 """
 import base64
 import ctypes as C
+import datetime
 
 import numpy as np
 
@@ -153,6 +154,131 @@ class ExpandedKeys:
             ih, oh = (hashes[i, :43].tobytes().decode(), hashes[i, 43:].tobytes().decode()) if hash_data else ("", "")
             out.append({"vc_document": buf[int(off[i]):int(off[i + 1])], "signature": pv[i].tobytes().decode(), "input_hash": ih, "output_hash": oh})
         return out
+
+    # -- workflow credentials (afc_vc_issue_workflow_batch)
+    _wf_coef = None
+
+    @classmethod
+    def _workflow_bound(cls, n, col_bytes, records, rec_bytes):
+        """afc_vc_workflow_bound for n workflows with these totals, without building their offset arrays: the bound is linear in the four,
+        so its coefficients are read off the library once."""
+        if cls._wf_coef is None:
+            lib = _abi.load()
+            col_off = np.zeros(len(_abi.WORKFLOW_COLUMNS) + 1, dtype=np.uint64)
+            rec_off = np.zeros(2, dtype=np.uint64)
+            rec_col_off = np.zeros(3, dtype=np.uint64)
+
+            def f():
+                return lib.afc_vc_workflow_bound(_abi.ptr(col_off), _abi.ptr(rec_off), _abi.ptr(rec_col_off), 1)
+            fixed = f()
+            col_off[-1] = 1
+            per_col = f() - fixed
+            col_off[-1] = 0
+            rec_off[1] = 1
+            per_rec = f() - fixed
+            rec_col_off[2] = 1
+            per_rec_byte = f() - fixed - per_rec
+            cls._wf_coef = (fixed, per_col, per_rec, per_rec_byte)
+        fixed, per_col, per_rec, per_rec_byte = cls._wf_coef
+        return n * fixed + per_col * col_bytes + per_rec * records + per_rec_byte * rec_bytes if n else 0
+
+    @staticmethod
+    def workflow_issuer(w):
+        """The issuer generateWorkflowVCDocument signs with: the first record's issuer_did, the root DID without records."""
+        evs = w["execution_vcs"]
+        return evs[0]["issuer_did"] if evs else w["root_did"]
+
+    @staticmethod
+    def pack_workflow_requests(workflows):
+        """generateWorkflowVCDocument inputs (the dicts of services.VCService.issue_workflow_vc_batch: workflow_id, execution_vcs of vc_id,
+        session_id, status, created_at (an aware datetime), issuer_did; root_did, vc_id, issuance_date, snapshot_time, proof_created) -> the
+        host arrays of afc_vc_issue_workflow_batch: (cols, col_off, rec_off, rec_cols, rec_col_off, created_at).  Strings are UTF-8 with lone surrogates kept as their three bytes; bytes pass as they are."""
+        def b(v):
+            return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+        flat, rflat, created, counts = [], [], [], []
+        for w in workflows:
+            evs = w["execution_vcs"]
+            flat += [b(w["workflow_id"]), b(evs[0]["session_id"] if evs else ""), b(ExpandedKeys.workflow_issuer(w)), b(w["vc_id"]),
+                     b(w["issuance_date"]), b(w["snapshot_time"]), b(w["proof_created"])]
+            for v in evs:
+                rflat += [b(v["vc_id"]), b(v["status"])]
+                created += unix_pair(v["created_at"])
+            counts.append(len(evs))
+        cols, col_off = pack(flat)
+        rec_cols, rec_col_off = pack(rflat)
+        rec_off = np.zeros(len(workflows) + 1, dtype=np.uint64)
+        rec_off[1:] = np.cumsum(counts, dtype=np.uint64)
+        return cols, col_off, rec_off, rec_cols, rec_col_off, np.array(created, dtype=np.int64)
+
+    def issue_workflow_packed(self, key_index, cols, col_off, rec_off, rec_cols, rec_col_off, created_at, expanded=None):
+        """afc_vc_issue_workflow_batch on host arrays (the layout of pack_workflow_requests).  Returns (docs uint8, doc_off uint64 [n+1],
+        proof_values uint8 [n, 86], state uint8 [n], summary uint32 [n, 4])."""
+        n = len(key_index)
+        exp = self._expanded if expanded is None else expanded
+        lib = _abi.load()
+        cap = lib.afc_vc_workflow_bound(_abi.ptr(col_off), _abi.ptr(rec_off), _abi.ptr(rec_col_off), n)
+        docs = np.empty(max(cap, 1), dtype=np.uint8)
+        doc_off = np.zeros(n + 1, dtype=np.uint64)
+        pv = np.empty((n, 86), dtype=np.uint8)
+        state = np.empty(n, dtype=np.uint8)
+        summary = np.empty((n, 4), dtype=np.uint32)
+        _abi.check(lib.afc_vc_issue_workflow_batch(self.ctx.handle, _abi.ptr(exp), exp.shape[0], _abi.ptr(key_index), _abi.ptr(cols),
+                                                   _abi.ptr(col_off), _abi.ptr(rec_off), _abi.ptr(rec_cols), _abi.ptr(rec_col_off),
+                                                   _abi.ptr(created_at), n, _abi.ptr(docs), cap, _abi.ptr(doc_off), _abi.ptr(pv), _abi.ptr(state),
+                                                   _abi.ptr(summary)), self.ctx.handle)
+        return docs[:int(doc_off[n])], doc_off, pv, state, summary
+
+    def issue_workflow_dev(self, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, stream=None, d_expanded=None):
+        """afc_vc_issue_workflow_batch_dev: n workflows on the device.  d_key_index: int32 [n] into this cache (or into d_expanded, K x 96);
+        d_cols / d_col_off: uint8 columns and int64 [7n+1] absolute offsets (_abi.WORKFLOW_COLUMNS order); d_rec_off: int64 [n+1] absolute
+        record indices; d_rec_cols / d_rec_col_off: the records' vc_id and status, int64 [2 per record + 1]; d_created_at: int64 [2 per
+        record] (Unix seconds, nanoseconds).  Returns (d_docs uint8, d_doc_off int64 [n+1], d_proof_values uint8 [n, 86], d_state uint8 [n],
+        d_summary int32 [n, 4], to be read as uint32)."""
+        import torch
+        dev = d_col_off.device
+        if d_expanded is None:
+            d_expanded = torch.from_numpy(self._expanded).to(dev)
+        if n:
+            r0, r1 = int(d_rec_off[0]), int(d_rec_off[n])
+            cap = self._workflow_bound(n, int(d_col_off[n * len(_abi.WORKFLOW_COLUMNS)]) - int(d_col_off[0]), r1 - r0,
+                                       int(d_rec_col_off[2 * r1]) - int(d_rec_col_off[2 * r0]))
+        else:
+            cap = 0
+        d_docs = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        d_doc_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_pv = torch.empty((n, 86), dtype=torch.uint8, device=dev)
+        d_state = torch.empty(n, dtype=torch.uint8, device=dev)
+        d_summary = torch.empty((n, 4), dtype=torch.int32, device=dev)
+        _abi.check(_abi.load().afc_vc_issue_workflow_batch_dev(self.ctx.handle, _abi.ptr(d_expanded), d_expanded.shape[0], _abi.ptr(d_key_index),
+                                                               _abi.ptr(d_cols), _abi.ptr(d_col_off), _abi.ptr(d_rec_off), _abi.ptr(d_rec_cols),
+                                                               _abi.ptr(d_rec_col_off), _abi.ptr(d_created_at), n, _abi.ptr(d_docs), cap,
+                                                               _abi.ptr(d_doc_off), _abi.ptr(d_pv), _abi.ptr(d_state), _abi.ptr(d_summary),
+                                                               self.ctx._stream(stream)), self.ctx.handle)
+        total = int(d_doc_off[n]) if n else 0
+        return d_docs[:total], d_doc_off, d_pv, d_state, d_summary
+
+    def issue_workflows(self, workflows):
+        """generateWorkflowVCDocument for many workflows in one host-buffer call: [{"vc_document": bytes, "signature": str, "state": int,
+        "summary": [status id, completed, start record, end record]}] (an AFC_WORKFLOW_HOST workflow has an empty document and signature)."""
+        n = len(workflows)
+        if n == 0:
+            return []
+        ki = self.key_index([self.workflow_issuer(w) for w in workflows])
+        docs, off, pv, state, summ = self.issue_workflow_packed(ki, *self.pack_workflow_requests(workflows))
+        buf = docs.tobytes()
+        return [{"vc_document": buf[int(off[i]):int(off[i + 1])], "signature": pv[i].tobytes().decode() if state[i] == _abi.WORKFLOW_BUILT else "",
+                 "state": int(state[i]), "summary": [int(x) for x in summ[i]]} for i in range(n)]
+
+
+_EPOCH = datetime.datetime(1970, 1, 1, tzinfo=datetime.timezone.utc)
+
+
+def unix_pair(t):
+    """(Unix seconds, nanoseconds) of an aware datetime."""
+    if t.tzinfo is None:
+        raise ValueError("created_at must be an aware datetime")
+    d = t - _EPOCH
+    return [d.days * 86400 + d.seconds, d.microseconds * 1000]
 
 
 class KeySet:

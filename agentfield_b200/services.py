@@ -16,6 +16,7 @@ every hash / signature on the GPU through the C ABI.  The canonical JSON bytes c
 canonical_on_device=True, from the device: GenerateExecutionVC's hashes, documents and signatures in one call (afc_vc_issue_execution_batch).
 """
 import base64
+import datetime
 import json
 
 import numpy as np
@@ -73,6 +74,16 @@ def determine_workflow_status(execution_vcs) -> str:
 
 def count_completed_steps(execution_vcs) -> int:
     return sum(1 for v in execution_vcs if normalize_execution_status(v["status"]) == "succeeded")
+
+
+_STATUS_NAMES = ("unknown", "pending", "queued", "running", "succeeded", "failed", "cancelled", "timeout")     # AFC_WORKFLOW summary[0]
+_NO_RECORD = 0xFFFFFFFF
+
+
+def _rfc3339(t) -> str:
+    """time.Time.UTC().Format(time.RFC3339) of an aware datetime."""
+    u = t.astimezone(datetime.timezone.utc)
+    return "%04d-%02d-%02dT%02d:%02d:%02dZ" % (u.year, u.month, u.day, u.hour, u.minute, u.second)
 
 
 def create_workflow_vc_document(workflow_id, session_id, component_vc_ids, status, start_time, end_time, issuer_did, vc_id, issuance_date,
@@ -285,6 +296,37 @@ class VCService:
                         "completed_steps": count_completed_steps(evs), "vc_document": vc_bytes, "signature": proof["proofValue"],
                         "issuer_did": issuer, "snapshot_time": w["snapshot_time"], "storage_uri": "", "document_size_bytes": len(vc_bytes),
                         "doc": doc, "proof": proof})
+        return out
+
+    def issue_workflow_vc_batch(self, workflows):
+        """generate_workflow_vc_batch in one device call (ExpandedKeys.issue_workflows): the same inputs, except that each record's
+        created_at is an aware datetime, and the same WorkflowVC-shaped dicts without "doc" / "proof".  Workflows the device declines
+        (AFC_WORKFLOW_HOST: a status that is not printable ASCII) go through generate_workflow_vc_batch."""
+        if not workflows:
+            return []
+        issued = self.keys.issue_workflows(workflows)
+        host = [i for i, v in enumerate(issued) if v["state"] == _abi.WORKFLOW_HOST]
+        by_host = {}
+        if host:
+            text = [dict(workflows[i], execution_vcs=[dict(v, created_at=_rfc3339(v["created_at"])) for v in workflows[i]["execution_vcs"]])
+                    for i in host]
+            for i, v in zip(host, self.generate_workflow_vc_batch(text)):
+                del v["doc"], v["proof"]
+                by_host[i] = v
+        out = []
+        for i, (w, v) in enumerate(zip(workflows, issued)):
+            if i in by_host:
+                out.append(by_host[i])
+                continue
+            evs = w["execution_vcs"]
+            status, completed, start, end = v["summary"]
+            vc_bytes = v["vc_document"]
+            out.append({"workflow_id": w["workflow_id"], "session_id": evs[0]["session_id"] if evs else "", "component_vcs": [e["vc_id"] for e in evs],
+                        "workflow_vc_id": w["workflow_vc_id"], "status": _STATUS_NAMES[status],
+                        "start_time": _rfc3339(evs[start]["created_at"]) if evs else w["snapshot_time"],
+                        "end_time": _rfc3339(evs[end]["created_at"]) if end != _NO_RECORD else None, "total_steps": len(evs),
+                        "completed_steps": completed, "vc_document": vc_bytes, "signature": v["signature"], "issuer_did": self.keys.workflow_issuer(w),
+                        "snapshot_time": w["snapshot_time"], "storage_uri": "", "document_size_bytes": len(vc_bytes)})
         return out
 
     def _keyed_verify(self, dids, msgs, proof_values):

@@ -339,6 +339,62 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
                                      uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off, uint8_t* d_hashes, uint8_t* d_proof_values,
                                      void* stream);
 
+/* ---- E3: issuing workflow credentials in one call: generateWorkflowVCDocument (internal/services/vc_service.go:525-632), which
+ * GetWorkflowVCChain (:292-338) runs on every chain view and VerifyWorkflowVCComprehensive (:1397) on every workflow audit, for n workflows.
+ * Workflow i owns records rec_off[i] .. rec_off[i+1] (its ExecutionVC records in GetExecutionVCsByWorkflow order).  The call writes:
+ *   docs[doc_off[i] .. doc_off[i+1])   the stored vc_document: json.Marshal(WorkflowVCDocument) with the signed proof; the signature
+ *                                       covers the same document with the zero-valued proof (signWorkflowVC).  componentVcIds is always an
+ *                                       array ([] without records); totalSteps, completedSteps and metadata.total_executions are the record
+ *                                       count; endTime is omitted when nil; issuer, orchestrator.did / agentNodeDid and verificationMethod
+ *                                       (+ "#key-1") are the issuer_did column; every column is escaped as Go escapes strings
+ *   proof_values[86 i .. 86 i + 86)     the signature (proofValue, base64url without padding)
+ *   summary[4 i .. 4 i + 4)             [0] the workflow status (determineWorkflowStatus over NormalizeExecutionStatus of each record, numbered
+ *                                       0 unknown, 1 pending, 2 queued, 3 running, 4 succeeded, 5 failed, 6 cancelled, 7 timeout; pending
+ *                                       without records), the name the document holds; [1] countCompletedSteps (records whose status
+ *                                       normalises to succeeded; the document's completedSteps is the record count, as in the reference);
+ *                                       [2] the start record: the first with the earliest (seconds, nanoseconds) (time.Before), relative to
+ *                                       rec_off[i]; [3] the end record: the first with the latest time (time.After), 0xFFFFFFFF unless the
+ *                                       status is terminal.  Both are 0xFFFFFFFF without records.  The caller takes the full-precision StartTime
+ *                                       and EndTime from those records; the document holds them as UTC().Format(time.RFC3339).
+ *   state[i]                            AFC_WORKFLOW_BUILT, or AFC_WORKFLOW_HOST: a zero-length document, a zeroed proof value and summary;
+ *                                       the caller builds that workflow itself.  HOST: a record status with a byte outside printable ASCII
+ *                                       and \t \n \v \f \r (Go's TrimSpace / ToLower are Unicode-aware), a created_at outside
+ *                                       0001-01-01T00:00:00Z .. 9999-12-31T23:59:59Z, or nanoseconds outside [0, 10^9).
+ * Deviation: without records the reference reads time.Now() for startTime, then again for snapshotTime; this call writes the snapshot_time
+ * column's text for both.
+ * Inputs:
+ *   expanded96 / n_keys / key_index   the issuers' expanded keys and each workflow's key (issuer_did's); signing is constant time unless
+ *                                     afc_sign_configure says otherwise
+ *   cols / col_off                    AFC_WORKFLOW_COLUMNS byte strings per workflow, n * 7 + 1 absolute offsets.  session_id and issuer_did
+ *                                     are the first record's (issuer_did: the root DID without records); vc_id, issuance_date, snapshot_time
+ *                                     and proof_created are the caller's (the reference makes up an id and reads a clock)
+ *   rec_off                           n + 1 absolute record indices, non-decreasing
+ *   rec_cols / rec_col_off            AFC_WORKFLOW_RECORD_COLUMNS byte strings per record; record r's column k is
+ *                                     rec_cols[rec_col_off[2 r + k] .. rec_col_off[2 r + k + 1])
+ *   created_at                        2 int64 per record (created_at[2 r], [2 r + 1]): CreatedAt as Unix seconds and nanoseconds
+ * docs_cap must be at least afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n), computed from the ends of the three offset arrays
+ * alone and additive over workflows (else AFC_EINVAL, before any work).  Other AFC_EINVAL: a NULL pointer, n_keys == 0; in the host-buffer
+ * call also key_index[i] >= n_keys and offsets that run backwards.  The _dev call cannot inspect its index array without a sync: an index
+ * >= n_keys signs with key 0.  The host-buffer call streams chunks of whole workflows through the context's staging ring (a workflow
+ * bigger than a slot goes alone) and writes every document at its final offset; the expanded keys it stages are wiped from the device
+ * when it returns.  The _dev call synchronises `stream` once, to read the ends of the offset arrays; expanded96 must be 16-byte aligned
+ * there.  n = 0 writes doc_off[0] = 0 in the host-buffer call and nothing in the _dev call.  Nothing is logged: the reference
+ * neither persists nor logs these snapshots. */
+#define AFC_WORKFLOW_COLUMNS 7         /* workflow_id, session_id, issuer_did, vc_id, issuance_date, snapshot_time, proof_created */
+#define AFC_WORKFLOW_RECORD_COLUMNS 2  /* vc_id, status of each ExecutionVC record, in GetExecutionVCsByWorkflow order */
+#define AFC_WORKFLOW_BUILT 0
+#define AFC_WORKFLOW_HOST 1
+uint64_t afc_vc_workflow_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n);
+int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index /* n */, const uint8_t* cols,
+                                const uint64_t* col_off /* 7n+1 */, const uint64_t* rec_off /* n+1 absolute record indices */,
+                                const uint8_t* rec_cols, const uint64_t* rec_col_off /* 2 per record +1 */,
+                                const int64_t* created_at /* per record: Unix seconds, nanoseconds */, uint32_t n, uint8_t* docs, uint64_t docs_cap,
+                                uint64_t* doc_off /* n+1 */, uint8_t* proof_values /* n x 86 */, uint8_t* state /* n */, uint32_t* summary /* n x 4 */);
+int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                    const uint64_t* d_col_off, const uint64_t* d_rec_off, const uint8_t* d_rec_cols, const uint64_t* d_rec_col_off,
+                                    const int64_t* d_created_at, uint32_t n, uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off,
+                                    uint8_t* d_proof_values, uint8_t* d_state, uint32_t* d_summary, void* stream);
+
 /* ---- W2: execution webhook deliveries built and signed in one call: determineWebhookEvent + buildPayload + json.Marshal +
  * generateWebhookSignature (internal/services/webhook_dispatcher.go:294-320, 394-474) for n deliveries.  For delivery i:
  *   bodies[body_off[i] .. body_off[i+1])   the request body json.Marshal(types.ExecutionWebhookPayload), the result member being

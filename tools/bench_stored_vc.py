@@ -7,6 +7,7 @@ in the same run.  The audit_stored block does the same for the audit of stored e
 documents in three client spellings (afc_vc_verify_json_batch_dev) next to the stored-verify call on the canonical form.  The
 issue_execution block measures execution credentials issued in one call (afc_vc_issue_execution_batch[_dev]).  The webhook block
 measures webhook deliveries built and signed in one call (afc_webhook_sign_batch[_dev]) next to HMAC alone over the same bodies.
+The issue_workflow block measures workflow credentials issued in one call (afc_vc_issue_workflow_batch[_dev]) next to the host-built path.
 Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
@@ -456,12 +457,91 @@ def webhook_block(ctx, dev, timed):
                           "note": "every buffer pinned"}}
 
 
+def issue_workflow_block(ctx, dev, timed):
+    """Workflow credentials issued on the device (afc_vc_issue_workflow_batch): 2^16 workflows of 1-64 records each (~2^21 records) from
+    1024 issuers, ids shaped like generateVCID's vc-<nanos>, a status mix of mostly succeeded with failed, running, cancelled, timeout,
+    queued and pending records and aliases; then a skewed batch in which 1 % of the workflows hold 4096 records.  Next to them, the
+    host-built path (generate_workflow_vc_batch: documents in Python, signatures in one GPU batch) on 2000 of the workflows, whose documents
+    must equal the device's byte for byte, and the host-buffer call from unpinned numpy arrays.  Every device document is verified
+    (afc_vc_verify_stored_batch) before timing."""
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import services
+    from agentfield_b200.identity import KeySet
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import workflow_cases as WC
+    n, K = 1 << 16, 1024
+    rng = np.random.default_rng(0xAF2A)
+    cache = afb.ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (8500 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    ks = KeySet([cache.public_key(d) for d in dids], ctx, dids=dids)
+
+    def measure(arrays, nw):
+        ki, cols, coff, roff, rcols, rcoff, created = arrays
+        D = (t(ki.view(np.int32)), t(cols), t(coff.view(np.int64)), t(roff.view(np.int64)), t(rcols), t(rcoff.view(np.int64)), t(created))
+        run = lambda: cache.issue_workflow_dev(*D, nw, d_expanded=d_exp)
+        d_docs, d_off, d_pv, d_state, d_summ = run()
+        d_st = torch.empty(nw, dtype=torch.uint8, device=dev)
+        ks.verify_stored_dev(afb._abi.DOC_WORKFLOW_VC, d_docs, d_off, nw, d_st)
+        torch.cuda.synchronize()
+        ok = bool((d_state == 0).all()) and bool((d_st == 1).all())
+        ms = timed(run)
+        ctx.profile_begin()
+        timed(run, reps=3)
+        kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+        m = int(roff[nw])
+        return {"workflows": nw, "records": m, "doc_bytes": int(d_off[nw]), "all_verified": ok, "ms": ms, "workflows_per_s": nw / (ms * 1e-3),
+                "records_per_s": m / (ms * 1e-3), "kernels_ms": kms}, (d_docs, d_off, d_pv)
+    arrays, case = WC.bulk(n, rng, dids, counts=rng.integers(1, 65, n))
+    main, (d_docs, d_off, d_pv) = measure(arrays, n)
+    # the host-built path on 2000 of the workflows: the same documents, built in Python, signed in one GPU batch
+    sample = rng.choice(n, 2000, replace=False)
+    svc = services.VCService(cache)
+    wfs = []
+    for i in sample.tolist():
+        c = case(i)
+        evs = [{"vc_id": r[0].decode(), "session_id": c["cols"][1].decode(), "status": r[1].decode(), "created_at": WC.time_text(r[2]),
+                "issuer_did": c["cols"][2].decode()} for r in c["records"]]
+        wfs.append({"workflow_id": c["cols"][0].decode(), "execution_vcs": evs, "root_did": dids[0], "vc_id": c["cols"][3].decode(),
+                    "workflow_vc_id": "wvc-%d" % i, "issuance_date": c["cols"][4].decode(), "snapshot_time": c["cols"][5].decode(),
+                    "proof_created": c["cols"][6].decode()})
+    t_0 = time.perf_counter()
+    mirror = svc.generate_workflow_vc_batch(wfs)
+    ms_mirror = (time.perf_counter() - t_0) * 1e3
+    docs, off = d_docs.cpu().numpy().tobytes(), d_off.cpu().numpy()
+    sample_ok = all(m["vc_document"] == docs[int(off[i]):int(off[i + 1])] for m, i in zip(mirror, sample.tolist()))
+    mrec = sum(len(w["execution_vcs"]) for w in wfs)
+    # the host-buffer call, unpinned arrays
+    hdocs, hoff, _, _, _ = cache.issue_workflow_packed(*arrays)
+    host_same = hoff[n] == off[n] and hdocs.tobytes() == docs
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        cache.issue_workflow_packed(*arrays)
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    del d_docs, d_off, d_pv, hdocs, docs
+    torch.cuda.empty_cache()
+    # skewed: 1 % of the workflows hold 4096 records
+    sk_arrays, _ = WC.bulk(n, rng, dids, counts=rng.integers(1, 65, n), skew=(0.01, 4096))
+    skewed, _ = measure(sk_arrays, n)
+    ks.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "dev_call": main, "skewed_1pct_4096": skewed,
+            "host_built": {"workflows": len(wfs), "records": mrec, "ms": ms_mirror, "workflows_per_s": len(wfs) / (ms_mirror * 1e-3),
+                           "same_documents": bool(sample_ok), "note": "generate_workflow_vc_batch: documents in Python, one GPU signing batch"},
+            "host_call": {"workflows": n, "ms": ms_host, "workflows_per_s": n / (ms_host * 1e-3), "same_as_dev": bool(host_same),
+                          "note": "unpinned numpy buffers"}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook"], default=None, help="run one block")
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow"], default=None,
+                    help="run one block")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     ctx = afb.Context(0)
@@ -475,7 +555,7 @@ def main():
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
-              "issue_execution": issue_execution_block, "webhook": webhook_block}
+              "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
