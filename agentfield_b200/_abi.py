@@ -29,6 +29,7 @@ WEBHOOK_COLUMNS = ("execution_id", "run_id", "status", "node_id", "reasoner_id",
 WEBHOOK_HAS_DURATION, WEBHOOK_HAS_ERROR_MESSAGE, WEBHOOK_HAS_SECRET = 1, 2, 4
 WEBHOOK_BUILT, WEBHOOK_HOST = 0, 1
 WEBHOOK_HEADER_CHARS = 71
+DID_CHARS, DID_PATH_SLOT, DID_KEPT = 55, 48, 1
 MERKLE_STATE_BYTES = 8 + 64 * 32
 SHA256_STATE_BYTES = 108
 
@@ -100,6 +101,10 @@ SYMBOLS = {
     "afc_webhook_bound": (C.c_uint64, [vp, vp, C.c_uint32]),
     "afc_webhook_sign_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_sign_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),
+    "afc_did_register_bound": (C.c_uint64, [vp, vp, vp, C.c_uint32, C.c_uint64]),
+    "afc_did_register_batch": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp]),
+    "afc_did_register_batch_dev": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp,
+                                             vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),
     "afc_merkle_free": (None, [vp]),
     "afc_merkle_append": (C.c_int, [vp, vp, vp, C.c_uint32, vp, u64p]),
@@ -135,6 +140,7 @@ SYMBOLS = {
     "afc_ingest_stats_get": (C.c_int, [vp, vp]),
     "afc_ingest_soak": (C.c_int, [vp, C.c_double, C.c_double, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, vp, C.POINTER(C.c_double), u64p]),
     "afc_selftest": (C.c_int, [vp, C.c_uint32]),
+    "afc_staging_find": (C.c_int, [vp, vp, C.c_uint32, u64p]),
     "afc_profile_begin": (C.c_int, [vp, C.c_int]),
     "afc_profile_end": (C.c_int, [vp, vp, C.c_int]),
     "afc_microbench": (C.c_int, [vp, C.c_int, C.c_uint32, C.POINTER(C.c_double), C.POINTER(C.c_double)]),

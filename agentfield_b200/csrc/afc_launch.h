@@ -157,6 +157,31 @@ cudaError_t vcw_proof(const uint8_t* sigs, const uint8_t* state, uint32_t n, con
                       cudaStream_t s, LaunchLog* lg);
 uint64_t vcw_literal_bytes();          // constant text of both document forms together
 
+// ---- k_didreg.cu: agent DIDs registered on the device (afc_didreg.cuh).  node_off: n + 1 absolute offsets; id_idx: 2n + 1 absolute id
+// indices (request i's reasoners [id_idx[2i], id_idx[2i+1]), skills [id_idx[2i+1], id_idx[2i+2])); id_off: absolute, indexed by absolute id.
+// The m = id_idx[2n] - id_idx[0] ids have per-id scratch; the component outputs hold n + m entries (the components, then zeros).
+struct DidrArgs {
+    const void* comb; const void* ct16;                  // ed_expand_batch's tables (ct16 nullptr: variable-time expansion)
+    const uint8_t* master;                               // 32 bytes, 16-byte aligned
+    uint32_t h;                                          // didr_server_hash of the server id
+    const uint8_t* server; uint64_t server_len;          // the server id's bytes, on the device
+    const uint8_t* nodes; const uint64_t* node_off; const uint32_t* agent_index; const uint64_t* id_idx; const uint8_t* ids; const uint64_t* id_off;
+    uint32_t n, m;
+    // outputs (expanded96, pks, paths 16-byte aligned)
+    uint64_t* comp_off; uint8_t* expanded96; uint8_t* pks; uint8_t* dids; uint8_t* paths; uint8_t* comp_flags; uint8_t* body; uint64_t* body_off;
+    // scratch: list, flags, esc, rank, before per id; nz m + 1; map_bytes, map_cnt per list; seeds 32 per slot (16-byte aligned);
+    // scan json_scan_scratch_bytes(max(n, m))
+    uint32_t* list; uint8_t* flags; uint64_t* esc; uint64_t* nz; uint32_t* rank; uint64_t* before; uint64_t* map_bytes; uint32_t* map_cnt;
+    uint8_t* seeds; uint64_t* scan;
+};
+// out: node_off[0], node_off[n], id_idx[0], id_idx[2n], id_off at both (one thread)
+cudaError_t didr_ends(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t* out, cudaStream_t s,
+                      LaunchLog* lg);
+// every pass; the seeds scratch holds the derived seeds when it has run (the caller wipes it)
+cudaError_t didr_register(const DidrArgs& A, cudaStream_t s, LaunchLog* lg);
+uint64_t didr_req_fixed();             // the body bound's constant per request and per id (afc_didreg.cuh)
+uint64_t didr_per_id_fixed();
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

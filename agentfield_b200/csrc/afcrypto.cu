@@ -1923,6 +1923,242 @@ int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* co
     return wh_host_run(ctx, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off, n, bodies, body_off, headers, status);
 }
 
+// ---------------------------------------------------------------------------------- registering agent DIDs
+// Bounds from the three offset arrays' ends alone (afc_didreg.cuh): per request its frame with two 10-digit counts, its agent's identity
+// with the longest path and 6 bytes per node-id and server-id byte; per id its map entry with the longest path and type, and 6 bytes per
+// id byte for each of its two appearances (the key, function_name).  Empty and shadowed ids write nothing, so the bound only gains there.
+static uint64_t didr_bound(uint32_t n, uint64_t node_bytes, uint64_t server_len, uint64_t m, uint64_t id_bytes) {
+    return (uint64_t)n * (launch::didr_req_fixed() + 6 * server_len) + 6 * node_bytes + m * launch::didr_per_id_fixed() + 12 * id_bytes;
+}
+
+uint64_t afc_did_register_bound(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t server_id_len) {
+    if (!node_off || !id_idx || !id_off || n == 0) return 0;
+    const uint64_t a = node_off[0], b = node_off[n], r0 = id_idx[0], r1 = id_idx[2 * (size_t)n];
+    const uint64_t nb = b >= a ? b - a : 0;
+    if (r1 < r0) return didr_bound(n, nb, server_id_len, 0, 0);
+    const uint64_t c = id_off[r0], d = id_off[r1];
+    return didr_bound(n, nb, server_id_len, r1 - r0, d >= c ? d - c : 0);
+}
+
+// per-call device scratch (launch::DidrArgs), then the server id's bytes
+static size_t didr_scratch_bytes(uint32_t n, uint32_t m, uint64_t server_len) {
+    const size_t slots = (size_t)n + m;
+    return vc_align((size_t)m * 4) + vc_align(m) + vc_align((size_t)m * 8) + vc_align(((size_t)m + 1) * 8) + vc_align((size_t)m * 4) +
+           vc_align((size_t)m * 8) + vc_align((size_t)n * 16) + vc_align((size_t)n * 8) + vc_align(slots * 32) +
+           vc_align(launch::json_scan_scratch_bytes(n > m ? n : m)) + vc_align(server_len + 16);
+}
+static uint8_t* didr_scratch(launch::DidrArgs& A, uint8_t* p, uint32_t n, uint32_t m) {
+    auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
+    A.list = (uint32_t*)take((size_t)m * 4);
+    A.flags = take(m);
+    A.esc = (uint64_t*)take((size_t)m * 8);
+    A.nz = (uint64_t*)take(((size_t)m + 1) * 8);
+    A.rank = (uint32_t*)take((size_t)m * 4);
+    A.before = (uint64_t*)take((size_t)m * 8);
+    A.map_bytes = (uint64_t*)take((size_t)n * 16);
+    A.map_cnt = (uint32_t*)take((size_t)n * 8);
+    A.seeds = take(((size_t)n + m) * 32);
+    A.scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n > m ? n : m));
+    return p;
+}
+
+int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* d_node_ids,
+                               const uint64_t* d_node_off, const uint32_t* d_agent_index, const uint64_t* d_id_idx, const uint8_t* d_ids,
+                               const uint64_t* d_id_off, uint32_t n, uint64_t* d_comp_off, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids,
+                               uint8_t* d_paths, uint8_t* d_comp_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream) {
+    if (!ctx || !d_node_off || !d_id_idx || !d_id_off || !d_comp_off || !d_body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!d_master_seed || !d_node_ids || !d_agent_index || !d_expanded96 || !d_pks || !d_dids || !d_paths || !d_comp_flags || !d_body ||
+        (server_id_len && !server_id))
+        return AFC_EINVAL;
+    if (!aligned16(d_master_seed) || !aligned16(d_expanded96) || !aligned16(d_pks) || !aligned16(d_paths)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[6];                       // the ends of the three offset arrays bound the bodies: gathered by one thread, read once
+    {
+        uint64_t* d_ends = nullptr;
+        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
+        cudaError_t e = launch::didr_ends(d_node_off, d_id_idx, d_id_off, n, d_ends, st, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(d_ends, st);
+        CK(e);
+        CK(cudaStreamSynchronize(st));
+    }
+    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] + n > 0xffffffffull) return AFC_EINVAL;
+    const uint32_t m = (uint32_t)(ends[3] - ends[2]);
+    if (ends[5] > ends[4] && !d_ids) return AFC_EINVAL;
+    if (body_cap < didr_bound(n, ends[1] - ends[0], server_id_len, m, ends[5] - ends[4])) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, didr_scratch_bytes(n, m, server_id_len), st));
+    launch::DidrArgs A{};
+    uint8_t* d_server = didr_scratch(A, scratch, n, m);
+    A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+    A.master = d_master_seed; A.h = did_hash(server_id, server_id_len) & 0x7fffffffu; A.server = d_server; A.server_len = server_id_len;
+    A.nodes = d_node_ids; A.node_off = d_node_off; A.agent_index = d_agent_index; A.id_idx = d_id_idx; A.ids = d_ids; A.id_off = d_id_off;
+    A.n = n; A.m = m;
+    A.comp_off = d_comp_off; A.expanded96 = d_expanded96; A.pks = d_pks; A.dids = d_dids; A.paths = d_paths; A.comp_flags = d_comp_flags;
+    A.body = d_body; A.body_off = d_body_off;
+    cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
+    if (e == cudaSuccess) e = launch::didr_register(A, st, lc);
+    const cudaError_t wipe = cudaMemsetAsync(A.seeds, 0, ((size_t)n + m) * 32, st);       // derived seeds do not outlive the call
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    CK(wipe);
+    return AFC_OK;
+}
+
+// Device bytes one chunk stages (didr_host_run's reservation, to within alignment): inputs, per component its outputs (96 + 32 + 55 + 48 + 1)
+// and seed, per id its scratch, and the body bound.  kChunkBytes caps this; a request over it goes alone.
+static uint64_t didr_chunk_bytes(uint32_t cnt, uint64_t nbytes, uint64_t server_len, uint64_t mc, uint64_t ibytes) {
+    return nbytes + ibytes + 64 * (uint64_t)cnt + 48 * mc + 264 * ((uint64_t)cnt + mc) + didr_bound(cnt, nbytes, server_len, mc, ibytes);
+}
+
+// The host-buffer call: chunks of whole requests through one slot of the lane, each staged, run, copied back and wiped before the next
+// (the expansion dominates, so there is little copy time to overlap).  A chunk's ids travel with it: the kernels index them by absolute id,
+// so the staged arrays are addressed from a shifted base.  A request larger than a chunk's byte budget goes alone.
+// Secrets in the slot: the staged master seed (device and its pinned bounce), the expanded keys, the seeds and the bodies (every private
+// JWK).  They are wiped after each chunk's copy-back and, on any early return, by the guard below, after the lane has drained.
+int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* node_ids,
+                           const uint64_t* node_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint8_t* ids, const uint64_t* id_off,
+                           uint32_t n, uint64_t* comp_off, uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* comp_flags,
+                           uint8_t* body, uint64_t body_cap, uint64_t* body_off) {
+    if (!ctx || !node_off || !id_idx || !id_off || !comp_off || !body_off) return AFC_EINVAL;
+    if (n == 0) { comp_off[0] = 0; body_off[0] = 0; return AFC_OK; }
+    if (!master_seed || !node_ids || !agent_index || !expanded96 || !pks || !dids || !paths || !comp_flags || !body || (server_id_len && !server_id))
+        return AFC_EINVAL;
+    if (!monotone(node_off, n) || !monotone(id_idx, 2 * n)) return AFC_EINVAL;
+    const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n];
+    if (r_last - r_first + n > 0xffffffffull) return AFC_EINVAL;
+    uint64_t bad = 0;
+    for (uint64_t k = r_first; k < r_last; k++) bad |= (uint64_t)(id_off[k + 1] < id_off[k]);
+    if (bad || (id_off[r_last] > id_off[r_first] && !ids)) return AFC_EINVAL;
+    if (body_cap < afc_did_register_bound(node_off, id_idx, id_off, n, server_id_len)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    LaneGuard lg(ctx);
+    Lane& lane = lg.lane();
+    Slot& sl = lane.slot[0];
+    struct StagedSecrets {
+        Slot& sl;
+        uint8_t* dev[4] = {};
+        size_t dev_bytes[4] = {};
+        uint8_t* host = nullptr;
+        size_t host_bytes = 0;
+        cudaError_t wipe() {
+            cudaError_t e = cudaSuccess;
+            for (int k = 0; k < 4; k++) {
+                if (!dev_bytes[k]) continue;
+                const cudaError_t w = cudaMemsetAsync(dev[k], 0, dev_bytes[k], sl.stream);
+                if (e == cudaSuccess) e = w;
+                dev_bytes[k] = 0;
+            }
+            const cudaError_t w = cudaStreamSynchronize(sl.stream);
+            if (e == cudaSuccess) e = w;
+            if (host_bytes) { memset(host, 0, host_bytes); host_bytes = 0; }     // after the sync: no copy still reads it
+            return e;
+        }
+        ~StagedSecrets() { wipe(); }                      // runs after LaneDrain (declared before it)
+    } secrets{sl};
+    LaneDrain drain_on_exit(lane);
+    CallLog lc(ctx);
+    const bool pin_nodes = is_pinned(node_ids), pin_ids = ids && is_pinned(ids), pin_ioff = is_pinned(id_off);
+    const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
+    const uint32_t max_chunk = max_chunk_items();
+    const uint64_t total_slots = (uint64_t)n + (r_last - r_first);
+    uint32_t i0 = 0;
+    uint64_t cbase = 0, bbase = 0;
+    while (i0 < n) {
+        const uint64_t nb0 = node_off[i0], r0 = id_idx[2 * (size_t)i0], ib0 = id_off[r0];
+        uint32_t i1 = i0;
+        while (i1 < n && i1 - i0 < max_chunk) {
+            const uint64_t r = id_idx[2 * (size_t)i1 + 2];
+            const uint64_t bytes = didr_chunk_bytes(i1 + 1 - i0, node_off[i1 + 1] - nb0, server_id_len, r - r0, id_off[r] - ib0);
+            if (bytes > kChunkBytes && i1 != i0) break;
+            i1++;
+        }
+        const uint32_t cnt = i1 - i0;
+        const uint64_t r1 = id_idx[2 * (size_t)i1];
+        const uint32_t mc = (uint32_t)(r1 - r0);
+        const size_t slots = (size_t)cnt + mc;
+        const uint64_t nbytes = node_off[i1] - nb0, ibytes = id_off[r1] - ib0;
+        const uint64_t dbound = didr_bound(cnt, nbytes, server_id_len, mc, ibytes);
+        const size_t sz[] = {nbytes + 32, ((size_t)cnt + 1) * 8, (size_t)cnt * 4, ((size_t)2 * cnt + 1) * 8, ibytes + 32, ((size_t)mc + 1) * 8, 32,
+                             ((size_t)cnt + 1) * 8, slots * 96, slots * 32, slots * AFC_DID_CHARS, slots * AFC_DID_PATH_SLOT, slots, dbound + 64,
+                             ((size_t)cnt + 1) * 8, didr_scratch_bytes(cnt, mc, server_id_len)};
+        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
+        size_t total = 0;
+        for (size_t b : sz) total += vc_align(b);
+        CK(sl.vc.reserve(total));
+        uint8_t* q[NB];
+        {
+            uint8_t* p = sl.vc.p;
+            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
+        }
+        CK(sl.h_in.reserve(vc_align(nbytes) + vc_align(ibytes) + vc_align(((size_t)mc + 1) * 8) + vc_align(sz[1]) + vc_align(sz[2]) + vc_align(sz[3]) +
+                           vc_align(32) + vc_align(server_id_len) + 256, ctx));
+        CK(sl.h_out2.reserve(16, ctx));
+        size_t used = 0;
+        launch::DidrArgs A{};
+        uint8_t* d_server = didr_scratch(A, q[15], cnt, mc);
+        A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+        A.master = q[6]; A.h = h; A.server = d_server; A.server_len = server_id_len;
+        A.nodes = q[0] + (nb0 & 15) - nb0;                        // absolute offsets stay valid, alignment as in the caller's buffer
+        A.node_off = (const uint64_t*)q[1];
+        A.agent_index = (const uint32_t*)q[2];
+        A.id_idx = (const uint64_t*)q[3];
+        A.ids = q[4] + (ib0 & 15) - ib0;
+        A.id_off = (const uint64_t*)q[5] - r0;                    // absolute id indices stay valid
+        A.n = cnt; A.m = mc;
+        A.comp_off = (uint64_t*)q[7]; A.expanded96 = q[8]; A.pks = q[9]; A.dids = q[10]; A.paths = q[11]; A.comp_flags = q[12];
+        A.body = q[13]; A.body_off = (uint64_t*)q[14];
+        CK(h2d(sl, q[0] + (nb0 & 15), node_ids + nb0, nbytes, pin_nodes, &used));
+        CK(h2d(sl, q[1], node_off + i0, sz[1], false, &used));
+        CK(h2d(sl, q[2], agent_index + i0, sz[2], false, &used));
+        CK(h2d(sl, q[3], id_idx + 2 * (size_t)i0, sz[3], false, &used));
+        if (ibytes) CK(h2d(sl, q[4] + (ib0 & 15), ids + ib0, ibytes, pin_ids, &used));
+        CK(h2d(sl, q[5], id_off + r0, sz[5], pin_ioff, &used));
+        secrets.dev[0] = q[6]; secrets.dev_bytes[0] = 32;
+        secrets.dev[1] = q[8]; secrets.dev_bytes[1] = slots * 96;
+        secrets.dev[2] = A.seeds; secrets.dev_bytes[2] = slots * 32;
+        secrets.dev[3] = q[13]; secrets.dev_bytes[3] = dbound + 64;
+        secrets.host = sl.h_in.p + used; secrets.host_bytes = 32;     // where h2d bounces the master seed
+        CK(h2d(sl, q[6], master_seed, 32, false, &used));
+        CK(h2d(sl, d_server, server_id, server_id_len, false, &used));
+        cudaError_t e = launch::didr_register(A, sl.stream, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(sl.h_out2.p, A.comp_off + cnt, 8, cudaMemcpyDeviceToHost, sl.stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(sl.h_out2.p + 8, A.body_off + cnt, 8, cudaMemcpyDeviceToHost, sl.stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(sl.stream);
+        uint64_t cc = 0, bb = 0;
+        if (e == cudaSuccess) { memcpy(&cc, sl.h_out2.p, 8); memcpy(&bb, sl.h_out2.p + 8, 8); }
+        auto d2h = [&](void* dst, const void* src, size_t bytes) {
+            if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, sl.stream);
+        };
+        d2h(comp_off + i0, A.comp_off, ((size_t)cnt + 1) * 8);
+        d2h(expanded96 + 96 * cbase, A.expanded96, cc * 96);
+        d2h(pks + 32 * cbase, A.pks, cc * 32);
+        d2h(dids + AFC_DID_CHARS * cbase, A.dids, cc * AFC_DID_CHARS);
+        d2h(paths + AFC_DID_PATH_SLOT * cbase, A.paths, cc * AFC_DID_PATH_SLOT);
+        d2h(comp_flags + cbase, A.comp_flags, cc);
+        d2h(body + bbase, A.body, bb);
+        d2h(body_off + i0, A.body_off, ((size_t)cnt + 1) * 8);
+        // the staged master seed, expanded keys, seeds and bodies are wiped whatever happened above
+        const cudaError_t w = secrets.wipe();
+        CK(e); CK(w);
+        for (uint32_t k = 0; k <= cnt; k++) { comp_off[i0 + k] += cbase; body_off[i0 + k] += bbase; }
+        cbase += cc;
+        bbase += bb;
+        i0 = i1;
+    }
+    const size_t tail = (size_t)(total_slots - cbase);            // the empty ids' entries: zeros, as the _dev call leaves them
+    memset(expanded96 + 96 * cbase, 0, tail * 96);
+    memset(pks + 32 * cbase, 0, tail * 32);
+    memset(dids + AFC_DID_CHARS * cbase, 0, tail * AFC_DID_CHARS);
+    memset(paths + AFC_DID_PATH_SLOT * cbase, 0, tail * AFC_DID_PATH_SLOT);
+    memset(comp_flags + cbase, 0, tail);
+    drain_on_exit.armed = false;
+    return AFC_OK;
+}
+
 // ---------------------------------------------------------------------------------- Merkle log
 int afc_merkle_new(afc_ctx* ctx, afc_merkle** out) {
     if (!ctx || !out) return AFC_EINVAL;
@@ -2402,6 +2638,61 @@ int afc_profile_end(afc_ctx* ctx, afc_profile_entry* out, int cap) {
 }
 
 // ---------------------------------------------------------------------------------- diagnostics
+// Counts the occurrences of a byte pattern in every lane's staging memory (device slot buffers and pinned bounce buffers), with every
+// lane held so that no call runs meanwhile: what a test uses to check that no secret outlives a host-buffer call.
+int afc_staging_find(afc_ctx* ctx, const uint8_t* pattern, uint32_t len, uint64_t* hits) {
+    if (!ctx || !pattern || !hits || len == 0 || len > 64) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    {
+        std::unique_lock<std::mutex> lk(ctx->mu);
+        for (;;) {
+            bool idle = true;
+            for (int i = 0; i < kLanes; i++) idle = idle && !ctx->lanes[i].busy;
+            if (idle) break;
+            ctx->cv.wait(lk);
+        }
+        for (int i = 0; i < kLanes; i++) ctx->lanes[i].busy = true;
+    }
+    struct Release {
+        afc_ctx* ctx;
+        ~Release() {
+            { std::lock_guard<std::mutex> g(ctx->mu); for (int i = 0; i < kLanes; i++) ctx->lanes[i].busy = false; }
+            ctx->cv.notify_all();
+        }
+    } release{ctx};
+    uint64_t count = 0;
+    auto scan = [&](const uint8_t* p, size_t n) {
+        for (const uint8_t* q = p; n >= len;) {
+            const uint8_t* f = (const uint8_t*)memchr(q, pattern[0], n - len + 1);
+            if (!f) break;
+            if (memcmp(f, pattern, len) == 0) count++;
+            n -= (size_t)(f + 1 - q);
+            q = f + 1;
+        }
+    };
+    constexpr size_t kPiece = 64u << 20;
+    std::vector<uint8_t> host;
+    for (int i = 0; i < kLanes; i++) {
+        for (int w = 0; w < kSlots; w++) {
+            Slot& sl = ctx->lanes[i].slot[w];
+            if (sl.stream) CK(cudaStreamSynchronize(sl.stream));
+            DevBuf* dev[] = {&sl.msgs, &sl.off, &sl.a, &sl.b, &sl.k, &sl.out, &sl.koff, &sl.vc};
+            for (DevBuf* d : dev) {
+                for (size_t at = 0; at < d->cap; at += kPiece) {      // pieces overlap by len - 1 bytes, so no match is cut in two
+                    const size_t n = d->cap - at < kPiece + len - 1 ? d->cap - at : kPiece + len - 1;
+                    host.resize(n);
+                    CK(cudaMemcpy(host.data(), d->p + at, n, cudaMemcpyDeviceToHost));
+                    scan(host.data(), n);
+                }
+            }
+            PinBuf* pin[] = {&sl.h_in, &sl.h_out, &sl.h_out2};
+            for (PinBuf* b : pin) if (b->p) scan(b->p, b->cap);
+        }
+    }
+    *hits = count;
+    return AFC_OK;
+}
+
 int afc_selftest(afc_ctx* ctx, uint32_t iters) {
     if (!ctx) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));

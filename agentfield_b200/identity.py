@@ -269,6 +269,120 @@ class ExpandedKeys:
         return [{"vc_document": buf[int(off[i]):int(off[i + 1])], "signature": pv[i].tobytes().decode() if state[i] == _abi.WORKFLOW_BUILT else "",
                  "state": int(state[i]), "summary": [int(x) for x in summ[i]]} for i in range(n)]
 
+    # -- agent DID registration (afc_did_register_batch)
+    def _append(self, expanded, dids):
+        base = self._expanded.shape[0]
+        self._expanded = np.concatenate([self._expanded, expanded])
+        for i, d in enumerate(dids):
+            self._index[d] = base + i
+
+    @staticmethod
+    def pack_register_requests(requests):
+        """DIDRegistrationRequests ({"agent_node_id", "reasoners": [ids], "skills": [ids]}; str or bytes, str as UTF-8 with lone surrogates
+        kept as their three bytes) -> the host arrays of afc_did_register_batch: (node_ids, node_off, id_idx, ids, id_off)."""
+        def b(v):
+            return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+        flat, idx = [], [0]
+        for r in requests:
+            flat += [b(x) for x in r.get("reasoners") or ()]
+            idx.append(len(flat))
+            flat += [b(x) for x in r.get("skills") or ()]
+            idx.append(len(flat))
+        nodes, node_off = pack([b(r["agent_node_id"]) for r in requests])
+        ids, id_off = pack(flat)
+        return nodes, node_off, np.array(idx, dtype=np.uint64), ids, id_off
+
+    def register_packed(self, master_seed, server_id, node_ids, node_off, agent_index, id_idx, ids, id_off, append=True):
+        """afc_did_register_batch on host arrays (the layout of pack_register_requests; agent_index uint32 [n]).  Returns a dict: comp_off
+        uint64 [n+1], expanded uint8 [C, 96], pks [C, 32], dids [C, 55], paths [C, 48], flags uint8 [C] (_abi.DID_KEPT), body uint8,
+        body_off uint64 [n+1], for the C = comp_off[n] components.  With append the expanded keys join this cache under their DIDs."""
+        n = len(agent_index)
+        sid = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
+        if len(master_seed) != 32:
+            raise ValueError("the master seed is 32 bytes")
+        lib = _abi.load()
+        m = int(id_idx[2 * n]) - int(id_idx[0]) if n else 0
+        S = n + m
+        cap = lib.afc_did_register_bound(_abi.ptr(node_off), _abi.ptr(id_idx), _abi.ptr(id_off), n, len(sid))
+        out = {"comp_off": np.zeros(n + 1, dtype=np.uint64), "expanded": np.empty((S, 96), dtype=np.uint8), "pks": np.empty((S, 32), dtype=np.uint8),
+               "dids": np.empty((S, _abi.DID_CHARS), dtype=np.uint8), "paths": np.empty((S, _abi.DID_PATH_SLOT), dtype=np.uint8),
+               "flags": np.empty(S, dtype=np.uint8), "body": np.empty(max(cap, 1), dtype=np.uint8), "body_off": np.zeros(n + 1, dtype=np.uint64)}
+        ms = np.frombuffer(bytes(master_seed), dtype=np.uint8).copy()
+        ai = np.ascontiguousarray(agent_index, dtype=np.uint32)
+        _abi.check(lib.afc_did_register_batch(self.ctx.handle, _abi.ptr(ms), sid, len(sid), _abi.ptr(node_ids), _abi.ptr(node_off), _abi.ptr(ai),
+                                              _abi.ptr(id_idx), _abi.ptr(ids), _abi.ptr(id_off), n, _abi.ptr(out["comp_off"]), _abi.ptr(out["expanded"]),
+                                              _abi.ptr(out["pks"]), _abi.ptr(out["dids"]), _abi.ptr(out["paths"]), _abi.ptr(out["flags"]),
+                                              _abi.ptr(out["body"]), cap, _abi.ptr(out["body_off"])), self.ctx.handle)
+        ms[:] = 0
+        C_ = int(out["comp_off"][n])
+        for k in ("expanded", "pks", "dids", "paths", "flags"):
+            out[k] = out[k][:C_]
+        out["body"] = out["body"][:int(out["body_off"][n])]
+        if append:
+            self._append(out["expanded"], [d.tobytes().decode() for d in out["dids"]])
+        return out
+
+    def register_dev(self, d_master_seed, server_id, d_node_ids, d_node_off, d_agent_index, d_id_idx, d_ids, d_id_off, n, stream=None, append=True):
+        """afc_did_register_batch_dev: n requests on the device (int64 offset arrays, int32 agent indices, a 32-byte uint8 master seed).
+        Returns a dict of device tensors as register_packed returns arrays, each cut to the C components (comp_off, body_off int64).  With
+        append the expanded keys are copied into this cache under their DIDs."""
+        import torch
+        dev = d_node_off.device
+        sid = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
+        lib = _abi.load()
+        if n:
+            r0, r1 = int(d_id_idx[0]), int(d_id_idx[2 * n])
+            m = r1 - r0
+            node_bytes = int(d_node_off[n]) - int(d_node_off[0])
+            ends = np.array([0, node_bytes], dtype=np.uint64)
+            idx = np.array([0, 0, m], dtype=np.uint64)
+            off = np.zeros(m + 1, dtype=np.uint64)
+            off[m] = int(d_id_off[r1]) - int(d_id_off[r0])
+            cap = lib.afc_did_register_bound(_abi.ptr(ends), _abi.ptr(idx), _abi.ptr(off), 1, len(sid))
+            cap += (n - 1) * lib.afc_did_register_bound(_abi.ptr(np.zeros(2, dtype=np.uint64)), _abi.ptr(np.zeros(3, dtype=np.uint64)),
+                                                        _abi.ptr(np.zeros(1, dtype=np.uint64)), 1, len(sid))
+        else:
+            m, cap = 0, 0
+        S = n + m
+        out = {"comp_off": torch.zeros(n + 1, dtype=torch.int64, device=dev), "expanded": torch.empty((S, 96), dtype=torch.uint8, device=dev),
+               "pks": torch.empty((S, 32), dtype=torch.uint8, device=dev), "dids": torch.empty((S, _abi.DID_CHARS), dtype=torch.uint8, device=dev),
+               "paths": torch.empty((S, _abi.DID_PATH_SLOT), dtype=torch.uint8, device=dev), "flags": torch.empty(S, dtype=torch.uint8, device=dev),
+               "body": torch.empty(max(cap, 1), dtype=torch.uint8, device=dev), "body_off": torch.zeros(n + 1, dtype=torch.int64, device=dev)}
+        _abi.check(lib.afc_did_register_batch_dev(self.ctx.handle, _abi.ptr(d_master_seed), sid, len(sid), _abi.ptr(d_node_ids), _abi.ptr(d_node_off),
+                                                  _abi.ptr(d_agent_index), _abi.ptr(d_id_idx), _abi.ptr(d_ids), _abi.ptr(d_id_off), n,
+                                                  _abi.ptr(out["comp_off"]), _abi.ptr(out["expanded"]), _abi.ptr(out["pks"]), _abi.ptr(out["dids"]),
+                                                  _abi.ptr(out["paths"]), _abi.ptr(out["flags"]), _abi.ptr(out["body"]), cap, _abi.ptr(out["body_off"]),
+                                                  self.ctx._stream(stream)), self.ctx.handle)
+        if n:
+            C_ = int(out["comp_off"][n])
+            for k in ("expanded", "pks", "dids", "paths", "flags"):
+                out[k] = out[k][:C_]
+            out["body"] = out["body"][:int(out["body_off"][n])]
+        if append and n:
+            self._append(out["expanded"].cpu().numpy(), [d.tobytes().decode() for d in out["dids"].cpu().numpy()])
+        return out
+
+    def register(self, master_seed, server_id, requests, agent_base):
+        """handleNewRegistration for many new agents in one host-buffer call; request k gets agent index agent_base + k.  Returns per
+        request {"body": the DIDRegistrationResponse bytes, "components": [{"did", "pk", "path", "type", "id", "kept"}]} (agent first,
+        then the non-empty reasoner ids, then the non-empty skill ids, in request order)."""
+        n = len(requests)
+        if n == 0:
+            return []
+        nodes, node_off, id_idx, ids, id_off = self.pack_register_requests(requests)
+        ai = np.arange(agent_base, agent_base + n, dtype=np.uint64).astype(np.uint32)
+        R = self.register_packed(master_seed, server_id, nodes, node_off, ai, id_idx, ids, id_off)
+        body = R["body"].tobytes()
+        out = []
+        for i, r in enumerate(requests):
+            c0, c1 = int(R["comp_off"][i]), int(R["comp_off"][i + 1])
+            kinds = [("agent", r["agent_node_id"])] + [("reasoner", x) for x in r.get("reasoners") or () if len(x)] + \
+                    [("skill", x) for x in r.get("skills") or () if len(x)]
+            comps = [{"did": R["dids"][c].tobytes().decode(), "pk": R["pks"][c].tobytes(), "path": R["paths"][c].tobytes().rstrip(b"\0").decode(),
+                      "type": t, "id": x, "kept": bool(R["flags"][c] & _abi.DID_KEPT)} for c, (t, x) in zip(range(c0, c1), kinds)]
+            out.append({"body": body[int(R["body_off"][i]):int(R["body_off"][i + 1])], "components": comps})
+        return out
+
 
 _EPOCH = datetime.datetime(1970, 1, 1, tzinfo=datetime.timezone.utc)
 

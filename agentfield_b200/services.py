@@ -862,3 +862,56 @@ def _is_rfc3339(ts: str) -> bool:
         return False
     import calendar
     return d <= calendar.monthrange(int(m.group(1)), mo)[1]
+
+
+class DIDService:
+    """The registration half of the reference's DIDService (control-plane/internal/services/did_service.go:186-365, 653-723) over one
+    registry: its server id, master seed and agent nodes.  Every new agent's keys, DIDs and DIDRegistrationResponse come from one
+    afc_did_register_batch call (ExpandedKeys.register), and the keys join `keys`, so the agents can issue credentials at once.
+    PartialRegisterAgent (new components of a known agent) is not mirrored."""
+
+    def __init__(self, keys: ExpandedKeys, master_seed: bytes, server_id):
+        if len(master_seed) != 32:
+            raise ValueError("the master seed is 32 bytes")
+        self.keys = keys
+        self.master_seed = bytes(master_seed)
+        self.server_id = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
+        self.agent_nodes = {}     # node id (bytes) -> {"did", "derivation_path", "reasoners": {id: did}, "skills": {id: did}}
+
+    @staticmethod
+    def _node_key(v):
+        return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+
+    def _register(self, requests):
+        results = self.keys.register(self.master_seed, self.server_id, requests, len(self.agent_nodes))
+        for r, res in zip(requests, results):
+            comps = res["components"]
+            entry = {"did": comps[0]["did"], "derivation_path": comps[0]["path"], "reasoners": {}, "skills": {}}
+            for c in comps[1:]:
+                if c["kept"]:
+                    entry["reasoners" if c["type"] == "reasoner" else "skills"][self._node_key(c["id"])] = c["did"]
+            self.agent_nodes[self._node_key(r["agent_node_id"])] = entry
+        return results
+
+    def register_agents_batch(self, requests):
+        """handleNewRegistration for new agents, in order (request k gets agent index len(registry) + k).  A node id already registered,
+        or repeated in the batch, raises ValueError: that is PartialRegisterAgent's case.  Returns per request {"body", "components"}."""
+        seen = set()
+        for r in requests:
+            k = self._node_key(r["agent_node_id"])
+            if k in self.agent_nodes or k in seen:
+                raise ValueError("agent node %r is already registered" % k)
+            seen.add(k)
+        return self._register(requests)
+
+    def backfill_existing_nodes(self, nodes):
+        """BackfillExistingNodes: every node ({"agent_node_id", "reasoners", "skills"}) the registry lacks is registered, in list order,
+        in one call; registered nodes (and later repeats of a node) are skipped.  Returns the new nodes' results."""
+        todo, seen = [], set()
+        for r in nodes:
+            k = self._node_key(r["agent_node_id"])
+            if k in self.agent_nodes or k in seen:
+                continue
+            seen.add(k)
+            todo.append(r)
+        return self._register(todo) if todo else []

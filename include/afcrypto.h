@@ -438,6 +438,49 @@ int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64
                                uint32_t n, uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_headers, uint8_t* d_status,
                                void* stream);
 
+/* ---- K1/K2: agent DIDs registered in one call: handleNewRegistration (internal/services/did_service.go:186-365) for n new agents.
+ * For request i, its components are comp_off[i] .. comp_off[i+1]: the agent, then its non-empty reasoner ids in request order, then its
+ * non-empty skill ids.  Paths: agent m/44'/<h>'/<a>', reasoner m/44'/<h>'/<a>'/0'/<j>', skill m/44'/<h>'/<a>'/1'/<j>', where h =
+ * FNV-1a 32(server_id) mod 2^31, a = agent_index[i] and j counts the non-empty ids before this one in its list.  Component c:
+ *   expanded96[96 c ..]   ed25519.NewKeyFromSeed(SHA-256(master_seed || path)) as afc_ed25519_expand_batch writes it (s || prefix || pk),
+ *                         ready for afc_ed25519_sign_expanded* and both issue calls
+ *   pks[32 c ..]          the public key
+ *   dids[55 c ..]         did:key:z + base64url(0xED 0x01 || pk)
+ *   paths[48 c ..]        the derivation path, NUL-padded (at most 44 bytes)
+ *   comp_flags[c]         AFC_DID_KEPT: in the identity package (and the registry); clear for an id repeated later in its list, whose
+ *                         later occurrence the map keeps
+ * and body[body_off[i] .. body_off[i+1]) is json.Marshal(types.DIDRegistrationResponse), the bytes the registration handler writes: every
+ * kept component's identity with its private and public JWK, maps keyed by the raw ids in byte order, the server id and the message.
+ * Inputs:
+ *   master_seed              the registry's 32-byte master seed (a device pointer in the _dev call, 16-byte aligned)
+ *   server_id / _len         the server id (a host pointer in both calls)
+ *   node_ids / node_off      each request's agent_node_id, n + 1 absolute offsets
+ *   agent_index              n values: len(registry.AgentNodes) when the request is handled (the caller keeps the registry)
+ *   id_idx                   2n + 1 absolute id indices: request i's reasoner ids are [id_idx[2i], id_idx[2i+1]), its skill ids
+ *                            [id_idx[2i+1], id_idx[2i+2]); id k is ids[id_off[k] .. id_off[k+1])
+ * The component outputs hold n + m entries, m = id_idx[2n] - id_idx[0]: the comp_off[n] components, then zeros.  body_cap must be at
+ * least afc_did_register_bound(node_off, id_idx, id_off, n, server_id_len), computed from the ends of the three offset arrays and additive
+ * over requests (else AFC_EINVAL, before any work).  Other AFC_EINVAL: a NULL pointer, more than 2^32 - 1 components; in the host-buffer call
+ * also offsets that run backwards.  The host-buffer call runs chunks of whole requests, one after another, through one of the context's
+ * staging slots (a request bigger than a chunk's budget goes alone) and wipes every secret it staged there, the master seed and the
+ * bodies included, whatever the outcome.  The _dev call synchronises `stream` once, to read the ends of the offset arrays; expanded96, pks and
+ * paths must be 16-byte aligned there.  Derived seeds and expanded keys are wiped from every device scratch area before either call returns:
+ * the caller's outputs are the only place they remain.  The expansion is constant time unless afc_sign_configure says otherwise.  n = 0
+ * writes comp_off[0] = body_off[0] = 0 in the host-buffer call and nothing in the _dev call. */
+#define AFC_DID_CHARS 55
+#define AFC_DID_PATH_SLOT 48
+#define AFC_DID_KEPT 1
+uint64_t afc_did_register_bound(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t server_id_len);
+int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed /* 32 */, const uint8_t* server_id, uint64_t server_id_len,
+                           const uint8_t* node_ids, const uint64_t* node_off /* n+1 */, const uint32_t* agent_index /* n */,
+                           const uint64_t* id_idx /* 2n+1 */, const uint8_t* ids, const uint64_t* id_off, uint32_t n, uint64_t* comp_off /* n+1 */,
+                           uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* comp_flags, uint8_t* body, uint64_t body_cap,
+                           uint64_t* body_off /* n+1 */);
+int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* d_node_ids,
+                               const uint64_t* d_node_off, const uint32_t* d_agent_index, const uint64_t* d_id_idx, const uint8_t* d_ids,
+                               const uint64_t* d_id_off, uint32_t n, uint64_t* d_comp_off, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids,
+                               uint8_t* d_paths, uint8_t* d_comp_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream);
+
 /* ---- N4: audit proofs for bulk offline verification (`af vc verify`, internal/cli/vc.go:159-331; export bundles,
  * internal/handlers/ui/did.go:533-865) ------------------------------------------------------------------------
  * afc_merkle_tree materialises every level over a fixed set of leaf hashes (device memory, ~2n x 32 B) so that RFC 6962
@@ -528,6 +571,10 @@ int afc_ingest_soak(afc_ingest* g, double rate_per_s, double seconds, uint32_t p
  * afc_microbench: register-only throughput of a primitive; which = 0 fe_mul, 1 fe_sq, 2 fe_add,
  * 3 sha256 compress, 4 sha512 compress; returns primitive-ops per second (whole GPU) in *ops_per_s. */
 int afc_selftest(afc_ctx* ctx, uint32_t iters);
+/* afc_staging_find: counts the occurrences of pattern (1..64 bytes) in the context's staging memory — every lane's device slot buffers
+ * and pinned bounce buffers — waiting until no host-buffer call is running.  For tests that check that no secret (a master seed, a derived
+ * seed, an expanded key) outlives a call. */
+int afc_staging_find(afc_ctx* ctx, const uint8_t* pattern, uint32_t len, uint64_t* hits);
 /* Per-kernel CUDA-event timing (tracing hook, SURVEY.md §5): between begin and end every kernel this ctx launches is
  * bracketed by two events on its own stream; afc_profile_end synchronises the device and returns one aggregated entry
  * per kernel name (returns the number of entries, or a negative error). */

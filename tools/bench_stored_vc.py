@@ -535,12 +535,120 @@ def issue_workflow_block(ctx, dev, timed):
                           "note": "unpinned numpy buffers"}}
 
 
+def register_requests(n, rng, skew=None):
+    """2^16-style registration requests: 0-32 reasoners and 0-32 skills with ids like summarize_text_17; 1 % repeat an id, 1 % hold ids
+    that need escaping; skew = (fraction, reasoners) gives that fraction of the requests that many reasoners."""
+    verbs = [b"summarize", b"translate", b"classify", b"extract", b"rank", b"plan"]
+    out = []
+    for i in range(n):
+        nr, ns = int(rng.integers(0, 33)), int(rng.integers(0, 33))
+        if skew and rng.random() < skew[0]:
+            nr = skew[1]
+        rs = [b"%s_text_%d" % (verbs[k % 6], k) for k in range(nr)]
+        ss = [b"%s_skill_%d" % (verbs[(k + 3) % 6], k) for k in range(ns)]
+        u = rng.random()
+        if u < 0.01 and rs:
+            rs.append(rs[0])
+        elif u < 0.02 and ss:
+            ss[0] = b"tag<\"\xe2\x80\xa8\xff>&"
+        out.append({"agent_node_id": b"agent-node-%d" % i, "reasoners": rs, "skills": ss})
+    return out
+
+
+def register_block(ctx, dev, timed):
+    """Agent DIDs registered on the device (afc_did_register_batch): 2^16 registrations with 0-32 reasoners and 0-32 skills each (~2.2 M
+    components), then a skewed batch in which 1 % of the agents have 1024 reasoners.  Next to it: the same keys through the two calls
+    ExpandedKeys.derive makes (SHA-256, then the expansion, on device buffers), the host-buffer call from pinned memory, and the CPU figure:
+    the oracle's C port of NewKeyFromSeed over the same seeds on every core."""
+    import torch
+    import agentfield_b200 as afb
+    from oracle import c_oracle as CO
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import did_cases as DC
+    n = 1 << 16
+    rng = np.random.default_rng(0xAF2B)
+    master = rng.integers(0, 256, 32, dtype=np.uint8).tobytes()
+    server = b"agentfield-server-bench"
+    cache = afb.ExpandedKeys(ctx)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
+
+    def measure(reqs):
+        nodes, node_off, id_idx, ids, id_off = DC.pack(reqs)
+        ai = np.arange(len(reqs), dtype=np.uint32)
+        D = (t(np.frombuffer(master, dtype=np.uint8).copy()), server, t(nodes), t(node_off.view(np.int64)), t(ai.view(np.int32)),
+             t(id_idx.view(np.int64)), t(ids), t(id_off.view(np.int64)), len(reqs))
+        run = lambda: cache.register_dev(*D, append=False)  # noqa: E731
+        R = run()
+        torch.cuda.synchronize()
+        C_ = int(R["comp_off"][-1])
+        ms = timed(run)
+        ctx.profile_begin()
+        timed(run, reps=3)
+        kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+        return {"registrations": len(reqs), "components": C_, "body_bytes": int(R["body_off"][-1]), "ms": ms,
+                "registrations_per_s": len(reqs) / (ms * 1e-3), "components_per_s": C_ / (ms * 1e-3), "kernels_ms": kms}, R, (nodes, node_off, ai, id_idx,
+                                                                                                                                  ids, id_off)
+    reqs = register_requests(n, rng)
+    main, R, arrays = measure(reqs)
+    C_ = main["components"]
+    # the same keys through today's two calls: SHA-256(master || path), then the expansion
+    paths = R["paths"].cpu().numpy()
+    plen = (paths != 0).sum(axis=1).astype(np.uint64)
+    msgs = np.zeros((C_, 80), dtype=np.uint8)
+    msgs[:, :32] = np.frombuffer(master, dtype=np.uint8)
+    msgs[:, 32:80] = paths
+    flat = np.concatenate([msgs[c, :32 + int(plen[c])] for c in range(C_)])
+    off = np.zeros(C_ + 1, dtype=np.uint64)
+    off[1:] = np.cumsum(32 + plen)
+    d_msgs, d_off = t(flat), t(off.view(np.int64))
+    d_seeds = torch.empty((C_, 32), dtype=torch.uint8, device=dev)
+    d_exp = torch.empty((C_, 96), dtype=torch.uint8, device=dev)
+
+    def two_calls():
+        ctx.sha256_dev(d_msgs, d_off, C_, d_seeds)
+        ctx.expand_dev(d_seeds, C_, d_exp)
+    two_calls()
+    torch.cuda.synchronize()
+    same_keys = bool((d_exp == R["expanded"]).all())
+    ms_two = timed(two_calls)
+    seeds = d_seeds.cpu().numpy()
+    del R, d_msgs, d_off, d_exp
+    torch.cuda.empty_cache()
+    # the host-buffer call from pinned memory
+    nodes, node_off, ai, id_idx, ids, id_off = arrays
+    pin = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().numpy()  # noqa: E731
+    P = [pin(a) for a in (nodes, node_off, ai, id_idx, ids, id_off)]
+    host = lambda: cache.register_packed(master, server, *P, append=False)  # noqa: E731
+    host()
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        host()
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    # the CPU figure: NewKeyFromSeed (the oracle's C port) on every core, over a 2^16 sample of the seeds
+    threads = os.cpu_count() or 1
+    cpu_n = min(C_, 1 << 16)
+    t_0 = time.perf_counter()
+    CO.ed25519_pubkey_batch(np.ascontiguousarray(seeds[:cpu_n]), nthreads=threads)
+    s_cpu = time.perf_counter() - t_0
+    torch.cuda.empty_cache()
+    skewed, _, _ = measure(register_requests(n, rng, skew=(0.01, 1024)))
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "sign_mode": ctx.sign_mode(), "dev_call": main, "skewed_1pct_1024": skewed,
+            "two_calls": {"components": C_, "ms": ms_two, "components_per_s": C_ / (ms_two * 1e-3), "same_keys": same_keys,
+                          "note": "sha256_dev + expand_dev: keys only, no DIDs, JWKs or bodies"},
+            "host_call": {"registrations": n, "ms": ms_host, "registrations_per_s": n / (ms_host * 1e-3), "components_per_s": C_ / (ms_host * 1e-3),
+                          "note": "pinned numpy buffers"},
+            "cpu_new_key_from_seed": {"keys": cpu_n, "threads": threads, "s": s_cpu, "keys_per_s": cpu_n / s_cpu}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow"], default=None,
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register"],
+                    default=None,
                     help="run one block")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
@@ -555,7 +663,7 @@ def main():
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
-              "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block}
+              "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
