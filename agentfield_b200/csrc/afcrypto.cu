@@ -69,9 +69,8 @@ struct PinBuf {
 // One stage of a lane's ring of in-flight chunks
 struct Slot {
     cudaStream_t stream = nullptr;
-    DevBuf msgs, off, a, b, k, out, koff;   // a: pks/seeds/keys  b: sigs (stored documents: their field spans)
-    DevBuf vc;                               // stored documents: signing messages, signatures, key indices, verify scratch
-    PinBuf h_in, h_out, h_out2;              // bounce buffers when the caller's memory is not pinned
+    DevBuf arena;                            // a chunk's staged inputs, outputs and scratch, carved per call
+    PinBuf h_in, h_out;                      // bounce buffers for the caller's pageable memory: inputs, outputs
 };
 struct Lane {
     Slot slot[kSlots];
@@ -170,7 +169,7 @@ void set_err(afc_ctx* ctx, cudaError_t e, const char* what) {
 struct CallLog {
     afc_ctx* ctx;
     launch::LaunchLog lg;
-    explicit CallLog(afc_ctx* c, int = 0) : ctx(c) {
+    explicit CallLog(afc_ctx* c) : ctx(c) {
         if (ctx->profile) { lg.profile = true; lg.pool = ctx->prof_recs.data(); lg.cap = (int)ctx->prof_recs.size(); lg.next = &ctx->prof_next; }
     }
     ~CallLog() { ctx->launches += lg.n; }
@@ -273,85 +272,88 @@ bool is_pinned(const void* p) {
     return at.type == cudaMemoryTypeHost;
 }
 
-// H2D of [src, src+bytes) into dst on `st`; pageable sources go through the slot's pinned bounce buffer
-// (offset `*bounce_used` within it, advanced) so the copy is truly asynchronous.
-cudaError_t h2d(Slot& sl, void* dst, const void* src, size_t bytes, bool pinned, size_t* bounce_used) {
-    if (bytes == 0) return cudaSuccess;
-    if (pinned) return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, sl.stream);
-    memcpy(sl.h_in.p + *bounce_used, src, bytes);
-    cudaError_t e = cudaMemcpyAsync(dst, sl.h_in.p + *bounce_used, bytes, cudaMemcpyHostToDevice, sl.stream);
-    *bounce_used += (bytes + 255) & ~(size_t)255;
-    return e;
-}
-
 inline bool aligned16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-enum Op { OP_SHA256, OP_HMAC, OP_VERIFY, OP_SIGN, OP_SIGN_EXP, OP_LEAF, OP_VERIFY_KEYED, OP_VC_STORED, OP_VC_AUDIT, OP_VC_JSON };
+#define RC(expr)                                                           \
+    do {                                                                   \
+        const int _rc = (expr);                                            \
+        if (_rc != AFC_OK) return _rc;                                     \
+    } while (0)
 
-struct BatchArgs {
-    Op op;
-    const uint8_t* msgs; const uint64_t* off; uint32_t n;
-    const uint8_t* a = nullptr; size_t a_item = 0;     // per-item fixed-size input (pks / seeds)
-    const uint8_t* b = nullptr; size_t b_item = 0;     // second per-item input (sigs)
-    const uint8_t* keys = nullptr; const uint32_t* koff = nullptr;   // HMAC keys
-    const uint8_t* d_expanded = nullptr; const uint32_t* key_index = nullptr;  // sign-expanded / keyed verify
-    const afc_keyset* keyset = nullptr;
-    int doc_kind = 0;                                  // stored documents
-    const uint8_t* cols = nullptr; const uint64_t* col_off = nullptr;   // audit: the records' columns (AFC_AUDIT_COLUMNS per item)
-    uint8_t* out; size_t out_item;
-    uint8_t* out2 = nullptr; size_t out2_item = 0;     // optional second per-item output
+// ---- per-call scratch layouts
+size_t vc_align(size_t x) { return (x + 255) & ~(size_t)255; }
+typedef std::vector<std::pair<uint8_t*, size_t>> Regions;
+// A layout is written once and run twice: over a Carve without a base it only adds up the 256-aligned sizes (what to reserve), over one
+// with a base it hands out the pointers in the same order.  Regions taken as secret join `secrets` when the carver keeps that list.
+struct Carve {
+    uint8_t* base = nullptr;
+    size_t used = 0;
+    Regions* secrets = nullptr;
+    uint8_t* take(size_t bytes, bool secret = false) {
+        uint8_t* p = base ? base + used : nullptr;
+        if (p && secret && secrets) secrets->push_back({p, vc_align(bytes)});
+        used += vc_align(bytes);
+        return p;
+    }
+    template <class T> T* take(size_t count, bool secret = false) { return (T*)take(count * sizeof(T), secret); }
 };
+// A _dev call's scratch: sized by the layout, allocated from the stream-ordered pool, carved by the same layout (the caller frees it)
+template <class Layout> cudaError_t pool_carve(uint8_t** scratch, cudaStream_t st, Layout&& layout) {
+    Carve m;
+    layout(m);
+    const cudaError_t e = cudaMallocAsync((void**)scratch, m.used, st);
+    if (e != cudaSuccess) return e;
+    Carve k;
+    k.base = *scratch;
+    layout(k);
+    return cudaSuccess;
+}
 
 // ---- stored credential documents: parse -> scan -> emit -> keyed verify -> fold, in one scratch area
-size_t vc_align(size_t x) { return (x + 255) & ~(size_t)255; }
-size_t vc_scratch_bytes(uint32_t n, uint64_t doc_bytes, uint32_t n_keys, bool audit = false) {
-    return vc_align(doc_bytes + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) + vc_align((size_t)n * 4) + vc_align(n) +
-           vc_align(launch::json_scan_scratch_bytes(n)) + vc_align((size_t)n * 32 + launch::ed_keyed_scratch_bytes(n_keys, n)) +
-           (audit ? vc_align(launch::vc_capture_bytes(n)) : 0);
+// The signing messages of a batch are never longer than its documents (D[0:p] plus the zero-proof text, which is no longer than the proof
+// object it replaces), so doc_bytes bounds their buffer.  k_vcj_parse / k_vcj_emit decline a message longer than its document, so the same
+// bound holds for documents in any spelling.  The audit (`audit`) also captures each document for k_vc_crosscheck.
+struct VcScratch { uint8_t* msgs; uint64_t* msg_off; uint8_t* sigs; uint32_t* kidx; uint8_t* ok; uint64_t* scan; uint32_t* kscr; uint32_t* caps; };
+void vc_scratch(Carve& k, VcScratch& s, uint32_t n, uint64_t doc_bytes, uint32_t n_keys, bool audit) {
+    s.msgs = k.take(doc_bytes + 64);
+    s.msg_off = k.take<uint64_t>((size_t)n + 1);
+    s.sigs = k.take((size_t)n * 64);
+    s.kidx = k.take<uint32_t>(n);
+    s.ok = k.take(n);
+    s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
+    s.kscr = (uint32_t*)k.take((size_t)n * 32 + launch::ed_keyed_scratch_bytes(n_keys, n));
+    s.caps = audit ? (uint32_t*)k.take(launch::vc_capture_bytes(n)) : nullptr;
 }
-// docs + doc_off[i] is document i (absolute offsets); the signing messages of a batch are never longer than its documents
-// (D[0:p] plus the zero-proof text, which is no longer than the proof object it replaces), so doc_bytes bounds their buffer.
-// With `issues` (the audit) the parse also captures each document and k_vc_crosscheck compares it with its record's columns; the
-// scratch area then needs vc_scratch_bytes(..., true).  With `json` (afc_vc_verify_json_batch) documents in any spelling are read and
-// re-marshalled by k_vcj_parse / k_vcj_emit, which decline a message longer than its document, so the same bound holds.
+// docs + doc_off[i] is document i (absolute offsets).  With `issues` (the audit) the parse also captures each document and k_vc_crosscheck
+// compares it with its record's columns; the scratch is then carved with `audit`.  With `json` (afc_vc_verify_json_batch) documents in any
+// spelling are read and re-marshalled by k_vcj_parse / k_vcj_emit.
 cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
-                              uint64_t doc_bytes, uint8_t* status, uint32_t* fields, uint8_t* scratch, cudaStream_t st, launch::LaunchLog* lg,
+                              uint8_t* status, uint32_t* fields, const VcScratch& S, cudaStream_t st, launch::LaunchLog* lg,
                               uint32_t* issues = nullptr, const uint8_t* cols = nullptr, const uint64_t* col_off = nullptr, bool json = false) {
     if (n == 0) return cudaSuccess;
-    uint8_t* p = scratch;
-    auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
-    uint8_t* msgs = take(doc_bytes + 64);
-    uint64_t* msg_off = (uint64_t*)take(((size_t)n + 1) * 8);
-    uint8_t* sigs = take((size_t)n * 64);
-    uint32_t* kidx = (uint32_t*)take((size_t)n * 4);
-    uint8_t* ok = take(n);
-    uint64_t* scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n));
-    uint32_t* kscr = (uint32_t*)take((size_t)n * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, n));
     const void* schema = ks->d_schemas + (size_t)kind * launch::vc_schema_bytes();
     const void* jschema = ks->d_vcj_schemas + (size_t)kind * launch::vcj_schema_bytes();
     cudaError_t e;
     if (json) {
-        e = launch::vcj_parse(jschema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
-                              kidx, fields, st, lg);
+        e = launch::vcj_parse(jschema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, S.msg_off + 1, S.sigs,
+                              S.kidx, fields, st, lg);
     } else if (issues) {
-        uint32_t* caps = (uint32_t*)take(launch::vc_capture_bytes(n));
-        e = launch::vc_parse_capture(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
-                                     kidx, caps, st, lg);
-        if (e == cudaSuccess) e = launch::vc_crosscheck(kind, docs, doc_off, n, caps, status, cols, col_off, issues, st, lg);
+        e = launch::vc_parse_capture(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, S.msg_off + 1, S.sigs,
+                                     S.kidx, S.caps, st, lg);
+        if (e == cudaSuccess) e = launch::vc_crosscheck(kind, docs, doc_off, n, S.caps, status, cols, col_off, issues, st, lg);
     } else {
-        e = launch::vc_parse(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, msg_off + 1, sigs,
-                             kidx, fields, st, lg);
+        e = launch::vc_parse(schema, docs, doc_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, status, S.msg_off + 1, S.sigs,
+                             S.kidx, fields, st, lg);
     }
-    if (e == cudaSuccess) e = launch::offsets_from_lengths(msg_off, n, scan, st, lg);
-    if (e == cudaSuccess) e = json ? launch::vcj_emit(jschema, docs, doc_off, n, msg_off, msgs, st, lg)
-                                   : launch::vc_emit(schema, docs, doc_off, n, msg_off, msgs, st, lg);
-    if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, kidx, sigs, msgs, msg_off, n, ok,
-                                                            kscr, kscr + (size_t)n * 8, st, lg);
-    if (e == cudaSuccess) e = launch::vc_fold(status, ok, n, st, lg);
+    if (e == cudaSuccess) e = launch::offsets_from_lengths(S.msg_off, n, S.scan, st, lg);
+    if (e == cudaSuccess) e = json ? launch::vcj_emit(jschema, docs, doc_off, n, S.msg_off, S.msgs, st, lg)
+                                   : launch::vc_emit(schema, docs, doc_off, n, S.msg_off, S.msgs, st, lg);
+    if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, S.kidx, S.sigs, S.msgs,
+                                                            S.msg_off, n, S.ok, S.kscr, S.kscr + (size_t)n * 8, st, lg);
+    if (e == cudaSuccess) e = launch::vc_fold(status, S.ok, n, st, lg);
     return e;
 }
 
-// Generic chunked pipeline for host-buffer calls: a ring of kSlots chunks in flight so the H2D of later chunks overlaps the kernels of earlier ones.
 // offsets must be non-decreasing: a caller's slip would otherwise turn into an out-of-bounds copy from its own buffer
 template <class T>
 bool monotone(const T* off, uint32_t n) {
@@ -359,13 +361,6 @@ bool monotone(const T* off, uint32_t n) {
     for (uint32_t i = 0; i < n; i++) bad |= (T)(off[i + 1] < off[i]);
     return bad == 0;
 }
-// On ANY exit of a host-buffer call — error paths included — nothing may still be reading the caller's buffers or writing its
-// results: drain every stream of the lane before it is handed to the next caller.
-struct LaneDrain {
-    Lane& lane; bool armed = true;
-    explicit LaneDrain(Lane& l) : lane(l) {}
-    ~LaneDrain() { if (armed) for (int w = 0; w < kSlots; w++) cudaStreamSynchronize(lane.slot[w].stream); }
-};
 
 // AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments (read once per process)
 uint32_t max_chunk_items() {
@@ -377,161 +372,227 @@ uint32_t min_chunk_items() {
     return v;
 }
 
-int run_host_batch(afc_ctx* ctx, const BatchArgs& A) {
-    if (A.n == 0) return AFC_OK;
-    if (A.koff && !monotone(A.koff, A.n)) return AFC_EINVAL;
-    CK(cudaSetDevice(ctx->device));
-    LaneGuard lg(ctx);
-    Lane& lane = lg.lane();
-    LaneDrain drain_on_exit(lane);
-    const bool pin_msgs = is_pinned(A.msgs), pin_off = is_pinned(A.off), pin_out = is_pinned(A.out);
-    const bool pin_a = A.a ? is_pinned(A.a) : true, pin_b = A.b ? is_pinned(A.b) : true;
-    const bool pin_keys = A.keys ? is_pinned(A.keys) : true, pin_koff = A.koff ? is_pinned(A.koff) : true;
-    const bool pin_ki = A.key_index ? is_pinned(A.key_index) : true;
-    const bool pin_out2 = A.out2 ? is_pinned(A.out2) : true;
-    const bool pin_cols = A.cols ? is_pinned(A.cols) : true, pin_coff = A.col_off ? is_pinned(A.col_off) : true;
-    const uint32_t C = AFC_AUDIT_COLUMNS;
-    CallLog lc(ctx, 12 * (int)(A.n / kChunkItems + 8) + 8);
-    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
-    uint32_t i0 = 0;
-    int which = 0;
-    struct Pending { uint32_t i0, cnt; bool active; } pend[kSlots] = {};
-    auto drain = [&](int w) -> int {
-        if (!pend[w].active) return AFC_OK;
-        Slot& sl = lane.slot[w];
-        CK(cudaStreamSynchronize(sl.stream));
-        if (!pin_out) memcpy(A.out + (size_t)pend[w].i0 * A.out_item, sl.h_out.p, (size_t)pend[w].cnt * A.out_item);
-        if (A.out2 && !pin_out2) memcpy(A.out2 + (size_t)pend[w].i0 * A.out2_item, sl.h_out2.p, (size_t)pend[w].cnt * A.out2_item);
-        if (A.op == OP_SIGN && !pin_a && sl.h_in.p) memset(sl.h_in.p, 0, sl.h_in.cap);         // nor in the pinned bounce buffer
-        pend[w].active = false;
-        return AFC_OK;
+constexpr uint64_t kBadOffsets = ~0ull;     // a chunk measure's answer when an item's offsets run backwards
+
+// An output of a chunk: `bytes` from device `src` to `arg` + `at` in the caller's memory; with `offsets`, uint64 offsets rebased by `base`
+struct Out {
+    void* arg; size_t at; const void* src; size_t bytes;
+    bool secret = false;
+    bool offsets = false; uint64_t base = 0;
+};
+Out offsets_out(uint64_t* arg, size_t first, const uint64_t* src, size_t count, uint64_t base) {
+    return {arg, first * 8, src, count * 8, false, true, base};
+}
+
+// The staging pipeline of every host-buffer call.  It holds a lane and runs the call's chunks through `depth` of its slots, so that the
+// copies of later chunks overlap the kernels of earlier ones.  A chunk's function stages its inputs and carves its scratch (stage),
+// enqueues its kernels on `st`, and names its outputs (copy_back); the ring moves the bytes, through the slot's bounce buffers when the
+// caller's memory is pageable, and wipes whatever was marked secret:
+// - its device bytes on the slot's stream once the chunk's copy-back is enqueued;
+// - its bounce bytes once the slot has been synchronised;
+// - both, after every stream of the lane has drained, on any early return.
+// On ANY exit, error paths included, nothing may still be reading the caller's buffers or writing its results: every stream the call used
+// is drained before the lane is handed to the next caller.
+class Ring {
+public:
+    // Carves a chunk's slot arena and stages its inputs: a layout runs twice, measuring then carving (Carve)
+    struct Stager : Carve {
+        Ring* r = nullptr;
+        size_t bounce = 0;                  // bytes of the input bounce buffer: measured, then filled
+        cudaError_t err = cudaSuccess;
+        // arg[first, first + count): the result is the staged copy of arg[first]
+        template <class T> T* in(const T* arg, size_t first, size_t count, bool secret = false) {
+            return (T*)r->stage_in(*this, arg, first * sizeof(T), count * sizeof(T), count * sizeof(T) + 16, 0, secret);
+        }
+        // arg[first, first + bytes), congruent mod `mod` (16, or 4 for keys) with its absolute offsets: the result + first is the first byte,
+        // so that absolute offsets stay valid and the kernels see the alignment of the caller's buffer whatever the chunking
+        uint8_t* in_at(const uint8_t* arg, uint64_t first, uint64_t bytes, unsigned mod, bool secret = false) {
+            uint8_t* p = r->stage_in(*this, arg, first, bytes, bytes + 32, first & (mod - 1), secret);
+            return p ? p - first : nullptr;
+        }
     };
-    while (i0 < A.n) {
-        uint32_t i1 = i0;
-        uint64_t base = A.off[i0];
-        // chunks taper towards the end of the call (each takes at most half of what is left, down to kMinChunkItems): what
-        // remains to be done after the last H2D copy lands — the part of a transfer-bound call that nothing overlaps — is small
-        const uint32_t left = A.n - i0;
-        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
-        if (limit < min_chunk) limit = min_chunk;
-        if (limit > max_chunk) limit = max_chunk;
-        // the walk that sizes the chunk also checks that the offsets never run backwards (no separate pass over n offsets)
-        while (i1 < A.n && (i1 - i0) < limit) {
-            if (A.off[i1 + 1] < A.off[i1]) return AFC_EINVAL;
-            if (A.col_off) for (uint32_t k = 0; k < C; k++) if (A.col_off[(size_t)i1 * C + k + 1] < A.col_off[(size_t)i1 * C + k]) return AFC_EINVAL;
-            if (A.off[i1 + 1] - base > kChunkBytes && i1 != i0) break;
-            i1++;
+
+    afc_ctx* const ctx;
+    CallLog lc;
+    uint32_t i0 = 0, cnt = 0;               // the chunk being run: items [i0, i0 + cnt)
+    cudaStream_t st = nullptr;
+
+    explicit Ring(afc_ctx* c, int depth = kSlots) : ctx(c), lc(c), lane_(c), depth_(depth) {}
+    ~Ring() {
+        if (!armed_) return;
+        Lane& lane = lane_.lane();
+        for (int w = 0; w < depth_; w++) cudaStreamSynchronize(lane.slot[w].stream);
+        for (int w = 0; w < depth_; w++) {
+            for (const auto& s : pend_[w].dev_secrets) cudaMemsetAsync(s.first, 0, s.second, lane.slot[w].stream);
+            cudaStreamSynchronize(lane.slot[w].stream);
+            for (const auto& s : pend_[w].host_secrets) memset(s.first, 0, s.second);
         }
-        uint32_t cnt = i1 - i0;
-        uint64_t mbytes = A.off[i1] - base;
-        Slot& sl = lane.slot[which];
-        int rc = drain(which);
-        if (rc != AFC_OK) return rc;
-        // size buffers
-        CK(sl.msgs.reserve(mbytes + 32));
-        CK(sl.off.reserve((size_t)(cnt + 1) * 8));
-        CK(sl.out.reserve((size_t)cnt * A.out_item + 16));
-        if (A.a) CK(sl.a.reserve((size_t)cnt * A.a_item + 16));
-        if (A.b) CK(sl.b.reserve((size_t)cnt * A.b_item + 16));
-        if (A.op == OP_VERIFY) CK(sl.k.reserve((size_t)cnt * 32));
-        if (A.op == OP_VERIFY_KEYED) CK(sl.k.reserve((size_t)cnt * 32 + launch::ed_keyed_scratch_bytes(A.keyset->n_keys, cnt)));
-        uint32_t kbase = 0; size_t kbytes = 0;
-        if (A.op == OP_HMAC) {
-            kbase = A.koff[i0]; kbytes = A.koff[i1] - kbase;
-            CK(sl.a.reserve(kbytes + 16));
-            CK(sl.koff.reserve((size_t)(cnt + 1) * 4));
-        }
-        if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index) CK(sl.koff.reserve((size_t)cnt * 4));
-        if (A.op == OP_VC_STORED || A.op == OP_VC_JSON) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys)));
-        if (A.op == OP_VC_AUDIT) CK(sl.vc.reserve(vc_scratch_bytes(cnt, mbytes, A.keyset->n_keys, true)));
-        uint64_t cbase = 0, cbytes = 0;             // audit: this chunk's columns (slot buffers a: bytes, koff: offsets)
-        if (A.col_off) {
-            cbase = A.col_off[(size_t)i0 * C]; cbytes = A.col_off[(size_t)i1 * C] - cbase;
-            CK(sl.a.reserve(cbytes + 32));
-            CK(sl.koff.reserve(((size_t)cnt * C + 1) * 8));
-        }
-        if (A.out2) CK(sl.b.reserve((size_t)cnt * A.out2_item + 16));
-        size_t bounce = 0;
-        if (!pin_msgs) bounce += (mbytes + 255) & ~(size_t)255;
-        if (!pin_off) bounce += ((size_t)(cnt + 1) * 8 + 255) & ~(size_t)255;
-        if (A.a && !pin_a) bounce += ((size_t)cnt * A.a_item + 255) & ~(size_t)255;
-        if (A.b && !pin_b) bounce += ((size_t)cnt * A.b_item + 255) & ~(size_t)255;
-        if (A.op == OP_HMAC) { if (!pin_keys) bounce += (kbytes + 255) & ~(size_t)255; if (!pin_koff) bounce += ((size_t)(cnt + 1) * 4 + 255) & ~(size_t)255; }
-        if ((A.op == OP_SIGN_EXP || A.op == OP_VERIFY_KEYED) && A.key_index && !pin_ki) bounce += ((size_t)cnt * 4 + 255) & ~(size_t)255;
-        if (A.col_off) { if (!pin_cols) bounce += (cbytes + 255) & ~(size_t)255; if (!pin_coff) bounce += (((size_t)cnt * C + 1) * 8 + 255) & ~(size_t)255; }
-        CK(sl.h_in.reserve(bounce + 256, ctx));
-        if (!pin_out) CK(sl.h_out.reserve((size_t)cnt * A.out_item, ctx));
-        if (A.out2 && !pin_out2) CK(sl.h_out2.reserve((size_t)cnt * A.out2_item, ctx));
-        size_t used = 0;
-        // keep the device copy of the messages congruent mod 16 with the absolute offsets so that the kernels see the
-        // same alignment whatever the chunking (d_base + off[i] == sl.msgs.p + pad + off[i] - base)
-        size_t pad = (size_t)(base & 15);
-        CK(h2d(sl, sl.msgs.p + pad, A.msgs + base, mbytes, pin_msgs, &used));
-        CK(h2d(sl, sl.off.p, A.off + i0, (size_t)(cnt + 1) * 8, pin_off, &used));
-        if (A.a) CK(h2d(sl, sl.a.p, A.a + (size_t)i0 * A.a_item, (size_t)cnt * A.a_item, pin_a, &used));
-        if (A.b) CK(h2d(sl, sl.b.p, A.b + (size_t)i0 * A.b_item, (size_t)cnt * A.b_item, pin_b, &used));
-        const uint8_t* d_base = sl.msgs.p + pad - base;     // absolute offsets stay valid
-        const uint64_t* d_off = (const uint64_t*)sl.off.p;
-        cudaError_t e = cudaSuccess;
-        switch (A.op) {
-        case OP_SHA256: e = launch::sha256_batch(d_base, d_off, cnt, sl.out.p, sl.stream, lc); break;
-        case OP_LEAF: e = launch::merkle_leaf_hashes(d_base, d_off, cnt, sl.out.p, sl.stream, lc); break;
-        case OP_HMAC: {
-            CK(h2d(sl, sl.a.p + (kbase & 3), A.keys + kbase, kbytes, pin_keys, &used));
-            CK(h2d(sl, sl.koff.p, A.koff + i0, (size_t)(cnt + 1) * 4, pin_koff, &used));
-            e = launch::hmac_sha256_batch(sl.a.p + (kbase & 3) - kbase, (const uint32_t*)sl.koff.p, d_base, d_off, cnt, sl.out.p, sl.stream, lc);
-            break;
-        }
-        case OP_VERIFY:
-            e = verify_with_cache(ctx, sl.a.p, sl.b.p, d_base, d_off, cnt, sl.out.p, (uint32_t*)sl.k.p, sl.stream, lc);
-            break;
-        case OP_VERIFY_KEYED: {
-            CK(h2d(sl, sl.koff.p, A.key_index + i0, (size_t)cnt * 4, pin_ki, &used));
-            e = launch::ed_verify_keyed_batch(ctx->comb, A.keyset->d_tabs, A.keyset->d_valid, A.keyset->d_pks, A.keyset->n_keys,
-                                              (const uint32_t*)sl.koff.p, sl.b.p, d_base, d_off, cnt, sl.out.p, (uint32_t*)sl.k.p,
-                                              (uint32_t*)(sl.k.p + (size_t)cnt * 32), sl.stream, lc);
-            break;
-        }
-        case OP_VC_STORED:
-        case OP_VC_JSON:
-            e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, A.out2 ? (uint32_t*)sl.b.p : nullptr, sl.vc.p,
-                                  sl.stream, lc, nullptr, nullptr, nullptr, A.op == OP_VC_JSON);
-            break;
-        case OP_VC_AUDIT: {
-            const uint8_t* d_cols = nullptr; const uint64_t* d_coff = nullptr;
-            if (A.col_off) {
-                CK(h2d(sl, sl.a.p + (cbase & 15), A.cols + cbase, cbytes, pin_cols, &used));
-                CK(h2d(sl, sl.koff.p, A.col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
-                d_cols = sl.a.p + (cbase & 15) - cbase; d_coff = (const uint64_t*)sl.koff.p;
+    }
+
+    // The chunk walk: each chunk takes at most max_chunk_items() items and, with more than one slot, at most half of what is left, down to
+    // min_chunk_items() (what remains after the last H2D copy lands, the part of a transfer-bound call that nothing overlaps, stays small);
+    // and no more items than keep measure(i0, i) — the bytes of items [i0, i] — within kChunkBytes, but always at least one.  The walk that
+    // sizes a chunk is also where its offsets are checked (measure returns kBadOffsets), so no separate pass reads them.
+    template <class Measure, class Fn> int walk(uint32_t n, Measure&& measure, Fn&& fn) {
+        const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
+        for (uint32_t a = 0, b; a < n; a = b) {
+            const uint32_t left = n - a;
+            uint32_t limit = max_chunk;
+            if (depth_ > 1) {
+                limit = left <= min_chunk ? left : (left + 1) / 2;
+                if (limit < min_chunk) limit = min_chunk;
+                if (limit > max_chunk) limit = max_chunk;
             }
-            e = vc_stored_enqueue(ctx, A.keyset, A.doc_kind, d_base, d_off, cnt, mbytes, sl.out.p, nullptr, sl.vc.p, sl.stream, lc,
-                                  (uint32_t*)sl.b.p, d_cols, d_coff);
-            break;
+            for (b = a; b < n && b - a < limit; b++) {
+                const uint64_t bytes = measure(a, b);
+                if (bytes == kBadOffsets) return AFC_EINVAL;
+                if (bytes > kChunkBytes && b != a) break;
+            }
+            RC(chunk(a, b - a, fn));
         }
-        case OP_SIGN: e = launch::ed_sign_batch(ctx->comb, afc_internal_sign_table(ctx), sl.a.p, d_base, d_off, cnt, sl.out.p, sl.stream, lc); break;
-        case OP_SIGN_EXP: {
-            const uint32_t* d_ki = nullptr;
-            if (A.key_index) { CK(h2d(sl, sl.koff.p, A.key_index + i0, (size_t)cnt * 4, pin_ki, &used)); d_ki = (const uint32_t*)sl.koff.p; }
-            e = launch::ed_sign_expanded_batch(ctx->comb, afc_internal_sign_table(ctx), A.d_expanded + (A.key_index ? 0 : (size_t)i0 * 96), 0xffffffffu, d_ki, d_base, d_off, cnt, sl.out.p, sl.stream, lc);
-            break;
-        }
-        }
-        CK(e);
-        if (A.op == OP_SIGN) CK(cudaMemsetAsync(sl.a.p, 0, (size_t)cnt * A.a_item, sl.stream));   // seeds do not stay behind in the staging slot
-        CK(cudaMemcpyAsync(pin_out ? A.out + (size_t)i0 * A.out_item : sl.h_out.p, sl.out.p, (size_t)cnt * A.out_item,
-                           cudaMemcpyDeviceToHost, sl.stream));
-        if (A.out2) CK(cudaMemcpyAsync(pin_out2 ? A.out2 + (size_t)i0 * A.out2_item : sl.h_out2.p, sl.b.p, (size_t)cnt * A.out2_item,
-                                       cudaMemcpyDeviceToHost, sl.stream));
-        pend[which] = {i0, cnt, true};
-        which = (which + 1) % kSlots;
-        i0 = i1;
+        return finish();
     }
-    for (int w = 0; w < kSlots; w++) {      // oldest first
-        int rc = drain((which + w) % kSlots);
-        if (rc != AFC_OK) return rc;
+    // all n items as one chunk
+    template <class Fn> int once(uint32_t n, Fn&& fn) {
+        RC(chunk(0, n, fn));
+        return finish();
     }
-    drain_on_exit.armed = false;            // every slot was drained above
-    return AFC_OK;
+
+    template <class Layout> int stage(Layout&& layout) {
+        Stager m;
+        m.r = this;
+        layout(m);
+        Slot& sl = slot();
+        CK(sl.arena.reserve(m.used));
+        CK(sl.h_in.reserve(m.bounce + 256, ctx));
+        Stager k;
+        k.r = this; k.base = sl.arena.p; k.secrets = &pend_[which_].dev_secrets;
+        layout(k);
+        CK(k.err);
+        return AFC_OK;
+    }
+    // reads the values at src into dst (where the chunk's outputs end): synchronises the slot's stream
+    int read(uint64_t* dst, std::initializer_list<const uint64_t*> src) {
+        Slot& sl = slot();
+        CK(sl.h_out.reserve(src.size() * 8, ctx));
+        size_t k = 0;
+        for (const uint64_t* s : src) CK(cudaMemcpyAsync(sl.h_out.p + 8 * k++, s, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        memcpy(dst, sl.h_out.p, src.size() * 8);
+        return AFC_OK;
+    }
+    // enqueues the chunk's outputs; what goes through the output bounce reaches the caller when the slot is drained
+    int copy_back(std::initializer_list<Out> outs) {
+        Slot& sl = slot();
+        Pending& p = pend_[which_];
+        size_t bounce = 0;
+        for (const Out& o : outs) if (o.bytes && (o.offsets || !pinned(o.arg))) bounce += vc_align(o.bytes);
+        CK(sl.h_out.reserve(bounce + 256, ctx));
+        uint8_t* h = sl.h_out.p;
+        for (const Out& o : outs) {
+            if (!o.bytes) continue;
+            uint8_t* dst = (uint8_t*)o.arg + o.at;
+            if (o.offsets || !pinned(o.arg)) {
+                p.back.push_back({dst, h, o.bytes, o.offsets, o.base});
+                if (o.secret) p.host_secrets.push_back({h, o.bytes});
+                dst = h;
+                h += vc_align(o.bytes);
+            }
+            CK(cudaMemcpyAsync(dst, o.src, o.bytes, cudaMemcpyDeviceToHost, st));
+        }
+        return AFC_OK;
+    }
+
+private:
+    struct Back { uint8_t* dst; const uint8_t* src; size_t bytes; bool offsets; uint64_t base; };
+    struct Pending {
+        bool active = false;
+        std::vector<Back> back;             // outputs waiting in the output bounce
+        Regions dev_secrets, host_secrets;
+    };
+    LaneGuard lane_;
+    const int depth_;
+    int which_ = 0;
+    bool armed_ = true;
+    Pending pend_[kSlots];
+    std::vector<std::pair<const void*, bool>> pinned_;      // each argument's memory type, looked up once per call
+
+    Slot& slot() { return lane_.lane().slot[which_]; }
+    bool pinned(const void* arg) {
+        for (const auto& a : pinned_) if (a.first == arg) return a.second;
+        pinned_.push_back({arg, is_pinned(arg)});
+        return pinned_.back().second;
+    }
+    uint8_t* stage_in(Stager& k, const void* arg, size_t at, size_t bytes, size_t region, size_t pad, bool secret) {
+        uint8_t* d = k.take(region, secret);
+        const bool direct = bytes == 0 || pinned(arg);
+        if (!k.base) {
+            if (!direct) k.bounce += vc_align(bytes);
+            return nullptr;
+        }
+        if (bytes == 0 || k.err != cudaSuccess) return d + pad;
+        const uint8_t* src = (const uint8_t*)arg + at;
+        if (!direct) {
+            uint8_t* h = slot().h_in.p + k.bounce;
+            memcpy(h, src, bytes);
+            if (secret) pend_[which_].host_secrets.push_back({h, bytes});
+            k.bounce += vc_align(bytes);
+            src = h;
+        }
+        k.err = cudaMemcpyAsync(d + pad, src, bytes, cudaMemcpyHostToDevice, st);
+        return d + pad;
+    }
+    template <class Fn> int chunk(uint32_t a, uint32_t n, Fn&& fn) {
+        RC(drain(which_));
+        i0 = a; cnt = n; st = slot().stream;
+        Pending& p = pend_[which_];
+        p.active = true;
+        RC(fn(*this));
+        for (const auto& s : p.dev_secrets) CK(cudaMemsetAsync(s.first, 0, s.second, st));
+        which_ = (which_ + 1) % depth_;
+        return AFC_OK;
+    }
+    int drain(int w) {
+        Pending& p = pend_[w];
+        if (!p.active) return AFC_OK;
+        CK(cudaStreamSynchronize(lane_.lane().slot[w].stream));
+        for (const Back& b : p.back) {
+            if (!b.offsets) { memcpy(b.dst, b.src, b.bytes); continue; }
+            for (size_t j = 0; j < b.bytes / 8; j++) ((uint64_t*)b.dst)[j] = b.base + ((const uint64_t*)b.src)[j];
+        }
+        for (const auto& s : p.host_secrets) memset(s.first, 0, s.second);
+        p.active = false;
+        p.back.clear(); p.dev_secrets.clear(); p.host_secrets.clear();
+        return AFC_OK;
+    }
+    int finish() {
+        for (int w = 0; w < depth_; w++) RC(drain((which_ + w) % depth_));      // oldest first
+        armed_ = false;
+        return AFC_OK;
+    }
+};
+typedef Ring::Stager Stager;
+
+// A chunk of messages and their offsets (msgs + off[i] is message i, absolute offsets), and the walk's measure over them
+struct Msgs { const uint8_t* d; const uint64_t* off; };
+Msgs stage_msgs(Stager& k, const uint8_t* msgs, const uint64_t* off, uint32_t i0, uint32_t cnt) {
+    return {k.in_at(msgs, off[i0], off[i0 + cnt] - off[i0], 16), k.in(off, i0, (size_t)cnt + 1)};
+}
+auto msg_bytes(const uint64_t* off) {
+    return [off](uint32_t i0, uint32_t i) { return off[i + 1] < off[i] ? kBadOffsets : off[i + 1] - off[i0]; };
+}
+
+// Expanded private keys for a host-buffer call: on the device once for every chunk, zeroed and freed when the call returns
+template <class Fn> int with_device_keys(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, Fn&& run) {
+    uint8_t* d_keys = nullptr;
+    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
+    const cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
+    int rc = AFC_ECUDA;
+    if (e == cudaSuccess) rc = run(d_keys);
+    else set_err(ctx, e, "cudaMemcpy(expanded keys)");
+    cudaMemset(d_keys, 0, (size_t)n_keys * 96);
+    cudaFree(d_keys);
+    return rc;
 }
 
 }  // namespace
@@ -652,8 +713,7 @@ void afc_destroy(afc_ctx* ctx) {
         for (int s = 0; s < kSlots; s++) {
             Slot& sl = ctx->lanes[l].slot[s];
             if (sl.stream) { cudaStreamSynchronize(sl.stream); cudaStreamDestroy(sl.stream); }
-            sl.msgs.release(); sl.off.release(); sl.a.release(); sl.b.release(); sl.k.release(); sl.out.release(); sl.koff.release();
-            sl.vc.release(); sl.h_in.release(); sl.h_out.release(); sl.h_out2.release();
+            sl.arena.release(); sl.h_in.release(); sl.h_out.release();
         }
     kc_free(ctx);
     if (ctx->kc_event) cudaEventDestroy(ctx->kc_event);
@@ -697,26 +757,82 @@ int afc_numa_info(afc_ctx* ctx, int* numa_node, int* local_cpus) {
 // ---------------------------------------------------------------------------------- host-buffer batch calls
 int afc_sha256_batch(afc_ctx* ctx, const uint8_t* msgs, const uint64_t* offsets, uint32_t n, uint8_t* out32) {
     if (!ctx || !offsets || (!out32 && n) || (!msgs && n && offsets[n] != offsets[0])) return AFC_EINVAL;
-    BatchArgs A{}; A.op = OP_SHA256; A.msgs = msgs; A.off = offsets; A.n = n; A.out = out32; A.out_item = 32;
-    return run_host_batch(ctx, A);
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(offsets), [&](Ring& r) {
+        Msgs M;
+        uint8_t* d_out;
+        RC(r.stage([&](Stager& k) {
+            M = stage_msgs(k, msgs, offsets, r.i0, r.cnt);
+            d_out = k.take((size_t)r.cnt * 32 + 16);
+        }));
+        CK(launch::sha256_batch(M.d, M.off, r.cnt, d_out, r.st, r.lc));
+        return r.copy_back({{out32, (size_t)r.i0 * 32, d_out, (size_t)r.cnt * 32}});
+    });
 }
 int afc_hmac_sha256_batch(afc_ctx* ctx, const uint8_t* keys, const uint32_t* key_off, const uint8_t* msgs,
                           const uint64_t* msg_off, uint32_t n, uint8_t* out32) {
     if (!ctx || !key_off || !msg_off || (!out32 && n)) return AFC_EINVAL;
-    BatchArgs A{}; A.op = OP_HMAC; A.msgs = msgs; A.off = msg_off; A.n = n; A.keys = keys; A.koff = key_off; A.out = out32; A.out_item = 32;
-    return run_host_batch(ctx, A);
+    if (n == 0) return AFC_OK;
+    if (!monotone(key_off, n)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(msg_off), [&](Ring& r) {
+        Msgs M;
+        const uint8_t* d_keys;
+        const uint32_t* d_koff;
+        uint8_t* d_out;
+        RC(r.stage([&](Stager& k) {
+            M = stage_msgs(k, msgs, msg_off, r.i0, r.cnt);
+            d_keys = k.in_at(keys, key_off[r.i0], key_off[r.i0 + r.cnt] - key_off[r.i0], 4);
+            d_koff = k.in(key_off, r.i0, (size_t)r.cnt + 1);
+            d_out = k.take((size_t)r.cnt * 32 + 16);
+        }));
+        CK(launch::hmac_sha256_batch(d_keys, d_koff, M.d, M.off, r.cnt, d_out, r.st, r.lc));
+        return r.copy_back({{out32, (size_t)r.i0 * 32, d_out, (size_t)r.cnt * 32}});
+    });
 }
 int afc_ed25519_verify_batch(afc_ctx* ctx, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs,
                              const uint64_t* msg_off, uint32_t n, uint8_t* ok) {
     if (!ctx || !msg_off || (n && (!pks || !sigs || !ok))) return AFC_EINVAL;
-    BatchArgs A{}; A.op = OP_VERIFY; A.msgs = msgs; A.off = msg_off; A.n = n; A.a = pks; A.a_item = 32; A.b = sigs; A.b_item = 64; A.out = ok; A.out_item = 1;
-    return run_host_batch(ctx, A);
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(msg_off), [&](Ring& r) {
+        Msgs M;
+        const uint8_t *d_pks, *d_sigs;
+        uint8_t* d_ok;
+        uint32_t* d_k;
+        RC(r.stage([&](Stager& k) {
+            M = stage_msgs(k, msgs, msg_off, r.i0, r.cnt);
+            d_pks = k.in(pks, (size_t)r.i0 * 32, (size_t)r.cnt * 32);
+            d_sigs = k.in(sigs, (size_t)r.i0 * 64, (size_t)r.cnt * 64);
+            d_ok = k.take((size_t)r.cnt + 16);
+            d_k = k.take<uint32_t>((size_t)r.cnt * 8);
+        }));
+        CK(verify_with_cache(ctx, d_pks, d_sigs, M.d, M.off, r.cnt, d_ok, d_k, r.st, r.lc));
+        return r.copy_back({{ok, r.i0, d_ok, r.cnt}});
+    });
 }
 int afc_ed25519_sign_batch(afc_ctx* ctx, const uint8_t* seeds, const uint8_t* msgs, const uint64_t* msg_off,
                            uint32_t n, uint8_t* sigs) {
     if (!ctx || !msg_off || (n && (!seeds || !sigs))) return AFC_EINVAL;
-    BatchArgs A{}; A.op = OP_SIGN; A.msgs = msgs; A.off = msg_off; A.n = n; A.a = seeds; A.a_item = 32; A.out = sigs; A.out_item = 64;
-    return run_host_batch(ctx, A);
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(msg_off), [&](Ring& r) {
+        Msgs M;
+        const uint8_t* d_seeds;
+        uint8_t* d_sigs;
+        RC(r.stage([&](Stager& k) {
+            M = stage_msgs(k, msgs, msg_off, r.i0, r.cnt);
+            d_seeds = k.in(seeds, (size_t)r.i0 * 32, (size_t)r.cnt * 32, true);
+            d_sigs = k.take((size_t)r.cnt * 64 + 16);
+        }));
+        CK(launch::ed_sign_batch(ctx->comb, afc_internal_sign_table(ctx), d_seeds, M.d, M.off, r.cnt, d_sigs, r.st, r.lc));
+        return r.copy_back({{sigs, (size_t)r.i0 * 64, d_sigs, (size_t)r.cnt * 64}});
+    });
 }
 
 // ---------------------------------------------------------------------------------- H2: streaming SHA-256
@@ -746,28 +862,23 @@ int afc_sha256_update_batch(afc_ctx* ctx, uint8_t* states, const uint8_t* chunks
     const uint64_t base = chunk_off[0], bytes = chunk_off[n] - base;
     if (bytes && !chunks) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    LaneGuard lg(ctx);
-    Slot& sl = lg.lane().slot[0];
-    LaneDrain drain_on_exit(lg.lane());
-    const size_t pad = (size_t)(base & 15);
-    CK(sl.msgs.reserve(bytes + 32)); CK(sl.off.reserve((size_t)(n + 1) * 8)); CK(sl.a.reserve((size_t)n * AFC_SHA256_STATE_BYTES));
-    CK(sl.b.reserve((size_t)n * 2 + 16)); CK(sl.out.reserve((size_t)n * 32 + 16));
-    if (bytes) CK(cudaMemcpyAsync(sl.msgs.p + pad, chunks + base, bytes, cudaMemcpyHostToDevice, sl.stream));
-    CK(cudaMemcpyAsync(sl.off.p, chunk_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, sl.stream));
-    CK(cudaMemcpyAsync(sl.a.p, states, (size_t)n * AFC_SHA256_STATE_BYTES, cudaMemcpyHostToDevice, sl.stream));
-    uint8_t* d_fin = nullptr;
-    if (final_flags) { d_fin = sl.b.p; CK(cudaMemcpyAsync(d_fin, final_flags, n, cudaMemcpyHostToDevice, sl.stream)); }
-    uint8_t* d_status = sl.b.p + n;
-    {
-        CallLog lc(ctx);
-        CK(launch::sha256_update(sl.a.p, sl.msgs.p + pad - base, (const uint64_t*)sl.off.p, n, d_fin, sl.out.p, d_status, sl.stream, lc));
-    }
     std::vector<uint8_t> status(n), dig(any_final ? (size_t)n * 32 : 0);
-    CK(cudaMemcpyAsync(states, sl.a.p, (size_t)n * AFC_SHA256_STATE_BYTES, cudaMemcpyDeviceToHost, sl.stream));
-    CK(cudaMemcpyAsync(status.data(), d_status, n, cudaMemcpyDeviceToHost, sl.stream));
-    if (any_final) CK(cudaMemcpyAsync(dig.data(), sl.out.p, (size_t)n * 32, cudaMemcpyDeviceToHost, sl.stream));
-    CK(cudaStreamSynchronize(sl.stream));
-    drain_on_exit.armed = false;
+    Ring ring(ctx, 1);
+    RC(ring.once(n, [&](Ring& r) {
+        uint8_t *d_chunks, *d_states, *d_fin = nullptr, *d_dig, *d_status;
+        const uint64_t* d_off;
+        RC(r.stage([&](Stager& k) {
+            d_chunks = k.in_at(chunks, base, bytes, 16);
+            d_off = k.in(chunk_off, 0, (size_t)n + 1);
+            d_states = k.in(states, 0, (size_t)n * AFC_SHA256_STATE_BYTES);
+            if (final_flags) d_fin = k.in(final_flags, 0, n);
+            d_status = k.take(n);
+            d_dig = k.take((size_t)n * 32 + 16);
+        }));
+        CK(launch::sha256_update(d_states, d_chunks, d_off, n, d_fin, d_dig, d_status, r.st, r.lc));
+        return r.copy_back({{states, 0, d_states, (size_t)n * AFC_SHA256_STATE_BYTES}, {status.data(), 0, d_status, n},
+                            {dig.data(), 0, d_dig, dig.size()}});
+    }));
     for (uint32_t i = 0; i < n; i++) {
         if (!status[i]) return AFC_EINVAL;                                             // a state that is not ours (or not on a block boundary)
         if (final_flags && final_flags[i]) memcpy(out32 + 32ull * i, dig.data() + 32ull * i, 32);
@@ -787,17 +898,18 @@ static int expand_common(afc_ctx* ctx, const uint8_t* seeds, uint32_t n, uint8_t
     if (!ctx || (n && (!seeds || !out))) return AFC_EINVAL;
     if (n == 0) return AFC_OK;
     CK(cudaSetDevice(ctx->device));
-    LaneGuard lg(ctx);
-    Slot& sl = lg.lane().slot[0];
-    CK(sl.a.reserve((size_t)n * 32)); CK(sl.out.reserve((size_t)n * item));
-    CK(cudaMemcpyAsync(sl.a.p, seeds, (size_t)n * 32, cudaMemcpyHostToDevice, sl.stream));
-    CallLog lc(ctx);
-    CK(launch::ed_expand_batch(ctx->comb, afc_internal_sign_table(ctx), sl.a.p, n, expanded ? sl.out.p : nullptr, expanded ? nullptr : sl.out.p, sl.stream, lc));
-    CK(cudaMemcpyAsync(out, sl.out.p, (size_t)n * item, cudaMemcpyDeviceToHost, sl.stream));
-    CK(cudaMemsetAsync(sl.a.p, 0, (size_t)n * 32, sl.stream));                       // seeds and expanded private keys are wiped from the slot
-    if (expanded) CK(cudaMemsetAsync(sl.out.p, 0, (size_t)n * item, sl.stream));
-    CK(cudaStreamSynchronize(sl.stream));
-    return AFC_OK;
+    Ring ring(ctx, 1);
+    return ring.once(n, [&](Ring& r) {
+        const uint8_t* d_seeds;
+        uint8_t* d_out;
+        RC(r.stage([&](Stager& k) {
+            d_seeds = k.in(seeds, 0, (size_t)n * 32, true);
+            d_out = k.take((size_t)n * item, expanded);       // expanded private keys are secret, public keys are not
+        }));
+        CK(launch::ed_expand_batch(ctx->comb, afc_internal_sign_table(ctx), d_seeds, n, expanded ? d_out : nullptr, expanded ? nullptr : d_out, r.st,
+                                   r.lc));
+        return r.copy_back({{out, 0, d_out, (size_t)n * item, expanded}});
+    });
 }
 int afc_ed25519_pubkey_batch(afc_ctx* ctx, const uint8_t* seeds, uint32_t n, uint8_t* pks) { return expand_common(ctx, seeds, n, pks, 32, false); }
 int afc_ed25519_expand_batch(afc_ctx* ctx, const uint8_t* seeds, uint32_t n, uint8_t* expanded96) { return expand_common(ctx, seeds, n, expanded96, 96, true); }
@@ -809,17 +921,22 @@ int afc_ed25519_sign_expanded_batch(afc_ctx* ctx, const uint8_t* expanded96, con
     if (key_index) for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
     if (n == 0) return AFC_OK;
     CK(cudaSetDevice(ctx->device));
-    uint8_t* d_keys = nullptr;
-    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
-    cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
-    int rc = AFC_ECUDA;
-    if (e == cudaSuccess) {
-        BatchArgs A{}; A.op = OP_SIGN_EXP; A.msgs = msgs; A.off = msg_off; A.n = n; A.d_expanded = d_keys; A.key_index = key_index; A.out = sigs; A.out_item = 64;
-        rc = run_host_batch(ctx, A);
-    } else set_err(ctx, e, "cudaMemcpy(expanded keys)");
-    cudaMemset(d_keys, 0, (size_t)n_keys * 96);       // expanded private keys do not outlive the call on the device
-    cudaFree(d_keys);
-    return rc;
+    return with_device_keys(ctx, expanded96, n_keys, [&](const uint8_t* d_keys) {
+        Ring ring(ctx);
+        return ring.walk(n, msg_bytes(msg_off), [&](Ring& r) {
+            Msgs M;
+            const uint32_t* d_ki = nullptr;
+            uint8_t* d_sigs;
+            RC(r.stage([&](Stager& k) {
+                M = stage_msgs(k, msgs, msg_off, r.i0, r.cnt);
+                if (key_index) d_ki = k.in(key_index, r.i0, r.cnt);
+                d_sigs = k.take((size_t)r.cnt * 64 + 16);
+            }));
+            CK(launch::ed_sign_expanded_batch(ctx->comb, afc_internal_sign_table(ctx), d_keys + (key_index ? 0 : (size_t)r.i0 * 96), 0xffffffffu, d_ki,
+                                              M.d, M.off, r.cnt, d_sigs, r.st, r.lc));
+            return r.copy_back({{sigs, (size_t)r.i0 * 64, d_sigs, (size_t)r.cnt * 64}});
+        });
+    });
 }
 
 // ---------------------------------------------------------------------------------- device-pointer variants
@@ -1032,9 +1149,26 @@ int afc_keyset_info(afc_keyset* ks, uint32_t* n_keys, uint64_t* table_bytes) {
 int afc_ed25519_verify_keyed_batch(afc_ctx* ctx, afc_keyset* ks, const uint32_t* key_index, const uint8_t* sigs,
                                    const uint8_t* msgs, const uint64_t* msg_off, uint32_t n, uint8_t* ok) {
     if (!ctx || !ks || ks->ctx != ctx || !msg_off || (n && (!key_index || !sigs || !ok))) return AFC_EINVAL;
-    BatchArgs A{}; A.op = OP_VERIFY_KEYED; A.msgs = msgs; A.off = msg_off; A.n = n; A.b = sigs; A.b_item = 64; A.key_index = key_index;
-    A.keyset = ks; A.out = ok; A.out_item = 1;
-    return run_host_batch(ctx, A);
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(msg_off), [&](Ring& r) {
+        Msgs M;
+        const uint32_t* d_ki;
+        const uint8_t* d_sigs;
+        uint8_t* d_ok;
+        uint32_t* d_k;
+        RC(r.stage([&](Stager& k) {
+            M = stage_msgs(k, msgs, msg_off, r.i0, r.cnt);
+            d_sigs = k.in(sigs, (size_t)r.i0 * 64, (size_t)r.cnt * 64);
+            d_ki = k.in(key_index, r.i0, r.cnt);
+            d_ok = k.take((size_t)r.cnt + 16);
+            d_k = (uint32_t*)k.take((size_t)r.cnt * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, r.cnt));
+        }));
+        CK(launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_ki, d_sigs, M.d, M.off, r.cnt, d_ok, d_k,
+                                         d_k + (size_t)r.cnt * 8, r.st, r.lc));
+        return r.copy_back({{ok, r.i0, d_ok, r.cnt}});
+    });
 }
 int afc_ed25519_verify_keyed_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint32_t* d_key_index, const uint8_t* d_sigs,
                                        const uint8_t* d_msgs, const uint64_t* d_msg_off, uint32_t n, uint8_t* d_ok, void* stream) {
@@ -1113,13 +1247,31 @@ static int vc_stored_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uin
     if (!ks->named) return AFC_ESTATE;
     return AFC_OK;
 }
+// the host-buffer form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
+static int vc_verify_host(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, uint8_t* status,
+                          uint32_t* fields, bool json) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
+    if (rc != AFC_OK || n == 0) return rc;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    return ring.walk(n, msg_bytes(doc_off), [&](Ring& r) {
+        Msgs D;
+        uint8_t* d_status;
+        uint32_t* d_fields = nullptr;
+        VcScratch S;
+        RC(r.stage([&](Stager& k) {
+            D = stage_msgs(k, docs, doc_off, r.i0, r.cnt);
+            d_status = k.take((size_t)r.cnt + 16);
+            if (fields) d_fields = k.take<uint32_t>((size_t)r.cnt * 4 + 4);
+            vc_scratch(k, S, r.cnt, doc_off[r.i0 + r.cnt] - doc_off[r.i0], ks->n_keys, false);
+        }));
+        CK(vc_stored_enqueue(ctx, ks, doc_kind, D.d, D.off, r.cnt, d_status, d_fields, S, r.st, r.lc, nullptr, nullptr, nullptr, json));
+        return r.copy_back({{status, r.i0, d_status, r.cnt}, {fields, (size_t)r.i0 * 16, d_fields, fields ? (size_t)r.cnt * 16 : 0}});
+    });
+}
 int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
                                uint8_t* status, uint32_t* fields) {
-    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
-    if (rc != AFC_OK) return rc;
-    BatchArgs A{}; A.op = OP_VC_STORED; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
-    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)fields; A.out2_item = fields ? 16 : 0;
-    return run_host_batch(ctx, A);
+    return vc_verify_host(ctx, ks, doc_kind, docs, doc_off, n, status, fields, false);
 }
 // the _dev form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
 static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n, uint8_t* d_status,
@@ -1136,9 +1288,9 @@ static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8
     CK(cudaStreamSynchronize(st));
     if (ends[1] < ends[0]) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
-    CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys), st));
-    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, d_fields, scratch, st, lc, nullptr,
-                                      nullptr, nullptr, json);
+    VcScratch S;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { vc_scratch(k, S, n, ends[1] - ends[0], ks->n_keys, false); }));
+    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, S, st, lc, nullptr, nullptr, nullptr, json);
     cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;
@@ -1151,11 +1303,7 @@ int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, c
 // documents in any JSON spelling: the arguments, statuses and fields of afc_vc_verify_stored_batch
 int afc_vc_verify_json_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
                              uint8_t* status, uint32_t* fields) {
-    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
-    if (rc != AFC_OK) return rc;
-    BatchArgs A{}; A.op = OP_VC_JSON; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
-    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)fields; A.out2_item = fields ? 16 : 0;
-    return run_host_batch(ctx, A);
+    return vc_verify_host(ctx, ks, doc_kind, docs, doc_off, n, status, fields, true);
 }
 int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                  uint8_t* d_status, uint32_t* d_fields, void* stream) {
@@ -1174,11 +1322,35 @@ static int vc_audit_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint
 int afc_vc_audit_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
                               const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
     int rc = vc_audit_check(ctx, ks, doc_kind, docs, doc_off, cols, col_off, n, status, issues);
-    if (rc != AFC_OK) return rc;
-    BatchArgs A{}; A.op = OP_VC_AUDIT; A.msgs = docs; A.off = doc_off; A.n = n; A.keyset = ks; A.doc_kind = doc_kind;
-    A.cols = cols; A.col_off = col_off;
-    A.out = status; A.out_item = 1; A.out2 = (uint8_t*)issues; A.out2_item = 4;
-    return run_host_batch(ctx, A);
+    if (rc != AFC_OK || n == 0) return rc;
+    const uint32_t C = AFC_AUDIT_COLUMNS;
+    CK(cudaSetDevice(ctx->device));
+    Ring ring(ctx);
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        if (col_off) for (uint32_t k = 0; k < C; k++) if (col_off[(size_t)i * C + k + 1] < col_off[(size_t)i * C + k]) return kBadOffsets;
+        return msg_bytes(doc_off)(i0, i);
+    };
+    return ring.walk(n, measure, [&](Ring& r) {
+        Msgs D;
+        const uint8_t* d_cols = nullptr;
+        const uint64_t* d_coff = nullptr;
+        uint8_t* d_status;
+        uint32_t* d_issues;
+        VcScratch S;
+        RC(r.stage([&](Stager& k) {
+            D = stage_msgs(k, docs, doc_off, r.i0, r.cnt);
+            if (col_off) {
+                const uint64_t cbase = col_off[(size_t)r.i0 * C];
+                d_cols = k.in_at(cols, cbase, col_off[(size_t)(r.i0 + r.cnt) * C] - cbase, 16);
+                d_coff = k.in(col_off, (size_t)r.i0 * C, (size_t)r.cnt * C + 1);
+            }
+            d_status = k.take((size_t)r.cnt + 16);
+            d_issues = k.take<uint32_t>((size_t)r.cnt + 4);
+            vc_scratch(k, S, r.cnt, doc_off[r.i0 + r.cnt] - doc_off[r.i0], ks->n_keys, true);
+        }));
+        CK(vc_stored_enqueue(ctx, ks, doc_kind, D.d, D.off, r.cnt, d_status, nullptr, S, r.st, r.lc, d_issues, d_cols, d_coff));
+        return r.copy_back({{status, r.i0, d_status, r.cnt}, {issues, (size_t)r.i0 * 4, d_issues, (size_t)r.cnt * 4}});
+    });
 }
 int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
                                   const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_issues, void* stream) {
@@ -1193,9 +1365,9 @@ int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, co
     CK(cudaStreamSynchronize(st));
     if (ends[1] < ends[0]) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
-    CK(cudaMallocAsync((void**)&scratch, vc_scratch_bytes(n, ends[1] - ends[0], ks->n_keys, true), st));
-    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, ends[1] - ends[0], d_status, nullptr, scratch, st, lc, d_issues,
-                                      d_cols, d_col_off);
+    VcScratch S;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { vc_scratch(k, S, n, ends[1] - ends[0], ks->n_keys, true); }));
+    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, nullptr, S, st, lc, d_issues, d_cols, d_col_off);
     cudaFreeAsync(scratch, st);
     CK(e);
     return AFC_OK;
@@ -1218,17 +1390,11 @@ uint64_t afc_vc_issue_bound(const uint64_t* col_off, uint32_t n) {
 
 // per-call device scratch: signing messages and their offsets, signatures, scan tiles
 struct IssueScratch { uint8_t* msgs; uint64_t* msg_off; uint8_t* sigs; uint64_t* scan; };
-static size_t issue_scratch_bytes(uint32_t n, uint64_t col_bytes) {
-    return vc_align(issue_msg_bound(n, col_bytes) + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) +
-           vc_align(launch::json_scan_scratch_bytes(n));
-}
-static IssueScratch issue_scratch(uint8_t* p, uint32_t n, uint64_t col_bytes) {
-    IssueScratch s;
-    s.msgs = p; p += vc_align(issue_msg_bound(n, col_bytes) + 64);
-    s.msg_off = (uint64_t*)p; p += vc_align(((size_t)n + 1) * 8);
-    s.sigs = p; p += vc_align((size_t)n * 64);
-    s.scan = (uint64_t*)p;
-    return s;
+static void issue_scratch(Carve& k, IssueScratch& s, uint32_t n, uint64_t col_bytes) {
+    s.msgs = k.take(issue_msg_bound(n, col_bytes) + 64);
+    s.msg_off = k.take<uint64_t>((size_t)n + 1);
+    s.sigs = k.take((size_t)n * 64);
+    s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
 }
 // hashData, both lengths, both scans: doc_off is complete when this has run
 static cudaError_t issue_sizes(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* pay, const uint64_t* pay_off,
@@ -1283,8 +1449,8 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
     {
         CallLog lc(ctx);
         uint8_t* scratch = nullptr;
-        CK(cudaMallocAsync((void**)&scratch, issue_scratch_bytes(n, cb), st));
-        const IssueScratch S = issue_scratch(scratch, n, cb);
+        IssueScratch S;
+        CK(pool_carve(&scratch, st, [&](Carve& k) { issue_scratch(k, S, n, cb); }));
         cudaError_t e = issue_sizes(d_cols, d_col_off, d_duration_ms, d_payloads, d_payload_off, d_payload_nil, hashes, n, d_doc_off, S, st, lc);
         if (e == cudaSuccess) e = issue_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_duration_ms, hashes, n, d_docs, d_doc_off,
                                                d_proof_values, S, st, lc);
@@ -1292,127 +1458,6 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
         CK(e);
     }
     return log ? afc_merkle_append_dev(log, d_docs, d_doc_off, n, stream) : AFC_OK;
-}
-
-// The host-buffer call: chunks of credentials through the lane's ring.  A chunk's documents land at their final offsets, so its
-// stream is synchronised once after the sizes pass to learn where the chunk ends (the next chunk's copies are enqueued after that).
-static int issue_host_run(afc_ctx* ctx, const uint8_t* d_keys, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
-                          const int64_t* dur, const uint8_t* pay, const uint64_t* pay_off, const uint8_t* nil, bool hash, uint32_t n, afc_merkle* log,
-                          uint8_t* docs, uint64_t* doc_off, uint8_t* hashes, uint8_t* pv) {
-    const uint32_t C = AFC_ISSUE_COLUMNS;
-    LaneGuard lg(ctx);
-    Lane& lane = lg.lane();
-    LaneDrain drain_on_exit(lane);
-    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_dur = is_pinned(dur), pin_ki = is_pinned(key_index);
-    const bool pin_pay = hash ? is_pinned(pay) : true, pin_poff = hash ? is_pinned(pay_off) : true, pin_nil = hash ? is_pinned(nil) : true;
-    const bool pin_docs = is_pinned(docs), pin_h = hash ? is_pinned(hashes) : true, pin_pv = is_pinned(pv);
-    CallLog lc(ctx);
-    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
-    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
-    auto drain = [&](int w) -> int {
-        Pending& p = pend[w];
-        if (!p.active) return AFC_OK;
-        Slot& sl = lane.slot[w];
-        CK(cudaStreamSynchronize(sl.stream));
-        const uint8_t* h = sl.h_out.p;
-        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
-        for (uint32_t j = 0; j < p.cnt; j++) doc_off[p.i0 + j] = p.base + rel[j];
-        if (!pin_h) { memcpy(hashes + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
-        if (!pin_pv) { memcpy(pv + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
-        if (!pin_docs) memcpy(docs + p.base, h, p.bytes);
-        p.active = false;
-        return AFC_OK;
-    };
-    uint32_t i0 = 0;
-    uint64_t base = 0;
-    int which = 0;
-    while (i0 < n) {
-        const uint32_t left = n - i0;
-        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
-        if (limit < min_chunk) limit = min_chunk;
-        if (limit > max_chunk) limit = max_chunk;
-        uint32_t i1 = i0;
-        const uint64_t cbase = col_off[(size_t)i0 * C], pbase = hash ? pay_off[2 * (size_t)i0] : 0;
-        while (i1 < n && i1 - i0 < limit) {
-            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (hash ? pay_off[2 * (size_t)(i1 + 1)] - pbase : 0);
-            if (bytes > kChunkBytes && i1 != i0) break;
-            i1++;
-        }
-        const uint32_t cnt = i1 - i0;
-        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, pbytes = hash ? pay_off[2 * (size_t)i1] - pbase : 0;
-        Slot& sl = lane.slot[which];
-        int rc = drain(which);
-        if (rc != AFC_OK) return rc;
-        const uint64_t dbound = issue_doc_bound(cnt, cbytes);
-        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 8, (size_t)cnt * 4, pbytes + 32, ((size_t)2 * cnt + 1) * 8,
-                             (size_t)2 * cnt, dbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 86, (size_t)cnt * 86, issue_scratch_bytes(cnt, cbytes)};
-        size_t total = 0;
-        for (size_t b : sz) total += vc_align(b);
-        CK(sl.vc.reserve(total));
-        uint8_t* q[12];
-        {
-            uint8_t* p = sl.vc.p;
-            for (int k = 0; k < 12; k++) { q[k] = p; p += vc_align(sz[k]); }
-        }
-        size_t bounce = 0;
-        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_dur ? 0 : (size_t)cnt * 8,
-                                   pin_ki ? 0 : (size_t)cnt * 4, pin_pay ? 0 : pbytes, pin_poff ? 0 : ((size_t)2 * cnt + 1) * 8, pin_nil ? 0 : (size_t)2 * cnt};
-        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
-        CK(sl.h_in.reserve(bounce + 256, ctx));
-        CK(sl.h_out2.reserve(8, ctx));
-        size_t used = 0;
-        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
-        const uint64_t* d_coff = (const uint64_t*)q[1];
-        const int64_t* d_dur = (const int64_t*)q[2];
-        const uint32_t* d_ki = (const uint32_t*)q[3];
-        uint8_t* d_pay = q[4] + (pbase & 15) - pbase;
-        const uint64_t* d_poff = (const uint64_t*)q[5];
-        const uint8_t* d_nil = q[6];
-        uint8_t* d_docs = q[7];
-        uint64_t* d_doff = (uint64_t*)q[8];
-        uint8_t* d_h = hash ? q[9] : nullptr;
-        uint8_t* d_pv = q[10];
-        const IssueScratch S = issue_scratch(q[11], cnt, cbytes);
-        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
-        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
-        CK(h2d(sl, q[2], dur + i0, (size_t)cnt * 8, pin_dur, &used));
-        CK(h2d(sl, q[3], key_index + i0, (size_t)cnt * 4, pin_ki, &used));
-        if (hash) {
-            CK(h2d(sl, q[4] + (pbase & 15), pay + pbase, pbytes, pin_pay, &used));
-            CK(h2d(sl, q[5], pay_off + 2 * (size_t)i0, ((size_t)2 * cnt + 1) * 8, pin_poff, &used));
-            CK(h2d(sl, q[6], nil + 2 * (size_t)i0, (size_t)2 * cnt, pin_nil, &used));
-        }
-        CK(issue_sizes(d_cols, d_coff, d_dur, d_pay, d_poff, d_nil, d_h, cnt, d_doff, S, sl.stream, lc));
-        CK(cudaMemcpyAsync(sl.h_out2.p, d_doff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
-        CK(cudaStreamSynchronize(sl.stream));
-        uint64_t bytes;
-        memcpy(&bytes, sl.h_out2.p, 8);
-        CK(issue_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_dur, d_h, cnt, d_docs, d_doff, d_pv, S, sl.stream, lc));
-        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_h ? 0 : vc_align((size_t)cnt * 86)) + (pin_pv ? 0 : vc_align((size_t)cnt * 86)) +
-                            (pin_docs ? 0 : bytes) + 256, ctx));
-        uint8_t* h = sl.h_out.p;
-        CK(cudaMemcpyAsync(h, d_doff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
-        h += vc_align(((size_t)cnt + 1) * 8);
-        if (hash) {
-            CK(cudaMemcpyAsync(pin_h ? hashes + (size_t)i0 * 86 : h, d_h, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
-            if (!pin_h) h += vc_align((size_t)cnt * 86);
-        }
-        CK(cudaMemcpyAsync(pin_pv ? pv + (size_t)i0 * 86 : h, d_pv, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_pv) h += vc_align((size_t)cnt * 86);
-        CK(cudaMemcpyAsync(pin_docs ? docs + base : h, d_docs, bytes, cudaMemcpyDeviceToHost, sl.stream));
-        if (log) { rc = afc_merkle_append_dev(log, d_docs, d_doff, cnt, sl.stream); if (rc != AFC_OK) return rc; }
-        pend[which] = {i0, cnt, base, bytes, true};
-        base += bytes;
-        which = (which + 1) % kSlots;
-        i0 = i1;
-    }
-    for (int w = 0; w < kSlots; w++) {      // oldest first
-        int rc = drain((which + w) % kSlots);
-        if (rc != AFC_OK) return rc;
-    }
-    drain_on_exit.armed = false;
-    doc_off[n] = base;
-    return AFC_OK;
 }
 
 int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
@@ -1430,16 +1475,53 @@ int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32
     if (hash) for (size_t k = 0; k < (size_t)2 * n; k++) bad |= (uint64_t)(payload_off[k + 1] < payload_off[k]);
     if (bad || docs_cap < afc_vc_issue_bound(col_off, n)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    uint8_t* d_keys = nullptr;
-    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
-    cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        rc = issue_host_run(ctx, d_keys, n_keys, key_index, cols, col_off, duration_ms, payloads, payload_off, payload_nil, hash, n, log, docs, doc_off,
-                            hashes, proof_values);
-    } else { set_err(ctx, e, "cudaMemcpy(expanded keys)"); rc = AFC_ECUDA; }
-    cudaMemset(d_keys, 0, (size_t)n_keys * 96);       // expanded private keys do not outlive the call on the device
-    cudaFree(d_keys);
-    return rc;
+    // Chunks of credentials through the ring.  A chunk's documents land at their final offsets, so its stream is synchronised once after
+    // the sizes pass to learn where the chunk ends (the next chunk's copies are enqueued after that).
+    const uint32_t C = AFC_ISSUE_COLUMNS;
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        return (col_off[(size_t)(i + 1) * C] - col_off[(size_t)i0 * C]) + (hash ? payload_off[2 * (size_t)(i + 1)] - payload_off[2 * (size_t)i0] : 0);
+    };
+    uint64_t base = 0;
+    return with_device_keys(ctx, expanded96, n_keys, [&](const uint8_t* d_keys) {
+        Ring ring(ctx);
+        return ring.walk(n, measure, [&](Ring& r) {
+            const uint32_t i0 = r.i0, cnt = r.cnt;
+            const uint64_t cbase = col_off[(size_t)i0 * C], cbytes = col_off[(size_t)(i0 + cnt) * C] - cbase;
+            const uint64_t pbase = hash ? payload_off[2 * (size_t)i0] : 0, pbytes = hash ? payload_off[2 * (size_t)(i0 + cnt)] - pbase : 0;
+            const uint8_t *d_cols, *d_pay = nullptr, *d_nil = nullptr;
+            const uint64_t *d_coff, *d_poff = nullptr;
+            const int64_t* d_dur;
+            const uint32_t* d_ki;
+            uint8_t *d_docs, *d_h = nullptr, *d_pv;
+            uint64_t* d_doff;
+            IssueScratch S;
+            RC(r.stage([&](Stager& k) {
+                d_cols = k.in_at(cols, cbase, cbytes, 16);
+                d_coff = k.in(col_off, (size_t)i0 * C, (size_t)cnt * C + 1);
+                d_dur = k.in(duration_ms, i0, cnt);
+                d_ki = k.in(key_index, i0, cnt);
+                if (hash) {
+                    d_pay = k.in_at(payloads, pbase, pbytes, 16);
+                    d_poff = k.in(payload_off, 2 * (size_t)i0, 2 * (size_t)cnt + 1);
+                    d_nil = k.in(payload_nil, 2 * (size_t)i0, 2 * (size_t)cnt);
+                    d_h = k.take((size_t)cnt * 86);
+                }
+                d_docs = k.take(issue_doc_bound(cnt, cbytes) + 64);
+                d_doff = k.take<uint64_t>((size_t)cnt + 1);
+                d_pv = k.take((size_t)cnt * 86);
+                issue_scratch(k, S, cnt, cbytes);
+            }));
+            CK(issue_sizes(d_cols, d_coff, d_dur, d_pay, d_poff, d_nil, d_h, cnt, d_doff, S, r.st, r.lc));
+            uint64_t bytes;
+            RC(r.read(&bytes, {d_doff + cnt}));
+            CK(issue_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_dur, d_h, cnt, d_docs, d_doff, d_pv, S, r.st, r.lc));
+            RC(r.copy_back({offsets_out(doc_off, i0, d_doff, (size_t)cnt + 1, base), {hashes, (size_t)i0 * 86, d_h, hash ? (size_t)cnt * 86 : 0},
+                            {proof_values, (size_t)i0 * 86, d_pv, (size_t)cnt * 86}, {docs, base, d_docs, bytes}}));
+            if (log) RC(afc_merkle_append_dev(log, d_docs, d_doff, cnt, r.st));
+            base += bytes;
+            return AFC_OK;
+        });
+    });
 }
 
 // ---------------------------------------------------------------------------------- issuing workflow credentials
@@ -1462,20 +1544,14 @@ uint64_t afc_vc_workflow_bound(const uint64_t* col_off, const uint64_t* rec_off,
 
 // per-call device scratch: signing messages and their offsets, signatures, scan tiles, record classes, record id offsets, array places
 struct WorkflowScratch { uint8_t* msgs; uint64_t* msg_off; uint8_t* sigs; uint64_t* scan; uint8_t* cls; uint64_t* id_off; uint64_t* arr; };
-static size_t wf_scratch_bytes(uint32_t n, uint32_t m, uint64_t msg_bound) {
-    return vc_align(msg_bound + 64) + vc_align(((size_t)n + 1) * 8) + vc_align((size_t)n * 64) + vc_align(launch::json_scan_scratch_bytes(n > m ? n : m)) +
-           vc_align(m) + vc_align(((size_t)m + 1) * 8) + vc_align((size_t)n * 16);
-}
-static WorkflowScratch wf_scratch(uint8_t* p, uint32_t n, uint32_t m, uint64_t msg_bound) {
-    WorkflowScratch s;
-    s.msgs = p; p += vc_align(msg_bound + 64);
-    s.msg_off = (uint64_t*)p; p += vc_align(((size_t)n + 1) * 8);
-    s.sigs = p; p += vc_align((size_t)n * 64);
-    s.scan = (uint64_t*)p; p += vc_align(launch::json_scan_scratch_bytes(n > m ? n : m));
-    s.cls = p; p += vc_align(m);
-    s.id_off = (uint64_t*)p; p += vc_align(((size_t)m + 1) * 8);
-    s.arr = (uint64_t*)p;
-    return s;
+static void wf_scratch(Carve& k, WorkflowScratch& s, uint32_t n, uint32_t m, uint64_t msg_bound) {
+    s.msgs = k.take(msg_bound + 64);
+    s.msg_off = k.take<uint64_t>((size_t)n + 1);
+    s.sigs = k.take((size_t)n * 64);
+    s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n > m ? n : m));
+    s.cls = k.take(m);
+    s.id_off = k.take<uint64_t>((size_t)m + 1);
+    s.arr = k.take<uint64_t>((size_t)n * 2);
 }
 // records, plans and both lengths, the three scans: doc_off is complete when this has run
 static cudaError_t wf_sizes(const uint8_t* cols, const uint64_t* col_off, const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off,
@@ -1537,142 +1613,13 @@ int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
     const uint64_t bound = wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4]);
     if (docs_cap < bound) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
-    CK(cudaMallocAsync((void**)&scratch, wf_scratch_bytes(n, m, bound), st));
-    const WorkflowScratch S = wf_scratch(scratch, n, m, bound);
+    WorkflowScratch S;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { wf_scratch(k, S, n, m, bound); }));
     cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, d_doc_off, d_summary, d_state, S, st, lc);
     if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m,
                                         d_docs, d_doc_off, d_proof_values, d_state, d_summary, S, st, lc);
     cudaFreeAsync(scratch, st);
     CK(e);
-    return AFC_OK;
-}
-
-// The host-buffer call: chunks of whole workflows through the lane's ring, as issue_host_run does.  A chunk's records travel with it
-// (the kernels index them by absolute record, so the staged record arrays are addressed from a shifted base); a workflow larger than a
-// chunk's byte budget goes alone.
-static int wf_host_run(afc_ctx* ctx, const uint8_t* d_keys, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
-                       const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created, uint32_t n, uint8_t* docs,
-                       uint64_t* doc_off, uint8_t* pv, uint8_t* state, uint32_t* summary) {
-    const uint32_t C = AFC_WORKFLOW_COLUMNS;
-    LaneGuard lg(ctx);
-    Lane& lane = lg.lane();
-    LaneDrain drain_on_exit(lane);
-    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_ki = is_pinned(key_index), pin_roff = is_pinned(rec_off);
-    const bool pin_rcols = is_pinned(rec_cols), pin_rcoff = is_pinned(rec_col_off), pin_cr = is_pinned(created);
-    const bool pin_docs = is_pinned(docs), pin_pv = is_pinned(pv), pin_st = is_pinned(state), pin_sum = is_pinned(summary);
-    CallLog lc(ctx);
-    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
-    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
-    auto drain = [&](int w) -> int {
-        Pending& p = pend[w];
-        if (!p.active) return AFC_OK;
-        Slot& sl = lane.slot[w];
-        CK(cudaStreamSynchronize(sl.stream));
-        const uint8_t* h = sl.h_out.p;
-        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
-        for (uint32_t j = 0; j < p.cnt; j++) doc_off[p.i0 + j] = p.base + rel[j];
-        if (!pin_pv) { memcpy(pv + (size_t)p.i0 * 86, h, (size_t)p.cnt * 86); h += vc_align((size_t)p.cnt * 86); }
-        if (!pin_st) { memcpy(state + p.i0, h, p.cnt); h += vc_align(p.cnt); }
-        if (!pin_sum) { memcpy(summary + (size_t)p.i0 * 4, h, (size_t)p.cnt * 16); h += vc_align((size_t)p.cnt * 16); }
-        if (!pin_docs) memcpy(docs + p.base, h, p.bytes);
-        p.active = false;
-        return AFC_OK;
-    };
-    uint32_t i0 = 0;
-    uint64_t base = 0;
-    int which = 0;
-    while (i0 < n) {
-        const uint32_t left = n - i0;
-        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
-        if (limit < min_chunk) limit = min_chunk;
-        if (limit > max_chunk) limit = max_chunk;
-        uint32_t i1 = i0;
-        const uint64_t cbase = col_off[(size_t)i0 * C], r0 = rec_off[i0], rbase = rec_col_off[2 * r0];
-        while (i1 < n && i1 - i0 < limit) {
-            const uint64_t r = rec_off[i1 + 1];
-            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (rec_col_off[2 * r] - rbase) + 32 * (r - r0);
-            if (bytes > kChunkBytes && i1 != i0) break;
-            i1++;
-        }
-        const uint32_t cnt = i1 - i0;
-        const uint64_t r1 = rec_off[i1];
-        const uint32_t m = (uint32_t)(r1 - r0);
-        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, rbytes = rec_col_off[2 * r1] - rbase;
-        Slot& sl = lane.slot[which];
-        int rc = drain(which);
-        if (rc != AFC_OK) return rc;
-        const uint64_t dbound = wf_doc_bound(cnt, cbytes, m, rbytes);
-        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 4, ((size_t)cnt + 1) * 8, rbytes + 32, ((size_t)2 * m + 1) * 8,
-                             (size_t)m * 16, dbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 86, (size_t)cnt, (size_t)cnt * 16,
-                             wf_scratch_bytes(cnt, m, dbound)};
-        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
-        size_t total = 0;
-        for (size_t b : sz) total += vc_align(b);
-        CK(sl.vc.reserve(total));
-        uint8_t* q[NB];
-        {
-            uint8_t* p = sl.vc.p;
-            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
-        }
-        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_ki ? 0 : (size_t)cnt * 4,
-                                   pin_roff ? 0 : ((size_t)cnt + 1) * 8, pin_rcols ? 0 : rbytes, pin_rcoff ? 0 : ((size_t)2 * m + 1) * 8,
-                                   pin_cr ? 0 : (size_t)m * 16};
-        size_t bounce = 0;
-        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
-        CK(sl.h_in.reserve(bounce + 256, ctx));
-        CK(sl.h_out2.reserve(8, ctx));
-        size_t used = 0;
-        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
-        const uint64_t* d_coff = (const uint64_t*)q[1];
-        const uint32_t* d_ki = (const uint32_t*)q[2];
-        const uint64_t* d_roff = (const uint64_t*)q[3];
-        uint8_t* d_rcols = q[4] + (rbase & 15) - rbase;
-        const uint64_t* d_rcoff = (const uint64_t*)q[5] - 2 * r0;     // absolute record indices stay valid
-        const int64_t* d_cr = (const int64_t*)q[6] - 2 * r0;
-        uint8_t* d_docs = q[7];
-        uint64_t* d_doff = (uint64_t*)q[8];
-        uint8_t* d_pv = q[9];
-        uint8_t* d_st = q[10];
-        uint32_t* d_sum = (uint32_t*)q[11];
-        const WorkflowScratch S = wf_scratch(q[12], cnt, m, dbound);
-        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
-        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
-        CK(h2d(sl, q[2], key_index + i0, (size_t)cnt * 4, pin_ki, &used));
-        CK(h2d(sl, q[3], rec_off + i0, ((size_t)cnt + 1) * 8, pin_roff, &used));
-        if (m) {
-            CK(h2d(sl, q[4] + (rbase & 15), rec_cols + rbase, rbytes, pin_rcols, &used));
-            CK(h2d(sl, q[5], rec_col_off + 2 * r0, ((size_t)2 * m + 1) * 8, pin_rcoff, &used));
-            CK(h2d(sl, q[6], created + 2 * r0, (size_t)m * 16, pin_cr, &used));
-        }
-        CK(wf_sizes(d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_doff, d_sum, d_st, S, sl.stream, lc));
-        CK(cudaMemcpyAsync(sl.h_out2.p, d_doff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
-        CK(cudaStreamSynchronize(sl.stream));
-        uint64_t bytes;
-        memcpy(&bytes, sl.h_out2.p, 8);
-        CK(wf_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_docs, d_doff, d_pv, d_st, d_sum, S, sl.stream, lc));
-        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_pv ? 0 : vc_align((size_t)cnt * 86)) + (pin_st ? 0 : vc_align(cnt)) +
-                            (pin_sum ? 0 : vc_align((size_t)cnt * 16)) + (pin_docs ? 0 : bytes) + 256, ctx));
-        uint8_t* h = sl.h_out.p;
-        CK(cudaMemcpyAsync(h, d_doff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
-        h += vc_align(((size_t)cnt + 1) * 8);
-        CK(cudaMemcpyAsync(pin_pv ? pv + (size_t)i0 * 86 : h, d_pv, (size_t)cnt * 86, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_pv) h += vc_align((size_t)cnt * 86);
-        CK(cudaMemcpyAsync(pin_st ? state + i0 : h, d_st, cnt, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_st) h += vc_align(cnt);
-        CK(cudaMemcpyAsync(pin_sum ? (void*)(summary + (size_t)i0 * 4) : (void*)h, d_sum, (size_t)cnt * 16, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_sum) h += vc_align((size_t)cnt * 16);
-        if (bytes) CK(cudaMemcpyAsync(pin_docs ? docs + base : h, d_docs, bytes, cudaMemcpyDeviceToHost, sl.stream));
-        pend[which] = {i0, cnt, base, bytes, true};
-        base += bytes;
-        which = (which + 1) % kSlots;
-        i0 = i1;
-    }
-    for (int w = 0; w < kSlots; w++) {      // oldest first
-        int rc = drain((which + w) % kSlots);
-        if (rc != AFC_OK) return rc;
-    }
-    drain_on_exit.armed = false;
-    doc_off[n] = base;
     return AFC_OK;
 }
 
@@ -1692,16 +1639,59 @@ int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
     if (bad || docs_cap < afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n)) return AFC_EINVAL;
     if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    uint8_t* d_keys = nullptr;
-    CK(cudaMalloc(&d_keys, (size_t)n_keys * 96));
-    cudaError_t e = cudaMemcpy(d_keys, expanded96, (size_t)n_keys * 96, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        rc = wf_host_run(ctx, d_keys, n_keys, key_index, cols, col_off, rec_off, rec_cols, rec_col_off, created_at, n, docs, doc_off, proof_values, state,
-                         summary);
-    } else { set_err(ctx, e, "cudaMemcpy(expanded keys)"); rc = AFC_ECUDA; }
-    cudaMemset(d_keys, 0, (size_t)n_keys * 96);       // expanded private keys do not outlive the call on the device
-    cudaFree(d_keys);
-    return rc;
+    // Chunks of whole workflows through the ring, as for execution credentials.  A chunk's records travel with it (the kernels index them
+    // by absolute record, so the staged record arrays are addressed from a shifted base); a workflow larger than a chunk's byte budget
+    // goes alone.
+    const uint32_t C = AFC_WORKFLOW_COLUMNS;
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        const uint64_t r0 = rec_off[i0], r = rec_off[i + 1];
+        return (col_off[(size_t)(i + 1) * C] - col_off[(size_t)i0 * C]) + (rec_col_off[2 * r] - rec_col_off[2 * r0]) + 32 * (r - r0);
+    };
+    uint64_t base = 0;
+    return with_device_keys(ctx, expanded96, n_keys, [&](const uint8_t* d_keys) {
+        Ring ring(ctx);
+        return ring.walk(n, measure, [&](Ring& r) {
+            const uint32_t i0 = r.i0, cnt = r.cnt;
+            const uint64_t cbase = col_off[(size_t)i0 * C], cbytes = col_off[(size_t)(i0 + cnt) * C] - cbase;
+            const uint64_t r0 = rec_off[i0], rbase = rec_col_off[2 * r0], rbytes = rec_col_off[2 * rec_off[i0 + cnt]] - rbase;
+            const uint32_t m = (uint32_t)(rec_off[i0 + cnt] - r0);
+            const uint64_t dbound = wf_doc_bound(cnt, cbytes, m, rbytes);
+            const uint8_t *d_cols, *d_rcols;
+            const uint64_t *d_coff, *d_roff, *d_rcoff;
+            const uint32_t* d_ki;
+            const int64_t* d_cr;
+            uint8_t *d_docs, *d_pv, *d_st;
+            uint64_t* d_doff;
+            uint32_t* d_sum;
+            WorkflowScratch S;
+            RC(r.stage([&](Stager& k) {
+                d_cols = k.in_at(cols, cbase, cbytes, 16);
+                d_coff = k.in(col_off, (size_t)i0 * C, (size_t)cnt * C + 1);
+                d_ki = k.in(key_index, i0, cnt);
+                d_roff = k.in(rec_off, i0, (size_t)cnt + 1);
+                d_rcols = k.in_at(rec_cols, rbase, rbytes, 16);
+                d_rcoff = k.in(rec_col_off, 2 * r0, m ? 2 * (size_t)m + 1 : 0);
+                d_cr = k.in(created_at, 2 * r0, 2 * (size_t)m);
+                d_docs = k.take(dbound + 64);
+                d_doff = k.take<uint64_t>((size_t)cnt + 1);
+                d_pv = k.take((size_t)cnt * 86);
+                d_st = k.take(cnt);
+                d_sum = k.take<uint32_t>((size_t)cnt * 4);
+                wf_scratch(k, S, cnt, m, dbound);
+            }));
+            d_rcoff -= 2 * r0;                      // absolute record indices stay valid
+            d_cr -= 2 * r0;
+            CK(wf_sizes(d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_doff, d_sum, d_st, S, r.st, r.lc));
+            uint64_t bytes;
+            RC(r.read(&bytes, {d_doff + cnt}));
+            CK(wf_finish(ctx, d_keys, n_keys, d_ki, d_cols, d_coff, d_roff, d_rcols, d_rcoff, d_cr, cnt, m, d_docs, d_doff, d_pv, d_st, d_sum, S, r.st,
+                         r.lc));
+            RC(r.copy_back({offsets_out(doc_off, i0, d_doff, (size_t)cnt + 1, base), {proof_values, (size_t)i0 * 86, d_pv, (size_t)cnt * 86},
+                            {state, i0, d_st, cnt}, {summary, (size_t)i0 * 16, d_sum, (size_t)cnt * 16}, {docs, base, d_docs, bytes}}));
+            base += bytes;
+            return AFC_OK;
+        });
+    });
 }
 
 // ---------------------------------------------------------------------------------- webhook deliveries
@@ -1717,16 +1707,11 @@ uint64_t afc_webhook_bound(const uint64_t* col_off, const uint64_t* result_off, 
 
 // per-call device scratch: the result tapes, the plans, the HMACs, scan tiles
 struct WebhookScratch { uint32_t* tape; uint8_t* plan; uint8_t* mac; uint64_t* scan; };
-static size_t wh_scratch_bytes(uint32_t n, uint64_t result_bytes) {
-    return vc_align((result_bytes / 2 + 1) * 4) + vc_align(n) + vc_align((size_t)n * 32) + vc_align(launch::json_scan_scratch_bytes(n));
-}
-static WebhookScratch wh_scratch(uint8_t* p, uint32_t n, uint64_t result_bytes) {
-    WebhookScratch s;
-    s.tape = (uint32_t*)p; p += vc_align((result_bytes / 2 + 1) * 4);
-    s.plan = p; p += vc_align(n);
-    s.mac = p; p += vc_align((size_t)n * 32);
-    s.scan = (uint64_t*)p;
-    return s;
+static void wh_scratch(Carve& k, WebhookScratch& s, uint32_t n, uint64_t result_bytes) {
+    s.tape = k.take<uint32_t>(result_bytes / 2 + 1);
+    s.plan = k.take(n);
+    s.mac = k.take((size_t)n * 32);
+    s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
 }
 static cudaError_t wh_enqueue(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
                               const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, uint64_t* body_off,
@@ -1765,143 +1750,12 @@ int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64
     const uint64_t rb = ends[3] - ends[2];
     CallLog lc(ctx);
     uint8_t* scratch = nullptr;
-    CK(cudaMallocAsync((void**)&scratch, wh_scratch_bytes(n, rb), st));
+    WebhookScratch S;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { wh_scratch(k, S, n, rb); }));
     cudaError_t e = wh_enqueue(d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies, d_body_off,
-                               d_headers, d_status, wh_scratch(scratch, n, rb), st, lc);
+                               d_headers, d_status, S, st, lc);
     cudaFreeAsync(scratch, st);
     CK(e);
-    return AFC_OK;
-}
-
-// The host-buffer call: chunks of deliveries through the lane's ring, as issue_host_run does.  A chunk's stream is synchronised once
-// after the sizes pass to learn where its bodies end.  Staged secrets are wiped from the device slot after each chunk's headers and
-// from the pinned bounce buffer once the chunk is drained (or the call returns early).
-static int wh_host_run(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
-                       const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, uint64_t* body_off,
-                       uint8_t* headers, uint8_t* status) {
-    const uint32_t C = AFC_WEBHOOK_COLUMNS;
-    LaneGuard lg(ctx);
-    Lane& lane = lg.lane();
-    struct SecretBounce { uint8_t* p = nullptr; size_t bytes = 0; } bounce_sec[kSlots];
-    struct WipeOnExit {                     // runs after LaneDrain (declared before it): no copy still reads the bounce buffers
-        SecretBounce* b;
-        ~WipeOnExit() { for (int w = 0; w < kSlots; w++) if (b[w].bytes) memset(b[w].p, 0, b[w].bytes); }
-    } wipe{bounce_sec};
-    LaneDrain drain_on_exit(lane);
-    const bool pin_cols = is_pinned(cols), pin_coff = is_pinned(col_off), pin_dur = is_pinned(dur), pin_fl = is_pinned(flags);
-    const bool pin_res = is_pinned(res), pin_roff = is_pinned(res_off), pin_sec = is_pinned(sec), pin_soff = is_pinned(sec_off);
-    const bool pin_bodies = is_pinned(bodies), pin_h = is_pinned(headers), pin_st = is_pinned(status);
-    CallLog lc(ctx);
-    const uint32_t max_chunk = max_chunk_items(), min_chunk = min_chunk_items();
-    struct Pending { uint32_t i0, cnt; uint64_t base, bytes; bool active; } pend[kSlots] = {};
-    auto drain = [&](int w) -> int {
-        Pending& p = pend[w];
-        if (!p.active) return AFC_OK;
-        Slot& sl = lane.slot[w];
-        CK(cudaStreamSynchronize(sl.stream));
-        if (bounce_sec[w].bytes) { memset(bounce_sec[w].p, 0, bounce_sec[w].bytes); bounce_sec[w].bytes = 0; }
-        const uint8_t* h = sl.h_out.p;
-        const uint64_t* rel = (const uint64_t*)h; h += vc_align(((size_t)p.cnt + 1) * 8);
-        for (uint32_t j = 0; j < p.cnt; j++) body_off[p.i0 + j] = p.base + rel[j];
-        if (!pin_h) { memcpy(headers + (size_t)p.i0 * 71, h, (size_t)p.cnt * 71); h += vc_align((size_t)p.cnt * 71); }
-        if (!pin_st) { memcpy(status + p.i0, h, p.cnt); h += vc_align(p.cnt); }
-        if (!pin_bodies) memcpy(bodies + p.base, h, p.bytes);
-        p.active = false;
-        return AFC_OK;
-    };
-    uint32_t i0 = 0;
-    uint64_t base = 0;
-    int which = 0;
-    while (i0 < n) {
-        const uint32_t left = n - i0;
-        uint32_t limit = left <= min_chunk ? left : (left + 1) / 2;
-        if (limit < min_chunk) limit = min_chunk;
-        if (limit > max_chunk) limit = max_chunk;
-        uint32_t i1 = i0;
-        const uint64_t cbase = col_off[(size_t)i0 * C], rbase = res_off[i0];
-        while (i1 < n && i1 - i0 < limit) {
-            const uint64_t bytes = (col_off[(size_t)(i1 + 1) * C] - cbase) + (res_off[i1 + 1] - rbase);
-            if (bytes > kChunkBytes && i1 != i0) break;
-            i1++;
-        }
-        const uint32_t cnt = i1 - i0;
-        const uint64_t cbytes = col_off[(size_t)i1 * C] - cbase, rbytes = res_off[i1] - rbase;
-        const uint64_t kbase = sec_off[i0], kbytes = sec_off[i1] - kbase;
-        Slot& sl = lane.slot[which];
-        int rc = drain(which);
-        if (rc != AFC_OK) return rc;
-        const uint64_t bbound = wh_bound(cnt, cbytes + rbytes);
-        const size_t sz[] = {cbytes + 32, ((size_t)cnt * C + 1) * 8, (size_t)cnt * 8, (size_t)cnt, rbytes + 32, ((size_t)cnt + 1) * 8,
-                             kbytes + 32, ((size_t)cnt + 1) * 4, bbound + 64, ((size_t)cnt + 1) * 8, (size_t)cnt * 71, (size_t)cnt,
-                             wh_scratch_bytes(cnt, rbytes)};
-        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
-        size_t total = 0;
-        for (size_t b : sz) total += vc_align(b);
-        CK(sl.vc.reserve(total));
-        uint8_t* q[NB];
-        {
-            uint8_t* p = sl.vc.p;
-            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
-        }
-        const size_t in_bytes[] = {pin_cols ? 0 : cbytes, pin_coff ? 0 : ((size_t)cnt * C + 1) * 8, pin_dur ? 0 : (size_t)cnt * 8, pin_fl ? 0 : (size_t)cnt,
-                                   pin_res ? 0 : rbytes, pin_roff ? 0 : ((size_t)cnt + 1) * 8, pin_sec ? 0 : kbytes, pin_soff ? 0 : ((size_t)cnt + 1) * 4};
-        size_t bounce = 0;
-        for (size_t b : in_bytes) bounce += (b + 255) & ~(size_t)255;
-        CK(sl.h_in.reserve(bounce + 256, ctx));
-        CK(sl.h_out2.reserve(8, ctx));
-        size_t used = 0;
-        uint8_t* d_cols = q[0] + (cbase & 15) - cbase;          // absolute offsets stay valid, alignment as in the caller's buffer
-        const uint64_t* d_coff = (const uint64_t*)q[1];
-        const int64_t* d_dur = (const int64_t*)q[2];
-        const uint8_t* d_fl = q[3];
-        uint8_t* d_res = q[4] + (rbase & 15) - rbase;
-        const uint64_t* d_roff = (const uint64_t*)q[5];
-        uint8_t* d_sec = q[6] + (kbase & 3) - kbase;
-        const uint32_t* d_soff = (const uint32_t*)q[7];
-        uint8_t* d_bodies = q[8];
-        uint64_t* d_boff = (uint64_t*)q[9];
-        uint8_t* d_h = q[10];
-        uint8_t* d_st = q[11];
-        const WebhookScratch S = wh_scratch(q[12], cnt, rbytes);
-        CK(h2d(sl, q[0] + (cbase & 15), cols + cbase, cbytes, pin_cols, &used));
-        CK(h2d(sl, q[1], col_off + (size_t)i0 * C, ((size_t)cnt * C + 1) * 8, pin_coff, &used));
-        CK(h2d(sl, q[2], dur + i0, (size_t)cnt * 8, pin_dur, &used));
-        CK(h2d(sl, q[3], flags + i0, cnt, pin_fl, &used));
-        CK(h2d(sl, q[4] + (rbase & 15), res + rbase, rbytes, pin_res, &used));
-        CK(h2d(sl, q[5], res_off + i0, ((size_t)cnt + 1) * 8, pin_roff, &used));
-        if (!pin_sec && kbytes) bounce_sec[which] = {sl.h_in.p + used, (size_t)kbytes};
-        CK(h2d(sl, q[6] + (kbase & 3), sec + kbase, kbytes, pin_sec, &used));
-        CK(h2d(sl, q[7], sec_off + i0, ((size_t)cnt + 1) * 4, pin_soff, &used));
-        CK(launch::wh_sizes(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff + 1, d_st, sl.stream, lc));
-        CK(launch::offsets_from_lengths(d_boff, cnt, S.scan, sl.stream, lc));
-        CK(cudaMemcpyAsync(sl.h_out2.p, d_boff + cnt, 8, cudaMemcpyDeviceToHost, sl.stream));
-        CK(cudaStreamSynchronize(sl.stream));
-        uint64_t bytes;
-        memcpy(&bytes, sl.h_out2.p, 8);
-        CK(launch::wh_emit(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff, d_bodies, sl.stream, lc));
-        CK(launch::wh_sign(d_sec, d_soff, d_fl, d_st, d_bodies, d_boff, cnt, S.mac, d_h, sl.stream, lc));
-        if (kbytes) CK(cudaMemsetAsync(q[6], 0, kbytes + 32, sl.stream));          // secrets do not stay behind in the staging slot
-        CK(sl.h_out.reserve(vc_align(((size_t)cnt + 1) * 8) + (pin_h ? 0 : vc_align((size_t)cnt * 71)) + (pin_st ? 0 : vc_align(cnt)) +
-                            (pin_bodies ? 0 : bytes) + 256, ctx));
-        uint8_t* h = sl.h_out.p;
-        CK(cudaMemcpyAsync(h, d_boff, ((size_t)cnt + 1) * 8, cudaMemcpyDeviceToHost, sl.stream));
-        h += vc_align(((size_t)cnt + 1) * 8);
-        CK(cudaMemcpyAsync(pin_h ? headers + (size_t)i0 * 71 : h, d_h, (size_t)cnt * 71, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_h) h += vc_align((size_t)cnt * 71);
-        CK(cudaMemcpyAsync(pin_st ? status + i0 : h, d_st, cnt, cudaMemcpyDeviceToHost, sl.stream));
-        if (!pin_st) h += vc_align(cnt);
-        if (bytes) CK(cudaMemcpyAsync(pin_bodies ? bodies + base : h, d_bodies, bytes, cudaMemcpyDeviceToHost, sl.stream));
-        pend[which] = {i0, cnt, base, bytes, true};
-        base += bytes;
-        which = (which + 1) % kSlots;
-        i0 = i1;
-    }
-    for (int w = 0; w < kSlots; w++) {      // oldest first
-        int rc = drain((which + w) % kSlots);
-        if (rc != AFC_OK) return rc;
-    }
-    drain_on_exit.armed = false;
-    body_off[n] = base;
     return AFC_OK;
 }
 
@@ -1920,7 +1774,51 @@ int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* co
     if (bad || bodies_cap < afc_webhook_bound(col_off, result_off, n)) return AFC_EINVAL;
     if ((!results && result_off[n] != result_off[0]) || (!secrets && secret_off[n] != secret_off[0])) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    return wh_host_run(ctx, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off, n, bodies, body_off, headers, status);
+    // Chunks of deliveries through the ring, as for execution credentials: a chunk's stream is synchronised once after the sizes pass to
+    // learn where its bodies end.  The staged secrets are marked secret.
+    const uint32_t C = AFC_WEBHOOK_COLUMNS;
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        return (col_off[(size_t)(i + 1) * C] - col_off[(size_t)i0 * C]) + (result_off[i + 1] - result_off[i0]);
+    };
+    uint64_t base = 0;
+    Ring ring(ctx);
+    return ring.walk(n, measure, [&](Ring& r) {
+        const uint32_t i0 = r.i0, cnt = r.cnt;
+        const uint64_t cbase = col_off[(size_t)i0 * C], cbytes = col_off[(size_t)(i0 + cnt) * C] - cbase;
+        const uint64_t rbase = result_off[i0], rbytes = result_off[i0 + cnt] - rbase;
+        const uint8_t *d_cols, *d_fl, *d_res, *d_sec;
+        const uint64_t *d_coff, *d_roff;
+        const uint32_t* d_soff;
+        const int64_t* d_dur;
+        uint8_t *d_bodies, *d_h, *d_st;
+        uint64_t* d_boff;
+        WebhookScratch S;
+        RC(r.stage([&](Stager& k) {
+            d_cols = k.in_at(cols, cbase, cbytes, 16);
+            d_coff = k.in(col_off, (size_t)i0 * C, (size_t)cnt * C + 1);
+            d_dur = k.in(duration_ms, i0, cnt);
+            d_fl = k.in(flags, i0, cnt);
+            d_res = k.in_at(results, rbase, rbytes, 16);
+            d_roff = k.in(result_off, i0, (size_t)cnt + 1);
+            d_sec = k.in_at(secrets, secret_off[i0], secret_off[i0 + cnt] - secret_off[i0], 4, true);
+            d_soff = k.in(secret_off, i0, (size_t)cnt + 1);
+            d_bodies = k.take(wh_bound(cnt, cbytes + rbytes) + 64);
+            d_boff = k.take<uint64_t>((size_t)cnt + 1);
+            d_h = k.take((size_t)cnt * 71);
+            d_st = k.take(cnt);
+            wh_scratch(k, S, cnt, rbytes);
+        }));
+        CK(launch::wh_sizes(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff + 1, d_st, r.st, r.lc));
+        CK(launch::offsets_from_lengths(d_boff, cnt, S.scan, r.st, r.lc));
+        uint64_t bytes;
+        RC(r.read(&bytes, {d_boff + cnt}));
+        CK(launch::wh_emit(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff, d_bodies, r.st, r.lc));
+        CK(launch::wh_sign(d_sec, d_soff, d_fl, d_st, d_bodies, d_boff, cnt, S.mac, d_h, r.st, r.lc));
+        RC(r.copy_back({offsets_out(body_off, i0, d_boff, (size_t)cnt + 1, base), {headers, (size_t)i0 * 71, d_h, (size_t)cnt * 71},
+                        {status, i0, d_st, cnt}, {bodies, base, d_bodies, bytes}}));
+        base += bytes;
+        return AFC_OK;
+    });
 }
 
 // ---------------------------------------------------------------------------------- registering agent DIDs
@@ -1940,26 +1838,18 @@ uint64_t afc_did_register_bound(const uint64_t* node_off, const uint64_t* id_idx
     return didr_bound(n, nb, server_id_len, r1 - r0, d >= c ? d - c : 0);
 }
 
-// per-call device scratch (launch::DidrArgs), then the server id's bytes
-static size_t didr_scratch_bytes(uint32_t n, uint32_t m, uint64_t server_len) {
-    const size_t slots = (size_t)n + m;
-    return vc_align((size_t)m * 4) + vc_align(m) + vc_align((size_t)m * 8) + vc_align(((size_t)m + 1) * 8) + vc_align((size_t)m * 4) +
-           vc_align((size_t)m * 8) + vc_align((size_t)n * 16) + vc_align((size_t)n * 8) + vc_align(slots * 32) +
-           vc_align(launch::json_scan_scratch_bytes(n > m ? n : m)) + vc_align(server_len + 16);
-}
-static uint8_t* didr_scratch(launch::DidrArgs& A, uint8_t* p, uint32_t n, uint32_t m) {
-    auto take = [&](size_t b) { uint8_t* q = p; p += vc_align(b); return q; };
-    A.list = (uint32_t*)take((size_t)m * 4);
-    A.flags = take(m);
-    A.esc = (uint64_t*)take((size_t)m * 8);
-    A.nz = (uint64_t*)take(((size_t)m + 1) * 8);
-    A.rank = (uint32_t*)take((size_t)m * 4);
-    A.before = (uint64_t*)take((size_t)m * 8);
-    A.map_bytes = (uint64_t*)take((size_t)n * 16);
-    A.map_cnt = (uint32_t*)take((size_t)n * 8);
-    A.seeds = take(((size_t)n + m) * 32);
-    A.scan = (uint64_t*)take(launch::json_scan_scratch_bytes(n > m ? n : m));
-    return p;
+// per-call device scratch (launch::DidrArgs); the derived seeds are secret
+static void didr_scratch(Carve& k, launch::DidrArgs& A, uint32_t n, uint32_t m) {
+    A.list = k.take<uint32_t>(m);
+    A.flags = k.take(m);
+    A.esc = k.take<uint64_t>(m);
+    A.nz = k.take<uint64_t>((size_t)m + 1);
+    A.rank = k.take<uint32_t>(m);
+    A.before = k.take<uint64_t>(m);
+    A.map_bytes = k.take<uint64_t>((size_t)n * 2);
+    A.map_cnt = k.take<uint32_t>((size_t)n * 2);
+    A.seeds = k.take(((size_t)n + m) * 32, true);
+    A.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n > m ? n : m));
 }
 
 int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* d_node_ids,
@@ -1990,9 +1880,12 @@ int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const
     if (ends[5] > ends[4] && !d_ids) return AFC_EINVAL;
     if (body_cap < didr_bound(n, ends[1] - ends[0], server_id_len, m, ends[5] - ends[4])) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
-    CK(cudaMallocAsync((void**)&scratch, didr_scratch_bytes(n, m, server_id_len), st));
     launch::DidrArgs A{};
-    uint8_t* d_server = didr_scratch(A, scratch, n, m);
+    uint8_t* d_server;
+    CK(pool_carve(&scratch, st, [&](Carve& k) {
+        didr_scratch(k, A, n, m);
+        d_server = k.take(server_id_len + 16);
+    }));
     A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
     A.master = d_master_seed; A.h = did_hash(server_id, server_id_len) & 0x7fffffffu; A.server = d_server; A.server_len = server_id_len;
     A.nodes = d_node_ids; A.node_off = d_node_off; A.agent_index = d_agent_index; A.id_idx = d_id_idx; A.ids = d_ids; A.id_off = d_id_off;
@@ -2008,17 +1901,16 @@ int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const
     return AFC_OK;
 }
 
-// Device bytes one chunk stages (didr_host_run's reservation, to within alignment): inputs, per component its outputs (96 + 32 + 55 + 48 + 1)
-// and seed, per id its scratch, and the body bound.  kChunkBytes caps this; a request over it goes alone.
+// Device bytes one chunk stages (its arena, to within alignment): inputs, per component its outputs (96 + 32 + 55 + 48 + 1) and seed, per id
+// its scratch, and the body bound.  kChunkBytes caps this; a request over it goes alone.
 static uint64_t didr_chunk_bytes(uint32_t cnt, uint64_t nbytes, uint64_t server_len, uint64_t mc, uint64_t ibytes) {
     return nbytes + ibytes + 64 * (uint64_t)cnt + 48 * mc + 264 * ((uint64_t)cnt + mc) + didr_bound(cnt, nbytes, server_len, mc, ibytes);
 }
 
-// The host-buffer call: chunks of whole requests through one slot of the lane, each staged, run, copied back and wiped before the next
-// (the expansion dominates, so there is little copy time to overlap).  A chunk's ids travel with it: the kernels index them by absolute id,
-// so the staged arrays are addressed from a shifted base.  A request larger than a chunk's byte budget goes alone.
-// Secrets in the slot: the staged master seed (device and its pinned bounce), the expanded keys, the seeds and the bodies (every private
-// JWK).  They are wiped after each chunk's copy-back and, on any early return, by the guard below, after the lane has drained.
+// The host-buffer call: chunks of whole requests through one slot of the ring, one after another (the expansion dominates, so there is
+// little copy time to overlap).  A chunk's ids travel with it: the kernels index them by absolute id, so the staged arrays are addressed
+// from a shifted base.  A request larger than a chunk's byte budget goes alone.  The master seed, the derived seeds, the expanded keys and
+// the bodies (every private JWK) are secret.
 int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* node_ids,
                            const uint64_t* node_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint8_t* ids, const uint64_t* id_off,
                            uint32_t n, uint64_t* comp_off, uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* comp_flags,
@@ -2035,127 +1927,62 @@ int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8
     if (bad || (id_off[r_last] > id_off[r_first] && !ids)) return AFC_EINVAL;
     if (body_cap < afc_did_register_bound(node_off, id_idx, id_off, n, server_id_len)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    LaneGuard lg(ctx);
-    Lane& lane = lg.lane();
-    Slot& sl = lane.slot[0];
-    struct StagedSecrets {
-        Slot& sl;
-        uint8_t* dev[4] = {};
-        size_t dev_bytes[4] = {};
-        uint8_t* host = nullptr;
-        size_t host_bytes = 0;
-        cudaError_t wipe() {
-            cudaError_t e = cudaSuccess;
-            for (int k = 0; k < 4; k++) {
-                if (!dev_bytes[k]) continue;
-                const cudaError_t w = cudaMemsetAsync(dev[k], 0, dev_bytes[k], sl.stream);
-                if (e == cudaSuccess) e = w;
-                dev_bytes[k] = 0;
-            }
-            const cudaError_t w = cudaStreamSynchronize(sl.stream);
-            if (e == cudaSuccess) e = w;
-            if (host_bytes) { memset(host, 0, host_bytes); host_bytes = 0; }     // after the sync: no copy still reads it
-            return e;
-        }
-        ~StagedSecrets() { wipe(); }                      // runs after LaneDrain (declared before it)
-    } secrets{sl};
-    LaneDrain drain_on_exit(lane);
-    CallLog lc(ctx);
-    const bool pin_nodes = is_pinned(node_ids), pin_ids = ids && is_pinned(ids), pin_ioff = is_pinned(id_off);
     const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
-    const uint32_t max_chunk = max_chunk_items();
-    const uint64_t total_slots = (uint64_t)n + (r_last - r_first);
-    uint32_t i0 = 0;
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        const uint64_t r0 = id_idx[2 * (size_t)i0], r = id_idx[2 * (size_t)i + 2];
+        return didr_chunk_bytes(i + 1 - i0, node_off[i + 1] - node_off[i0], server_id_len, r - r0, id_off[r] - id_off[r0]);
+    };
     uint64_t cbase = 0, bbase = 0;
-    while (i0 < n) {
-        const uint64_t nb0 = node_off[i0], r0 = id_idx[2 * (size_t)i0], ib0 = id_off[r0];
-        uint32_t i1 = i0;
-        while (i1 < n && i1 - i0 < max_chunk) {
-            const uint64_t r = id_idx[2 * (size_t)i1 + 2];
-            const uint64_t bytes = didr_chunk_bytes(i1 + 1 - i0, node_off[i1 + 1] - nb0, server_id_len, r - r0, id_off[r] - ib0);
-            if (bytes > kChunkBytes && i1 != i0) break;
-            i1++;
-        }
-        const uint32_t cnt = i1 - i0;
-        const uint64_t r1 = id_idx[2 * (size_t)i1];
-        const uint32_t mc = (uint32_t)(r1 - r0);
-        const size_t slots = (size_t)cnt + mc;
-        const uint64_t nbytes = node_off[i1] - nb0, ibytes = id_off[r1] - ib0;
-        const uint64_t dbound = didr_bound(cnt, nbytes, server_id_len, mc, ibytes);
-        const size_t sz[] = {nbytes + 32, ((size_t)cnt + 1) * 8, (size_t)cnt * 4, ((size_t)2 * cnt + 1) * 8, ibytes + 32, ((size_t)mc + 1) * 8, 32,
-                             ((size_t)cnt + 1) * 8, slots * 96, slots * 32, slots * AFC_DID_CHARS, slots * AFC_DID_PATH_SLOT, slots, dbound + 64,
-                             ((size_t)cnt + 1) * 8, didr_scratch_bytes(cnt, mc, server_id_len)};
-        constexpr int NB = sizeof(sz) / sizeof(sz[0]);
-        size_t total = 0;
-        for (size_t b : sz) total += vc_align(b);
-        CK(sl.vc.reserve(total));
-        uint8_t* q[NB];
-        {
-            uint8_t* p = sl.vc.p;
-            for (int k = 0; k < NB; k++) { q[k] = p; p += vc_align(sz[k]); }
-        }
-        CK(sl.h_in.reserve(vc_align(nbytes) + vc_align(ibytes) + vc_align(((size_t)mc + 1) * 8) + vc_align(sz[1]) + vc_align(sz[2]) + vc_align(sz[3]) +
-                           vc_align(32) + vc_align(server_id_len) + 256, ctx));
-        CK(sl.h_out2.reserve(16, ctx));
-        size_t used = 0;
-        launch::DidrArgs A{};
-        uint8_t* d_server = didr_scratch(A, q[15], cnt, mc);
-        A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
-        A.master = q[6]; A.h = h; A.server = d_server; A.server_len = server_id_len;
-        A.nodes = q[0] + (nb0 & 15) - nb0;                        // absolute offsets stay valid, alignment as in the caller's buffer
-        A.node_off = (const uint64_t*)q[1];
-        A.agent_index = (const uint32_t*)q[2];
-        A.id_idx = (const uint64_t*)q[3];
-        A.ids = q[4] + (ib0 & 15) - ib0;
-        A.id_off = (const uint64_t*)q[5] - r0;                    // absolute id indices stay valid
-        A.n = cnt; A.m = mc;
-        A.comp_off = (uint64_t*)q[7]; A.expanded96 = q[8]; A.pks = q[9]; A.dids = q[10]; A.paths = q[11]; A.comp_flags = q[12];
-        A.body = q[13]; A.body_off = (uint64_t*)q[14];
-        CK(h2d(sl, q[0] + (nb0 & 15), node_ids + nb0, nbytes, pin_nodes, &used));
-        CK(h2d(sl, q[1], node_off + i0, sz[1], false, &used));
-        CK(h2d(sl, q[2], agent_index + i0, sz[2], false, &used));
-        CK(h2d(sl, q[3], id_idx + 2 * (size_t)i0, sz[3], false, &used));
-        if (ibytes) CK(h2d(sl, q[4] + (ib0 & 15), ids + ib0, ibytes, pin_ids, &used));
-        CK(h2d(sl, q[5], id_off + r0, sz[5], pin_ioff, &used));
-        secrets.dev[0] = q[6]; secrets.dev_bytes[0] = 32;
-        secrets.dev[1] = q[8]; secrets.dev_bytes[1] = slots * 96;
-        secrets.dev[2] = A.seeds; secrets.dev_bytes[2] = slots * 32;
-        secrets.dev[3] = q[13]; secrets.dev_bytes[3] = dbound + 64;
-        secrets.host = sl.h_in.p + used; secrets.host_bytes = 32;     // where h2d bounces the master seed
-        CK(h2d(sl, q[6], master_seed, 32, false, &used));
-        CK(h2d(sl, d_server, server_id, server_id_len, false, &used));
-        cudaError_t e = launch::didr_register(A, sl.stream, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(sl.h_out2.p, A.comp_off + cnt, 8, cudaMemcpyDeviceToHost, sl.stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(sl.h_out2.p + 8, A.body_off + cnt, 8, cudaMemcpyDeviceToHost, sl.stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(sl.stream);
-        uint64_t cc = 0, bb = 0;
-        if (e == cudaSuccess) { memcpy(&cc, sl.h_out2.p, 8); memcpy(&bb, sl.h_out2.p + 8, 8); }
-        auto d2h = [&](void* dst, const void* src, size_t bytes) {
-            if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, sl.stream);
-        };
-        d2h(comp_off + i0, A.comp_off, ((size_t)cnt + 1) * 8);
-        d2h(expanded96 + 96 * cbase, A.expanded96, cc * 96);
-        d2h(pks + 32 * cbase, A.pks, cc * 32);
-        d2h(dids + AFC_DID_CHARS * cbase, A.dids, cc * AFC_DID_CHARS);
-        d2h(paths + AFC_DID_PATH_SLOT * cbase, A.paths, cc * AFC_DID_PATH_SLOT);
-        d2h(comp_flags + cbase, A.comp_flags, cc);
-        d2h(body + bbase, A.body, bb);
-        d2h(body_off + i0, A.body_off, ((size_t)cnt + 1) * 8);
-        // the staged master seed, expanded keys, seeds and bodies are wiped whatever happened above
-        const cudaError_t w = secrets.wipe();
-        CK(e); CK(w);
-        for (uint32_t k = 0; k <= cnt; k++) { comp_off[i0 + k] += cbase; body_off[i0 + k] += bbase; }
-        cbase += cc;
-        bbase += bb;
-        i0 = i1;
+    {
+        Ring ring(ctx, 1);
+        RC(ring.walk(n, measure, [&](Ring& r) {
+            const uint32_t i0 = r.i0, cnt = r.cnt;
+            const uint64_t nb0 = node_off[i0], r0 = id_idx[2 * (size_t)i0], ib0 = id_off[r0], r1 = id_idx[2 * (size_t)(i0 + cnt)];
+            const uint32_t mc = (uint32_t)(r1 - r0);
+            const size_t slots = (size_t)cnt + mc;
+            const uint64_t nbytes = node_off[i0 + cnt] - nb0, ibytes = id_off[r1] - ib0;
+            launch::DidrArgs A{};
+            RC(r.stage([&](Stager& k) {
+                A.nodes = k.in_at(node_ids, nb0, nbytes, 16);
+                A.node_off = k.in(node_off, i0, (size_t)cnt + 1);
+                A.agent_index = k.in(agent_index, i0, cnt);
+                A.id_idx = k.in(id_idx, 2 * (size_t)i0, 2 * (size_t)cnt + 1);
+                A.ids = k.in_at(ids, ib0, ibytes, 16);
+                A.id_off = k.in(id_off, r0, (size_t)mc + 1);
+                A.master = k.in(master_seed, 0, 32, true);
+                A.server = k.in(server_id, 0, server_id_len);
+                A.comp_off = k.take<uint64_t>((size_t)cnt + 1);
+                A.expanded96 = k.take(slots * 96, true);
+                A.pks = k.take(slots * 32);
+                A.dids = k.take(slots * AFC_DID_CHARS);
+                A.paths = k.take(slots * AFC_DID_PATH_SLOT);
+                A.comp_flags = k.take(slots);
+                A.body = k.take(didr_bound(cnt, nbytes, server_id_len, mc, ibytes) + 64, true);
+                A.body_off = k.take<uint64_t>((size_t)cnt + 1);
+                didr_scratch(k, A, cnt, mc);
+            }));
+            A.id_off -= r0;                         // absolute id indices stay valid
+            A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+            A.h = h; A.server_len = server_id_len;
+            A.n = cnt; A.m = mc;
+            CK(launch::didr_register(A, r.st, r.lc));
+            uint64_t end[2];                        // components, body bytes
+            RC(r.read(end, {A.comp_off + cnt, A.body_off + cnt}));
+            RC(r.copy_back({offsets_out(comp_off, i0, A.comp_off, (size_t)cnt + 1, cbase), {expanded96, 96 * cbase, A.expanded96, end[0] * 96, true},
+                            {pks, 32 * cbase, A.pks, end[0] * 32}, {dids, AFC_DID_CHARS * cbase, A.dids, end[0] * AFC_DID_CHARS},
+                            {paths, AFC_DID_PATH_SLOT * cbase, A.paths, end[0] * AFC_DID_PATH_SLOT}, {comp_flags, cbase, A.comp_flags, end[0]},
+                            {body, bbase, A.body, end[1], true}, offsets_out(body_off, i0, A.body_off, (size_t)cnt + 1, bbase)}));
+            cbase += end[0];
+            bbase += end[1];
+            return AFC_OK;
+        }));
     }
-    const size_t tail = (size_t)(total_slots - cbase);            // the empty ids' entries: zeros, as the _dev call leaves them
+    const size_t tail = (size_t)((uint64_t)n + (r_last - r_first) - cbase);     // the empty ids' entries: zeros, as the _dev call leaves them
     memset(expanded96 + 96 * cbase, 0, tail * 96);
     memset(pks + 32 * cbase, 0, tail * 32);
     memset(dids + AFC_DID_CHARS * cbase, 0, tail * AFC_DID_CHARS);
     memset(paths + AFC_DID_PATH_SLOT * cbase, 0, tail * AFC_DID_PATH_SLOT);
     memset(comp_flags + cbase, 0, tail);
-    drain_on_exit.armed = false;
     return AFC_OK;
 }
 
@@ -2195,7 +2022,7 @@ static int merkle_append_hashes_locked(afc_merkle* m, const uint8_t* d_h, uint32
     afc_ctx* ctx = m->ctx;
     if (n == 0) return AFC_OK;
     if (!aligned16(d_h)) return AFC_EINVAL;
-    CallLog lc(ctx, 72);
+    CallLog lc(ctx);
     uint64_t s = m->size, e = m->size + n;
     const uint8_t* cur = d_h;
     int h = 0, pp = 0;
@@ -2345,7 +2172,7 @@ static int tree_build_common(afc_ctx* ctx, const uint8_t* src, bool src_is_devic
     afc_merkle_tree* t = new (std::nothrow) afc_merkle_tree();
     if (!t) return AFC_ENOMEM;
     t->ctx = ctx; t->n = n;
-    CallLog lc(ctx, 72);
+    CallLog lc(ctx);
     cudaError_t e = cudaSuccess;
     uint64_t cur = n;
     while (e == cudaSuccess) {
@@ -2676,16 +2503,13 @@ int afc_staging_find(afc_ctx* ctx, const uint8_t* pattern, uint32_t len, uint64_
         for (int w = 0; w < kSlots; w++) {
             Slot& sl = ctx->lanes[i].slot[w];
             if (sl.stream) CK(cudaStreamSynchronize(sl.stream));
-            DevBuf* dev[] = {&sl.msgs, &sl.off, &sl.a, &sl.b, &sl.k, &sl.out, &sl.koff, &sl.vc};
-            for (DevBuf* d : dev) {
-                for (size_t at = 0; at < d->cap; at += kPiece) {      // pieces overlap by len - 1 bytes, so no match is cut in two
-                    const size_t n = d->cap - at < kPiece + len - 1 ? d->cap - at : kPiece + len - 1;
-                    host.resize(n);
-                    CK(cudaMemcpy(host.data(), d->p + at, n, cudaMemcpyDeviceToHost));
-                    scan(host.data(), n);
-                }
+            for (size_t at = 0; at < sl.arena.cap; at += kPiece) {      // pieces overlap by len - 1 bytes, so no match is cut in two
+                const size_t n = sl.arena.cap - at < kPiece + len - 1 ? sl.arena.cap - at : kPiece + len - 1;
+                host.resize(n);
+                CK(cudaMemcpy(host.data(), sl.arena.p + at, n, cudaMemcpyDeviceToHost));
+                scan(host.data(), n);
             }
-            PinBuf* pin[] = {&sl.h_in, &sl.h_out, &sl.h_out2};
+            PinBuf* pin[] = {&sl.h_in, &sl.h_out};
             for (PinBuf* b : pin) if (b->p) scan(b->p, b->cap);
         }
     }
