@@ -30,6 +30,8 @@ WEBHOOK_HAS_DURATION, WEBHOOK_HAS_ERROR_MESSAGE, WEBHOOK_HAS_SECRET = 1, 2, 4
 WEBHOOK_BUILT, WEBHOOK_HOST = 0, 1
 WEBHOOK_HEADER_CHARS = 71
 DID_CHARS, DID_PATH_SLOT, DID_KEPT = 55, 48, 1
+DIDRR_UNCHANGED, DIDRR_REMOVED, DIDRR_PARTIAL, DIDRR_INVALID = 0, 1, 2, 3
+DIDRR_GONE, DIDRR_NEW = 1, 2
 MERKLE_STATE_BYTES = 8 + 64 * 32
 SHA256_STATE_BYTES = 108
 
@@ -105,6 +107,9 @@ SYMBOLS = {
     "afc_did_register_batch": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp]),
     "afc_did_register_batch_dev": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp,
                                              vp]),
+    "afc_did_reregister_bound": (C.c_uint64, [vp, vp, vp, vp, vp, C.c_uint32, C.c_uint64]),
+    "afc_did_reregister_batch": (C.c_int, [vp, vp, vp, C.c_uint64] + [vp] * 9 + [C.c_uint32] + [vp] * 9 + [C.c_uint64, vp]),
+    "afc_did_reregister_batch_dev": (C.c_int, [vp, vp, vp, C.c_uint64] + [vp] * 9 + [C.c_uint32] + [vp] * 9 + [C.c_uint64, vp, vp]),
     "afc_merkle_new": (C.c_int, [vp, C.POINTER(vp)]),
     "afc_merkle_free": (None, [vp]),
     "afc_merkle_append": (C.c_int, [vp, vp, vp, C.c_uint32, vp, u64p]),

@@ -182,6 +182,36 @@ cudaError_t didr_register(const DidrArgs& A, cudaStream_t s, LaunchLog* lg);
 uint64_t didr_req_fixed();             // the body bound's constant per request and per id (afc_didreg.cuh)
 uint64_t didr_per_id_fixed();
 
+// ---- k_didrereg.cu: known agents re-registered on the device (afc_didrereg.cuh).  agent_col_off: 3n + 1 absolute offsets; id_idx and
+// reg_idx: 2n + 1 absolute indices (request i's reasoners [x[2i], x[2i+1]), skills [x[2i+1], x[2i+2])); id_off absolute, indexed by
+// absolute id; reg_col_off absolute, component g's five columns at 5g .. 5g + 5.  The m = id_idx[2n] - id_idx[0] ids and the
+// G = reg_idx[2n] - reg_idx[0] components have per-item scratch; the key slots are 2n.
+struct DidrrArgs {
+    const void* comb; const void* ct16;                  // ed_expand_batch's tables (ct16 nullptr: variable-time expansion)
+    const uint8_t* master;                               // 32 bytes, 16-byte aligned
+    uint32_t h;                                          // didr_server_hash of the server id
+    const uint8_t* server; uint64_t server_len;          // the server id's bytes, on the device
+    const uint8_t* agent_cols; const uint64_t* agent_col_off; const uint32_t* agent_index;
+    const uint64_t* id_idx; const uint8_t* ids; const uint64_t* id_off;
+    const uint64_t* reg_idx; const uint8_t* reg_cols; const uint64_t* reg_col_off;
+    uint32_t n, m, G;
+    // outputs (expanded96, pks, paths 16-byte aligned): per request state, counts (4); per key slot expanded96, pks, dids, paths; per
+    // component reg_flags, per id id_flags; the bodies
+    uint8_t* state; uint32_t* counts; uint8_t* expanded96; uint8_t* pks; uint8_t* dids; uint8_t* paths; uint8_t* reg_flags; uint8_t* id_flags;
+    uint8_t* body; uint64_t* body_off;
+    // scratch: rflags, ebytes per component; iflags, esc per id; rank, before per component and id (G + m); bad, agent_bytes per request;
+    // map_bytes, map_cnt 4n (the surviving maps, then the new ones); seeds 32 per key slot (16-byte aligned); scan json_scan_scratch_bytes(n)
+    uint8_t* rflags; uint64_t* ebytes; uint8_t* iflags; uint64_t* esc; uint32_t* rank; uint64_t* before; uint32_t* bad; uint64_t* agent_bytes;
+    uint64_t* map_bytes; uint32_t* map_cnt; uint8_t* seeds; uint64_t* scan;
+};
+// out: agent_col_off at 0 and 3n, id_idx at 0 and 2n, id_off at both, reg_idx at 0 and 2n, reg_col_off at five times both (one thread)
+cudaError_t didrr_ends(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx, const uint64_t* reg_col_off,
+                       uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
+// every pass; the seeds scratch holds the derived seeds when it has run (the caller wipes it)
+cudaError_t didrr_reregister(const DidrrArgs& A, cudaStream_t s, LaunchLog* lg);
+uint64_t didrr_req_fixed();            // the body bound's constant per request and per registered component (afc_didrereg.cuh)
+uint64_t didrr_per_reg_fixed();
+
 // ---- k_ed25519.cu
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();

@@ -1986,6 +1986,192 @@ int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8
     return AFC_OK;
 }
 
+// ---------------------------------------------------------------------------------- re-registering known agents
+// Bounds from the five offset arrays' ends alone (afc_didrereg.cuh): per request its frame with the longest message and the agent's stored
+// identity, 6 bytes per agent-column and server-id byte; per request id what afc_did_register_bound allows it; per registered component
+// its stored entry, 6 bytes per column byte.  Every body lists either the survivors or the new ids, so the bound only gains there.
+static uint64_t didrr_bound(uint32_t n, uint64_t agent_bytes, uint64_t server_len, uint64_t m, uint64_t id_bytes, uint64_t G, uint64_t reg_bytes) {
+    return (uint64_t)n * (launch::didrr_req_fixed() + 6 * server_len) + 6 * agent_bytes + m * launch::didr_per_id_fixed() + 12 * id_bytes +
+           G * launch::didrr_per_reg_fixed() + 6 * reg_bytes;
+}
+
+uint64_t afc_did_reregister_bound(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
+                                  const uint64_t* reg_col_off, uint32_t n, uint64_t server_id_len) {
+    if (!agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || n == 0) return 0;
+    const uint64_t a = agent_col_off[0], b = agent_col_off[3 * (size_t)n];
+    const uint64_t r0 = id_idx[0], r1 = id_idx[2 * (size_t)n], g0 = reg_idx[0], g1 = reg_idx[2 * (size_t)n];
+    uint64_t m = 0, ib = 0, G = 0, rb = 0;
+    if (r1 >= r0) {
+        const uint64_t c = id_off[r0], d = id_off[r1];
+        m = r1 - r0; ib = d >= c ? d - c : 0;
+    }
+    if (g1 >= g0) {
+        const uint64_t c = reg_col_off[5 * g0], d = reg_col_off[5 * g1];
+        G = g1 - g0; rb = d >= c ? d - c : 0;
+    }
+    return didrr_bound(n, b >= a ? b - a : 0, server_id_len, m, ib, G, rb);
+}
+
+// per-call device scratch (launch::DidrrArgs); the derived seeds are secret
+static void didrr_scratch(Carve& k, launch::DidrrArgs& A, uint32_t n, uint32_t m, uint32_t G) {
+    A.rflags = k.take(G);
+    A.ebytes = k.take<uint64_t>(G);
+    A.iflags = k.take(m);
+    A.esc = k.take<uint64_t>(m);
+    A.rank = k.take<uint32_t>((size_t)G + m);
+    A.before = k.take<uint64_t>((size_t)G + m);
+    A.bad = k.take<uint32_t>(n);
+    A.agent_bytes = k.take<uint64_t>(n);
+    A.map_bytes = k.take<uint64_t>((size_t)n * 4);
+    A.map_cnt = k.take<uint32_t>((size_t)n * 4);
+    A.seeds = k.take((size_t)n * 64, true);
+    A.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
+}
+
+int afc_did_reregister_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* d_agent_cols,
+                                 const uint64_t* d_agent_col_off, const uint32_t* d_agent_index, const uint64_t* d_id_idx, const uint8_t* d_ids,
+                                 const uint64_t* d_id_off, const uint64_t* d_reg_idx, const uint8_t* d_reg_cols, const uint64_t* d_reg_col_off, uint32_t n,
+                                 uint8_t* d_state, uint32_t* d_counts, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids, uint8_t* d_paths,
+                                 uint8_t* d_reg_flags, uint8_t* d_id_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream) {
+    if (!ctx || !d_agent_col_off || !d_id_idx || !d_id_off || !d_reg_idx || !d_reg_col_off || !d_body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!d_master_seed || !d_agent_cols || !d_agent_index || !d_state || !d_counts || !d_expanded96 || !d_pks || !d_dids || !d_paths || !d_body ||
+        (server_id_len && !server_id))
+        return AFC_EINVAL;
+    if (!aligned16(d_master_seed) || !aligned16(d_expanded96) || !aligned16(d_pks) || !aligned16(d_paths)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies: gathered by one thread, read once
+    {
+        uint64_t* d_ends = nullptr;
+        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
+        cudaError_t e = launch::didrr_ends(d_agent_col_off, d_id_idx, d_id_off, d_reg_idx, d_reg_col_off, n, d_ends, st, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(d_ends, st);
+        CK(e);
+        CK(cudaStreamSynchronize(st));
+    }
+    for (int k = 0; k < 10; k += 2)
+        if (ends[k + 1] < ends[k]) return AFC_EINVAL;
+    if ((ends[3] - ends[2]) + (ends[7] - ends[6]) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
+    const uint32_t m = (uint32_t)(ends[3] - ends[2]), G = (uint32_t)(ends[7] - ends[6]);
+    if ((ends[5] > ends[4] && !d_ids) || (ends[9] > ends[8] && !d_reg_cols) || (m && !d_id_flags) || (G && !d_reg_flags)) return AFC_EINVAL;
+    if (body_cap < didrr_bound(n, ends[1] - ends[0], server_id_len, m, ends[5] - ends[4], G, ends[9] - ends[8])) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    launch::DidrrArgs A{};
+    uint8_t* d_server;
+    CK(pool_carve(&scratch, st, [&](Carve& k) {
+        didrr_scratch(k, A, n, m, G);
+        d_server = k.take(server_id_len + 16);
+    }));
+    A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+    A.master = d_master_seed; A.h = did_hash(server_id, server_id_len) & 0x7fffffffu; A.server = d_server; A.server_len = server_id_len;
+    A.agent_cols = d_agent_cols; A.agent_col_off = d_agent_col_off; A.agent_index = d_agent_index;
+    A.id_idx = d_id_idx; A.ids = d_ids; A.id_off = d_id_off; A.reg_idx = d_reg_idx; A.reg_cols = d_reg_cols; A.reg_col_off = d_reg_col_off;
+    A.n = n; A.m = m; A.G = G;
+    A.state = d_state; A.counts = d_counts; A.expanded96 = d_expanded96; A.pks = d_pks; A.dids = d_dids; A.paths = d_paths;
+    A.reg_flags = d_reg_flags; A.id_flags = d_id_flags; A.body = d_body; A.body_off = d_body_off;
+    cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
+    if (e == cudaSuccess) e = launch::didrr_reregister(A, st, lc);
+    const cudaError_t wipe = cudaMemsetAsync(A.seeds, 0, (size_t)n * 64, st);             // derived seeds do not outlive the call
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    CK(wipe);
+    return AFC_OK;
+}
+
+// Device bytes one chunk stages (its arena, to within alignment): inputs and their offsets, per request its outputs and two key slots
+// (2 x (96 + 32 + 55 + 48) + a seed each) and scratch, per id and component its flags and scratch, and the body bound.  kChunkBytes caps
+// this; a request over it goes alone.
+static uint64_t didrr_chunk_bytes(uint32_t cnt, uint64_t abytes, uint64_t server_len, uint64_t mc, uint64_t ibytes, uint64_t gc, uint64_t rbytes) {
+    return abytes + ibytes + rbytes + 8 * (8 * (uint64_t)cnt + mc + 5 * gc) + 640 * (uint64_t)cnt + 32 * (mc + gc) +
+           didrr_bound(cnt, abytes, server_len, mc, ibytes, gc, rbytes);
+}
+
+// The host-buffer call: chunks of whole requests through one slot of the ring, one after another, as afc_did_register_batch runs.  The
+// kernels index ids and components by absolute index, so their staged arrays are addressed from shifted bases.  The master seed, the
+// derived seeds, the expanded keys and the bodies (the private JWKs of new components) are secret.
+int afc_did_reregister_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* agent_cols,
+                             const uint64_t* agent_col_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint8_t* ids, const uint64_t* id_off,
+                             const uint64_t* reg_idx, const uint8_t* reg_cols, const uint64_t* reg_col_off, uint32_t n, uint8_t* state, uint32_t* counts,
+                             uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* reg_flags, uint8_t* id_flags, uint8_t* body,
+                             uint64_t body_cap, uint64_t* body_off) {
+    if (!ctx || !agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || !body_off) return AFC_EINVAL;
+    if (n == 0) { body_off[0] = 0; return AFC_OK; }
+    if (!master_seed || !agent_cols || !agent_index || !state || !counts || !expanded96 || !pks || !dids || !paths || !body ||
+        (server_id_len && !server_id))
+        return AFC_EINVAL;
+    if (!monotone(agent_col_off, 3 * n) || !monotone(id_idx, 2 * n) || !monotone(reg_idx, 2 * n)) return AFC_EINVAL;
+    const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n], g_first = reg_idx[0], g_last = reg_idx[2 * (size_t)n];
+    if ((r_last - r_first) + (g_last - g_first) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
+    uint64_t bad = 0;
+    for (uint64_t k = r_first; k < r_last; k++) bad |= (uint64_t)(id_off[k + 1] < id_off[k]);
+    for (uint64_t k = 5 * g_first; k < 5 * g_last; k++) bad |= (uint64_t)(reg_col_off[k + 1] < reg_col_off[k]);
+    if (bad || (id_off[r_last] > id_off[r_first] && !ids) || (reg_col_off[5 * g_last] > reg_col_off[5 * g_first] && !reg_cols) ||
+        (r_last > r_first && !id_flags) || (g_last > g_first && !reg_flags))
+        return AFC_EINVAL;
+    if (body_cap < afc_did_reregister_bound(agent_col_off, id_idx, id_off, reg_idx, reg_col_off, n, server_id_len)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        const uint64_t r0 = id_idx[2 * (size_t)i0], r = id_idx[2 * (size_t)i + 2], g0 = reg_idx[2 * (size_t)i0], g = reg_idx[2 * (size_t)i + 2];
+        return didrr_chunk_bytes(i + 1 - i0, agent_col_off[3 * (size_t)i + 3] - agent_col_off[3 * (size_t)i0], server_id_len, r - r0, id_off[r] - id_off[r0],
+                                 g - g0, reg_col_off[5 * g] - reg_col_off[5 * g0]);
+    };
+    uint64_t bbase = 0;
+    Ring ring(ctx, 1);
+    return ring.walk(n, measure, [&](Ring& r) {
+        const uint32_t i0 = r.i0, cnt = r.cnt;
+        const uint64_t ac0 = agent_col_off[3 * (size_t)i0], abytes = agent_col_off[3 * (size_t)(i0 + cnt)] - ac0;
+        const uint64_t r0 = id_idx[2 * (size_t)i0], r1 = id_idx[2 * (size_t)(i0 + cnt)], ib0 = id_off[r0], ibytes = id_off[r1] - ib0;
+        const uint64_t g0 = reg_idx[2 * (size_t)i0], g1 = reg_idx[2 * (size_t)(i0 + cnt)], rb0 = reg_col_off[5 * g0], rbytes = reg_col_off[5 * g1] - rb0;
+        const uint32_t mc = (uint32_t)(r1 - r0), gc = (uint32_t)(g1 - g0);
+        const size_t slots = 2 * (size_t)cnt;
+        launch::DidrrArgs A{};
+        RC(r.stage([&](Stager& k) {
+            A.agent_cols = k.in_at(agent_cols, ac0, abytes, 16);
+            A.agent_col_off = k.in(agent_col_off, 3 * (size_t)i0, 3 * (size_t)cnt + 1);
+            A.agent_index = k.in(agent_index, i0, cnt);
+            A.id_idx = k.in(id_idx, 2 * (size_t)i0, 2 * (size_t)cnt + 1);
+            A.ids = k.in_at(ids, ib0, ibytes, 16);
+            A.id_off = k.in(id_off, r0, (size_t)mc + 1);
+            A.reg_idx = k.in(reg_idx, 2 * (size_t)i0, 2 * (size_t)cnt + 1);
+            A.reg_cols = k.in_at(reg_cols, rb0, rbytes, 16);
+            A.reg_col_off = k.in(reg_col_off, 5 * g0, 5 * (size_t)gc + 1);
+            A.master = k.in(master_seed, 0, 32, true);
+            A.server = k.in(server_id, 0, server_id_len);
+            A.state = k.take(cnt);
+            A.counts = k.take<uint32_t>(4 * (size_t)cnt);
+            A.expanded96 = k.take(slots * 96, true);
+            A.pks = k.take(slots * 32);
+            A.dids = k.take(slots * AFC_DID_CHARS);
+            A.paths = k.take(slots * AFC_DID_PATH_SLOT);
+            A.reg_flags = k.take(gc);
+            A.id_flags = k.take(mc);
+            A.body = k.take(didrr_bound(cnt, abytes, server_id_len, mc, ibytes, gc, rbytes) + 64, true);
+            A.body_off = k.take<uint64_t>((size_t)cnt + 1);
+            didrr_scratch(k, A, cnt, mc, gc);
+        }));
+        A.id_off -= r0;                             // absolute indices stay valid
+        A.reg_col_off -= 5 * g0;
+        A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+        A.h = h; A.server_len = server_id_len;
+        A.n = cnt; A.m = mc; A.G = gc;
+        CK(launch::didrr_reregister(A, r.st, r.lc));
+        uint64_t bytes;
+        RC(r.read(&bytes, {A.body_off + cnt}));
+        RC(r.copy_back({{state, i0, A.state, cnt}, {counts, (size_t)i0 * 16, A.counts, (size_t)cnt * 16},
+                        {expanded96, 2 * (size_t)i0 * 96, A.expanded96, slots * 96, true}, {pks, 2 * (size_t)i0 * 32, A.pks, slots * 32},
+                        {dids, 2 * (size_t)i0 * AFC_DID_CHARS, A.dids, slots * AFC_DID_CHARS},
+                        {paths, 2 * (size_t)i0 * AFC_DID_PATH_SLOT, A.paths, slots * AFC_DID_PATH_SLOT},
+                        {reg_flags, g0 - g_first, A.reg_flags, gc}, {id_flags, r0 - r_first, A.id_flags, mc},
+                        {body, bbase, A.body, bytes, true}, offsets_out(body_off, i0, A.body_off, (size_t)cnt + 1, bbase)}));
+        bbase += bytes;
+        return AFC_OK;
+    });
+}
+
 // ---------------------------------------------------------------------------------- Merkle log
 int afc_merkle_new(afc_ctx* ctx, afc_merkle** out) {
     if (!ctx || !out) return AFC_EINVAL;

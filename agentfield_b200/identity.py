@@ -383,6 +383,164 @@ class ExpandedKeys:
             out.append({"body": body[int(R["body_off"][i]):int(R["body_off"][i + 1])], "components": comps})
         return out
 
+    # -- known agents re-registered (afc_did_reregister_batch)
+    REREG_COLUMNS = ("did", "public_key_jwk", "derivation_path", "function_name")
+
+    @staticmethod
+    def pack_reregister_requests(requests):
+        """Re-registrations of known agents ({"agent": {"did", "public_key_jwk", "derivation_path", "reasoners", "skills"}, "reasoners":
+        [ids], "skills": [ids]}; the agent's "reasoners" and "skills" map each key to {"did", "public_key_jwk", "derivation_path",
+        "function_name"}, as a dict or as (key, value) pairs; str or bytes as in pack_register_requests) -> the host arrays of
+        afc_did_reregister_batch: (agent_cols, agent_col_off, id_idx, ids, id_off, reg_idx, reg_cols, reg_col_off)."""
+        def b(v):
+            return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+
+        def pairs(m):
+            return list(m.items()) if isinstance(m, dict) else list(m)
+        acols, flat, idx, rflat, ridx = [], [], [0], [], [0]
+        for r in requests:
+            a = r["agent"]
+            acols += [b(a["did"]), b(a["public_key_jwk"]), b(a["derivation_path"])]
+            for kind in ("reasoners", "skills"):
+                flat += [b(x) for x in r.get(kind) or ()]
+                idx.append(len(flat))
+                for key, c in pairs(a.get(kind) or ()):
+                    rflat += [b(key)] + [b(c.get(k) or b"") for k in ExpandedKeys.REREG_COLUMNS]
+                ridx.append(len(rflat) // 5)
+        agent_cols, agent_col_off = pack(acols)
+        ids, id_off = pack(flat)
+        reg_cols, reg_col_off = pack(rflat)
+        return (agent_cols, agent_col_off, np.array(idx, dtype=np.uint64), ids, id_off, np.array(ridx, dtype=np.uint64), reg_cols, reg_col_off)
+
+    def _append_slots(self, state, counts, expanded, dids):
+        """The key slots that received a new component join this cache under their DIDs."""
+        n = len(state)
+        live = [t for t in range(2 * n) if state[t >> 1] == _abi.DIDRR_PARTIAL and counts[t >> 1][t & 1]]
+        if live:
+            self._append(expanded[live], [dids[t].tobytes().decode() for t in live])
+
+    def reregister_packed(self, master_seed, server_id, agent_cols, agent_col_off, agent_index, id_idx, ids, id_off, reg_idx, reg_cols, reg_col_off,
+                          append=True):
+        """afc_did_reregister_batch on host arrays (the layout of pack_reregister_requests; agent_index uint32 [n]).  Returns a dict: state
+        uint8 [n] (_abi.DIDRR_*), counts uint32 [n, 4], expanded uint8 [2n, 96], pks [2n, 32], dids [2n, 55], paths [2n, 48] (key slot 2i + 0
+        for reasoners, 2i + 1 for skills), reg_flags uint8 [G] (_abi.DIDRR_GONE), id_flags uint8 [m] (_abi.DIDRR_NEW | _abi.DID_KEPT), body
+        uint8, body_off uint64 [n+1].  With append the keys of the slots in use join this cache under their DIDs."""
+        n = len(agent_index)
+        sid = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
+        if len(master_seed) != 32:
+            raise ValueError("the master seed is 32 bytes")
+        lib = _abi.load()
+        m = int(id_idx[2 * n]) - int(id_idx[0]) if n else 0
+        G = int(reg_idx[2 * n]) - int(reg_idx[0]) if n else 0
+        cap = lib.afc_did_reregister_bound(_abi.ptr(agent_col_off), _abi.ptr(id_idx), _abi.ptr(id_off), _abi.ptr(reg_idx), _abi.ptr(reg_col_off), n,
+                                           len(sid))
+        out = {"state": np.zeros(n, dtype=np.uint8), "counts": np.zeros((n, 4), dtype=np.uint32), "expanded": np.empty((2 * n, 96), dtype=np.uint8),
+               "pks": np.empty((2 * n, 32), dtype=np.uint8), "dids": np.empty((2 * n, _abi.DID_CHARS), dtype=np.uint8),
+               "paths": np.empty((2 * n, _abi.DID_PATH_SLOT), dtype=np.uint8), "reg_flags": np.zeros(G, dtype=np.uint8),
+               "id_flags": np.zeros(m, dtype=np.uint8), "body": np.empty(max(cap, 1), dtype=np.uint8), "body_off": np.zeros(n + 1, dtype=np.uint64)}
+        ms = np.frombuffer(bytes(master_seed), dtype=np.uint8).copy()
+        ai = np.ascontiguousarray(agent_index, dtype=np.uint32)
+        _abi.check(lib.afc_did_reregister_batch(self.ctx.handle, _abi.ptr(ms), sid, len(sid), _abi.ptr(agent_cols), _abi.ptr(agent_col_off), _abi.ptr(ai),
+                                                _abi.ptr(id_idx), _abi.ptr(ids), _abi.ptr(id_off), _abi.ptr(reg_idx), _abi.ptr(reg_cols),
+                                                _abi.ptr(reg_col_off), n, _abi.ptr(out["state"]), _abi.ptr(out["counts"]), _abi.ptr(out["expanded"]),
+                                                _abi.ptr(out["pks"]), _abi.ptr(out["dids"]), _abi.ptr(out["paths"]), _abi.ptr(out["reg_flags"]),
+                                                _abi.ptr(out["id_flags"]), _abi.ptr(out["body"]), cap, _abi.ptr(out["body_off"])), self.ctx.handle)
+        ms[:] = 0
+        out["body"] = out["body"][:int(out["body_off"][n])]
+        if append:
+            self._append_slots(out["state"], out["counts"], out["expanded"], out["dids"])
+        return out
+
+    def reregister_dev(self, d_master_seed, server_id, d_agent_cols, d_agent_col_off, d_agent_index, d_id_idx, d_ids, d_id_off, d_reg_idx, d_reg_cols,
+                       d_reg_col_off, n, stream=None, append=True):
+        """afc_did_reregister_batch_dev: n requests on the device (int64 offset arrays, int32 agent indices, a 32-byte uint8 master seed).
+        Returns a dict of device tensors as reregister_packed returns arrays (body_off int64, counts int32).  With append the keys of the
+        slots in use are copied into this cache under their DIDs."""
+        import torch
+        dev = d_agent_col_off.device
+        sid = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
+        lib = _abi.load()
+        m = G = cap = 0
+        if n:
+            r0, r1, g0, g1 = int(d_id_idx[0]), int(d_id_idx[2 * n]), int(d_reg_idx[0]), int(d_reg_idx[2 * n])
+            m, G = r1 - r0, g1 - g0
+            aoff = np.array([0, 0, 0, int(d_agent_col_off[3 * n]) - int(d_agent_col_off[0])], dtype=np.uint64)
+            ioff = np.zeros(m + 1, dtype=np.uint64)
+            ioff[m] = int(d_id_off[r1]) - int(d_id_off[r0])
+            roff = np.zeros(5 * G + 1, dtype=np.uint64)
+            roff[5 * G] = int(d_reg_col_off[5 * g1]) - int(d_reg_col_off[5 * g0])
+            iidx, ridx = np.array([0, 0, m], dtype=np.uint64), np.array([0, 0, G], dtype=np.uint64)
+            zero = np.zeros(4, dtype=np.uint64)                   # an empty request: every end 0
+            cap = lib.afc_did_reregister_bound(_abi.ptr(aoff), _abi.ptr(iidx), _abi.ptr(ioff), _abi.ptr(ridx), _abi.ptr(roff), 1, len(sid))
+            cap += (n - 1) * lib.afc_did_reregister_bound(*[_abi.ptr(zero)] * 5, 1, len(sid))
+        e = lambda shape, dt=torch.uint8: torch.empty(shape, dtype=dt, device=dev)  # noqa: E731
+        out = {"state": e(n), "counts": e((n, 4), torch.int32), "expanded": e((2 * n, 96)), "pks": e((2 * n, 32)), "dids": e((2 * n, _abi.DID_CHARS)),
+               "paths": e((2 * n, _abi.DID_PATH_SLOT)), "reg_flags": e(G), "id_flags": e(m), "body": e(max(cap, 1)),
+               "body_off": torch.zeros(n + 1, dtype=torch.int64, device=dev)}
+        _abi.check(lib.afc_did_reregister_batch_dev(self.ctx.handle, _abi.ptr(d_master_seed), sid, len(sid), _abi.ptr(d_agent_cols),
+                                                    _abi.ptr(d_agent_col_off), _abi.ptr(d_agent_index), _abi.ptr(d_id_idx), _abi.ptr(d_ids),
+                                                    _abi.ptr(d_id_off), _abi.ptr(d_reg_idx), _abi.ptr(d_reg_cols), _abi.ptr(d_reg_col_off), n,
+                                                    _abi.ptr(out["state"]), _abi.ptr(out["counts"]), _abi.ptr(out["expanded"]), _abi.ptr(out["pks"]),
+                                                    _abi.ptr(out["dids"]), _abi.ptr(out["paths"]), _abi.ptr(out["reg_flags"]), _abi.ptr(out["id_flags"]),
+                                                    _abi.ptr(out["body"]), cap, _abi.ptr(out["body_off"]), self.ctx._stream(stream)), self.ctx.handle)
+        if n:
+            out["body"] = out["body"][:int(out["body_off"][n])]
+            if append:
+                self._append_slots(out["state"].cpu().numpy(), out["counts"].cpu().numpy(), out["expanded"].cpu().numpy(), out["dids"].cpu().numpy())
+        return out
+
+    @staticmethod
+    def agent_index_of(derivation_path):
+        """The <a> of an agent's stored path m/44'/<h>'/<a>': the index its new components' paths take (the reference's own choice, the
+        agent's place in Go's randomised map iteration, changes from run to run)."""
+        p = derivation_path.decode() if isinstance(derivation_path, (bytes, bytearray)) else derivation_path
+        parts = p.split("/")
+        if len(parts) != 4 or parts[0] != "m" or parts[1] != "44'" or not parts[3].endswith("'") or not parts[3][:-1].isdigit():
+            raise ValueError("not an agent derivation path: %r" % p)
+        return int(parts[3][:-1]) & 0xFFFFFFFF
+
+    def reregister(self, master_seed, server_id, requests):
+        """RegisterAgent for many known agents in one host-buffer call (pack_reregister_requests' requests; "agent_index" overrides the <a>
+        read from the agent's stored path).  Returns per request {"state", "counts", "body", "gone": [reasoners, skills] of bools in the
+        agent's order, "new": [reasoners, skills] of the ids the registry adds (the kept occurrences), "slots": [reasoners, skills] of None or
+        {"did", "pk", "path", "public_key_jwk"}}."""
+        n = len(requests)
+        if n == 0:
+            return []
+        ai = np.array([r["agent_index"] if "agent_index" in r else self.agent_index_of(r["agent"]["derivation_path"]) for r in requests],
+                      dtype=np.uint64).astype(np.uint32)
+        A = self.pack_reregister_requests(requests)
+        R = self.reregister_packed(master_seed, server_id, A[0], A[1], ai, *A[2:])
+        body = R["body"].tobytes()
+        out = []
+        g = k = 0
+        for i, r in enumerate(requests):
+            res = {"state": int(R["state"][i]), "counts": [int(x) for x in R["counts"][i]], "body": body[int(R["body_off"][i]):int(R["body_off"][i + 1])],
+                   "gone": [], "new": [], "slots": []}
+            for kind in ("reasoners", "skills"):
+                regs = r["agent"].get(kind) or ()
+                res["gone"].append([bool(f & _abi.DIDRR_GONE) for f in R["reg_flags"][g:g + len(regs)]])
+                g += len(regs)
+                ids = list(r.get(kind) or ())
+                fl = R["id_flags"][k:k + len(ids)]
+                res["new"].append([x for x, f in zip(ids, fl) if f == _abi.DIDRR_NEW | _abi.DID_KEPT])
+                k += len(ids)
+            for t in (2 * i, 2 * i + 1):
+                if res["state"] == _abi.DIDRR_PARTIAL and res["counts"][t & 1]:
+                    pk = R["pks"][t].tobytes()
+                    res["slots"].append({"did": R["dids"][t].tobytes().decode(), "pk": pk, "path": R["paths"][t].tobytes().rstrip(b"\0").decode(),
+                                         "public_key_jwk": public_jwk(pk)})
+                else:
+                    res["slots"].append(None)
+            out.append(res)
+        return out
+
+
+def public_jwk(pk: bytes) -> bytes:
+    """The public JWK text handleNewRegistration and PartialRegisterAgent store (json.Marshal of a map: keys sorted)."""
+    x = base64.urlsafe_b64encode(pk).rstrip(b"=")
+    return b'{"alg":"EdDSA","crv":"Ed25519","kty":"OKP","use":"sig","x":"' + x + b'"}'
+
 
 _EPOCH = datetime.datetime(1970, 1, 1, tzinfo=datetime.timezone.utc)
 

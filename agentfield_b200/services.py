@@ -23,7 +23,7 @@ import numpy as np
 
 from . import _abi, go_json
 from .crypto import Hasher, MAC, default_context, pack, pack32
-from .identity import ExpandedKeys, KeySet
+from .identity import ExpandedKeys, KeySet, public_jwk
 
 
 def _b64url(b: bytes) -> str:
@@ -867,8 +867,11 @@ def _is_rfc3339(ts: str) -> bool:
 class DIDService:
     """The registration half of the reference's DIDService (control-plane/internal/services/did_service.go:186-365, 653-723) over one
     registry: its server id, master seed and agent nodes.  Every new agent's keys, DIDs and DIDRegistrationResponse come from one
-    afc_did_register_batch call (ExpandedKeys.register), and the keys join `keys`, so the agents can issue credentials at once.
-    PartialRegisterAgent (new components of a known agent) is not mirrored."""
+    afc_did_register_batch call (ExpandedKeys.register), and the keys join `keys`, so the agents can issue credentials at once.  Known
+    agents take RegisterAgent's other branch (:154-179: the differential analysis, DeregisterComponents, PartialRegisterAgent or the
+    existing identity package) through one afc_did_reregister_batch call (ExpandedKeys.reregister); register_agents takes a mixed batch.
+    The agent index of a known agent's new components is the <a> of its own stored path (the reference uses its place in Go's randomised
+    map iteration)."""
 
     def __init__(self, keys: ExpandedKeys, master_seed: bytes, server_id):
         if len(master_seed) != 32:
@@ -876,7 +879,9 @@ class DIDService:
         self.keys = keys
         self.master_seed = bytes(master_seed)
         self.server_id = server_id.encode() if isinstance(server_id, str) else bytes(server_id)
-        self.agent_nodes = {}     # node id (bytes) -> {"did", "derivation_path", "reasoners": {id: did}, "skills": {id: did}}
+        # node id (bytes) -> {"did", "derivation_path", "public_key_jwk", "reasoners": {id: component}, "skills": {id: component}}, a
+        # component being {"did", "derivation_path", "public_key_jwk", "function_name"}: what the existing identity package needs
+        self.agent_nodes = {}
 
     @staticmethod
     def _node_key(v):
@@ -886,16 +891,19 @@ class DIDService:
         results = self.keys.register(self.master_seed, self.server_id, requests, len(self.agent_nodes))
         for r, res in zip(requests, results):
             comps = res["components"]
-            entry = {"did": comps[0]["did"], "derivation_path": comps[0]["path"], "reasoners": {}, "skills": {}}
+            entry = {"did": comps[0]["did"], "derivation_path": comps[0]["path"], "public_key_jwk": public_jwk(comps[0]["pk"]), "reasoners": {},
+                     "skills": {}}
             for c in comps[1:]:
                 if c["kept"]:
-                    entry["reasoners" if c["type"] == "reasoner" else "skills"][self._node_key(c["id"])] = c["did"]
+                    k = self._node_key(c["id"])
+                    entry["reasoners" if c["type"] == "reasoner" else "skills"][k] = {"did": c["did"], "derivation_path": c["path"],
+                                                                                     "public_key_jwk": public_jwk(c["pk"]), "function_name": k}
             self.agent_nodes[self._node_key(r["agent_node_id"])] = entry
         return results
 
     def register_agents_batch(self, requests):
         """handleNewRegistration for new agents, in order (request k gets agent index len(registry) + k).  A node id already registered,
-        or repeated in the batch, raises ValueError: that is PartialRegisterAgent's case.  Returns per request {"body", "components"}."""
+        or repeated in the batch, raises ValueError: a known node takes reregister_agents_batch or register_agents.  Returns per request {"body", "components"}."""
         seen = set()
         for r in requests:
             k = self._node_key(r["agent_node_id"])
@@ -915,3 +923,56 @@ class DIDService:
             seen.add(k)
             todo.append(r)
         return self._register(todo) if todo else []
+
+    def _reregister(self, requests):
+        reqs = []
+        for r in requests:
+            a = self.agent_nodes[self._node_key(r["agent_node_id"])]
+            reqs.append({"agent": a, "reasoners": r.get("reasoners") or (), "skills": r.get("skills") or ()})
+        results = self.keys.reregister(self.master_seed, self.server_id, reqs)
+        for q, res in zip(reqs, results):                         # the registry update: GONE first, then the kept NEW ids
+            a = q["agent"]
+            for kind, name in ((0, "reasoners"), (1, "skills")):
+                for key, gone in zip(list(a[name]), res["gone"][kind]):
+                    if gone:
+                        del a[name][key]
+                slot = res["slots"][kind]
+                for x in res["new"][kind]:
+                    k = self._node_key(x)
+                    a[name][k] = {"did": slot["did"], "derivation_path": slot["path"], "public_key_jwk": slot["public_key_jwk"], "function_name": k}
+        return results
+
+    def _distinct(self, requests):
+        seen = set()
+        for r in requests:
+            k = self._node_key(r["agent_node_id"])
+            if k in seen:
+                raise ValueError("agent node %r is named twice in one batch" % k)
+            seen.add(k)
+
+    def reregister_agents_batch(self, requests):
+        """RegisterAgent for agents the registry holds ({"agent_node_id", "reasoners", "skills"}): the removed components leave the registry
+        and the new ones join it with their keys (which join `keys`).  An unknown node, or one named twice, raises ValueError.  Returns per
+        request {"state", "counts", "body", "gone", "new", "slots"} (ExpandedKeys.reregister)."""
+        self._distinct(requests)
+        for r in requests:
+            if self._node_key(r["agent_node_id"]) not in self.agent_nodes:
+                raise ValueError("agent node %r is not registered" % self._node_key(r["agent_node_id"]))
+        return self._reregister(requests) if requests else []
+
+    def register_agents(self, requests):
+        """RegisterAgent over a mixed batch: new nodes through one afc_did_register_batch call (request order gives their agent indices),
+        known nodes through one afc_did_reregister_batch call.  A node named twice raises ValueError (the reference handles requests one
+        after another, so a second request for a node would see the first one's result).  Returns the results in request order: those of
+        register_agents_batch for new nodes, of reregister_agents_batch for known ones."""
+        self._distinct(requests)
+        known = [k for k, r in enumerate(requests) if self._node_key(r["agent_node_id"]) in self.agent_nodes]
+        fresh = [k for k, r in enumerate(requests) if self._node_key(r["agent_node_id"]) not in self.agent_nodes]
+        out = [None] * len(requests)
+        if known:
+            for k, res in zip(known, self._reregister([requests[k] for k in known])):
+                out[k] = res
+        if fresh:
+            for k, res in zip(fresh, self._register([requests[k] for k in fresh])):
+                out[k] = res
+        return out

@@ -481,6 +481,60 @@ int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const
                                const uint64_t* d_id_off, uint32_t n, uint64_t* d_comp_off, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids,
                                uint8_t* d_paths, uint8_t* d_comp_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream);
 
+/* ---- K3: known agents re-registered in one call: RegisterAgent's branch for an agent the registry holds (internal/services/
+ * did_service.go:154-179): PerformDifferentialAnalysis (:757-847), then buildExistingIdentityPackage (:940-986) when nothing changed,
+ * DeregisterComponents (:1239-1324) for the removed components, and PartialRegisterAgent (:1049-1236) for the new ones.  The call holds
+ * no registry: the caller passes each agent's record and applies the flags below to its registry.
+ * Inputs per request i (strings as in afc_did_register_batch: packed bytes and absolute offsets):
+ *   master_seed / server_id      as in afc_did_register_batch
+ *   agent_cols / agent_col_off   3 strings per request (3n + 1 offsets): the stored did, public_key_jwk and derivation_path of the agent
+ *   agent_index                  n values: the <a> of the new components' paths m/44'/<h>'/<a>'/<0|1>'/<j>'.  The reference takes the
+ *                                agent's place in Go's randomised iteration over the registry; a stable choice is the <a> of the agent's
+ *                                own stored derivation path
+ *   id_idx / ids / id_off        the request's reasoner and skill ids, laid out as in afc_did_register_batch
+ *   reg_idx / reg_cols / reg_col_off   the registered components: request i's reasoners are [reg_idx[2i], reg_idx[2i+1]), its skills
+ *                                [reg_idx[2i+1], reg_idx[2i+2]); component g has 5 strings at reg_col_off[5g .. 5g+5]: its map key, did,
+ *                                stored public_key_jwk, derivation_path and function_name
+ * Outputs per request:
+ *   state[i]        AFC_DIDRR_UNCHANGED (nothing new or removed), AFC_DIDRR_REMOVED (removals only), AFC_DIDRR_PARTIAL (new components),
+ *                   AFC_DIDRR_INVALID (a registered list holds one key twice, which no Go map can: refused, with an empty body, zero
+ *                   counts, flags and key slots)
+ *   counts[4i ..]   new reasoners, new skills (distinct ids: the maps' sizes), removed reasoners, removed skills
+ *   body[body_off[i] .. body_off[i+1])   json.Marshal(types.DIDRegistrationResponse): for UNCHANGED and REMOVED the existing identity package
+ *                   of the surviving components (every private_key_jwk "", public_key_jwk as stored, function_name omitted when empty);
+ *                   for PARTIAL only the new components, each with its private JWK; the agent's own identity always as stored
+ *   key slots 2i + kind (kind 0 reasoners, 1 skills): expanded96[96 ..], pks[32 ..], dids[55 ..], paths[48 ..] of the one key every new
+ *                   component of that kind receives (its path index j is the map's size after the removals, as in the reference); zeros
+ *                   where the request adds none
+ * Outputs per component and id:
+ *   reg_flags[g - reg_idx[0]]   AFC_DIDRR_GONE: DeregisterComponents removes it
+ *   id_flags[r - id_idx[0]]     AFC_DIDRR_NEW for a new id, with AFC_DID_KEPT on the occurrence the map keeps (the last)
+ * The caller's registry update: delete the GONE components, then add each NEW + KEPT id with its slot's DID, path and public key.
+ * body_cap must be at least afc_did_reregister_bound(...), computed from the ends of the five offset arrays and additive over requests (else
+ * AFC_EINVAL, before any work).  Other AFC_EINVAL: a NULL pointer, more than 2^32 - 1 ids, components or key slots; in the host-buffer call
+ * also offsets that run backwards.  Naming one node twice in a batch has no defined result (the reference handles requests one after
+ * another): the caller must not.  Chunking, secrets (the master seed, derived seeds, expanded keys and bodies are wiped from staging
+ * memory), alignment, the single synchronisation of the _dev call and n = 0 are as in afc_did_register_batch. */
+#define AFC_DIDRR_UNCHANGED 0
+#define AFC_DIDRR_REMOVED 1
+#define AFC_DIDRR_PARTIAL 2
+#define AFC_DIDRR_INVALID 3
+#define AFC_DIDRR_GONE 1
+#define AFC_DIDRR_NEW 2
+uint64_t afc_did_reregister_bound(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
+                                  const uint64_t* reg_col_off, uint32_t n, uint64_t server_id_len);
+int afc_did_reregister_batch(afc_ctx* ctx, const uint8_t* master_seed /* 32 */, const uint8_t* server_id, uint64_t server_id_len,
+                             const uint8_t* agent_cols, const uint64_t* agent_col_off /* 3n+1 */, const uint32_t* agent_index /* n */,
+                             const uint64_t* id_idx /* 2n+1 */, const uint8_t* ids, const uint64_t* id_off, const uint64_t* reg_idx /* 2n+1 */,
+                             const uint8_t* reg_cols, const uint64_t* reg_col_off, uint32_t n, uint8_t* state /* n */, uint32_t* counts /* 4n */,
+                             uint8_t* expanded96 /* 2n x 96 */, uint8_t* pks /* 2n x 32 */, uint8_t* dids /* 2n x 55 */, uint8_t* paths /* 2n x 48 */,
+                             uint8_t* reg_flags, uint8_t* id_flags, uint8_t* body, uint64_t body_cap, uint64_t* body_off /* n+1 */);
+int afc_did_reregister_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* d_agent_cols,
+                                 const uint64_t* d_agent_col_off, const uint32_t* d_agent_index, const uint64_t* d_id_idx, const uint8_t* d_ids,
+                                 const uint64_t* d_id_off, const uint64_t* d_reg_idx, const uint8_t* d_reg_cols, const uint64_t* d_reg_col_off, uint32_t n,
+                                 uint8_t* d_state, uint32_t* d_counts, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids, uint8_t* d_paths,
+                                 uint8_t* d_reg_flags, uint8_t* d_id_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream);
+
 /* ---- N4: audit proofs for bulk offline verification (`af vc verify`, internal/cli/vc.go:159-331; export bundles,
  * internal/handlers/ui/did.go:533-865) ------------------------------------------------------------------------
  * afc_merkle_tree materialises every level over a fixed set of leaf hashes (device memory, ~2n x 32 B) so that RFC 6962

@@ -8,6 +8,7 @@ documents in three client spellings (afc_vc_verify_json_batch_dev) next to the s
 issue_execution block measures execution credentials issued in one call (afc_vc_issue_execution_batch[_dev]).  The webhook block
 measures webhook deliveries built and signed in one call (afc_webhook_sign_batch[_dev]) next to HMAC alone over the same bodies.
 The issue_workflow block measures workflow credentials issued in one call (afc_vc_issue_workflow_batch[_dev]) next to the host-built path.
+The reregister block measures known agents re-registered in one call (afc_did_reregister_batch[_dev]) in a restart storm.
 Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
@@ -642,12 +643,104 @@ def register_block(ctx, dev, timed):
             "cpu_new_key_from_seed": {"keys": cpu_n, "threads": threads, "s": s_cpu, "keys_per_s": cpu_n / s_cpu}}
 
 
+def reregister_requests(n, rng, skew=None):
+    """A restart storm: n known agents, each with 0-32 registered reasoners and 0-32 skills (as handleNewRegistration stored them, in the
+    canonical JWK spelling), re-registering: about 90 % unchanged, 5 % removals only, 5 % partial (new ids, some with removals).
+    skew = (fraction, reasoners) gives that fraction of the agents that many registered reasoners."""
+    verbs = [b"summarize", b"translate", b"classify", b"extract", b"rank", b"plan"]
+    out = []
+    for i in range(n):
+        nr, ns = int(rng.integers(0, 33)), int(rng.integers(0, 33))
+        if skew and rng.random() < skew[0]:
+            nr = skew[1]
+        agent = {"did": b"did:key:z%046d" % i, "public_key_jwk": b'{"alg":"EdDSA","crv":"Ed25519","kty":"OKP","use":"sig","x":"%043d"}' % i,
+                 "derivation_path": b"m/44'/1234567'/%d'" % i}
+        for name, cnt, kind, w in (("reasoners", nr, 0, b"text"), ("skills", ns, 1, b"skill")):
+            agent[name] = [(b"%s_%s_%d" % (verbs[k % 6], w, k), {"did": b"did:key:z%023d%023d" % (i, k), "public_key_jwk":
+                            b'{"alg":"EdDSA","crv":"Ed25519","kty":"OKP","use":"sig","x":"%021d%022d"}' % (i, k),
+                            "derivation_path": b"m/44'/1234567'/%d'/%d'/%d'" % (i, kind, k), "function_name": b"%s_%s_%d" % (verbs[k % 6], w, k)})
+                           for k in range(cnt)]
+        req = {"reasoners": [k for k, _ in agent["reasoners"]], "skills": [k for k, _ in agent["skills"]]}
+        u = rng.random()
+        if u < 0.05:                                               # removals only
+            name = "reasoners" if req["reasoners"] else "skills"
+            req[name] = req[name][1:]
+        elif u < 0.10:                                             # partial
+            req["reasoners"] = req["reasoners"][1:] + [b"new_reasoner_%d" % i]
+            req["skills"] = req["skills"] + [b"new_skill_a", b"new_skill_a"]
+        out.append({"agent_node_id": b"agent-node-%d" % i, "agent": agent, "reasoners": req["reasoners"], "skills": req["skills"], "agent_index": i})
+    return out
+
+
+def reregister_block(ctx, dev, timed):
+    """Known agents re-registered on the device (afc_did_reregister_batch): a restart storm of 2^16 known agents with 0-32 registered
+    reasoners and 0-32 skills (about 90 % unchanged, 5 % removals only, 5 % partial), then the same with 1 % of the agents at 1024
+    registered reasoners.  Next to it: the host-buffer call from pinned memory, and the oracle (tests/didrr_oracle.py, the
+    reference's branch restated in Python on one core) over a sample of the same requests."""
+    import torch
+    import agentfield_b200 as afb
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import didrr_cases as RC
+    n = 1 << 16
+    rng = np.random.default_rng(0xAF3C)
+    master = rng.integers(0, 256, 32, dtype=np.uint8).tobytes()
+    server = b"agentfield-server-bench"
+    cache = afb.ExpandedKeys(ctx)
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a).view(dt)).to(dev)  # noqa: E731
+
+    def measure(reqs):
+        A = RC.pack(reqs)
+        D = (t(np.frombuffer(master, dtype=np.uint8).copy(), np.uint8), server, t(A[0], np.uint8), t(A[1], np.int64), t(A[2], np.int32),
+             t(A[3], np.int64), t(A[4], np.uint8), t(A[5], np.int64), t(A[6], np.int64), t(A[7], np.uint8), t(A[8], np.int64), len(reqs))
+        run = lambda: cache.reregister_dev(*D, append=False)  # noqa: E731
+        R = run()
+        torch.cuda.synchronize()
+        st = R["state"].cpu().numpy()
+        ms = timed(run)
+        ctx.profile_begin()
+        timed(run, reps=3)
+        kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+        return {"agents": len(reqs), "registered_components": int(A[6][-1]), "request_ids": int(A[3][-1]),
+                "states": {"unchanged": int((st == 0).sum()), "removed": int((st == 1).sum()), "partial": int((st == 2).sum()),
+                           "invalid": int((st == 3).sum())},
+                "body_bytes": int(R["body_off"][-1]), "ms": ms, "agents_per_s": len(reqs) / (ms * 1e-3), "kernels_ms": kms}, R, A
+    reqs = reregister_requests(n, rng)
+    main, R, A = measure(reqs)
+    # the host-buffer call from pinned memory
+    pin = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().numpy()  # noqa: E731
+    P = [pin(a) for a in A]
+    host = lambda: cache.reregister_packed(master, server, P[0], P[1], P[2], *P[3:], append=False)  # noqa: E731
+    H = host()
+    host_same = bool((H["body"] == R["body"].cpu().numpy()).all() and (H["state"] == R["state"].cpu().numpy()).all())
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        host()
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    # the oracle on a sample of the same requests (one core, Python)
+    sample = list(range(0, n, 16))
+    t_0 = time.perf_counter()
+    want = RC.oracle([reqs[i] for i in sample], master=master, server=server)
+    s_oracle = time.perf_counter() - t_0
+    body = H["body"].tobytes()
+    oracle_same = all(body[int(H["body_off"][i]):int(H["body_off"][i + 1])] == w["body"] for i, w in zip(sample, want))
+    del R, H, P
+    torch.cuda.empty_cache()
+    skewed, _, _ = measure(reregister_requests(n, rng, skew=(0.01, 1024)))
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "sign_mode": ctx.sign_mode(), "dev_call": main, "skewed_1pct_1024": skewed,
+            "host_call": {"agents": n, "ms": ms_host, "agents_per_s": n / (ms_host * 1e-3), "same_as_dev": host_same, "note": "pinned numpy buffers"},
+            "oracle": {"agents": len(sample), "s": s_oracle, "agents_per_s": len(sample) / s_oracle, "same_bodies": bool(oracle_same),
+                       "note": "tests/didrr_oracle.py: the reference's branch restated in Python, one core; not the Go service"}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register"],
+    ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register",
+                                        "reregister"],
                     default=None,
                     help="run one block")
     args = ap.parse_args()
@@ -663,7 +756,8 @@ def main():
         e1.record(); torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
-              "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block}
+              "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block,
+              "reregister": reregister_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
