@@ -160,7 +160,8 @@ class IngestStats(C.Structure):
 
 class KeycacheStats(C.Structure):
     _fields_ = [(k, C.c_uint32) for k in ("max_keys", "cached_keys", "last_hot", "last_cold", "last_distinct", "last_built", "last_evicted",
-                                          "total_built", "total_evicted", "calls")]
+                                          "total_built", "total_evicted", "calls", "base_window", "base_build_us")] + [
+        ("base_table_bytes", C.c_uint64)]
 
 
 class ProfileEntry(C.Structure):

@@ -13,11 +13,13 @@
 #if defined(AFC_HOSTSIM)
 #define AFC_HD static inline
 #define AFC_HDM inline
+#define AFC_HHD static inline
 #define AFC_DEVICE_CODE 0
 #else
 #include <cuda_runtime.h>
 #define AFC_HD __device__ __forceinline__
 #define AFC_HDM __device__ __forceinline__
+#define AFC_HHD __host__ __device__ __forceinline__     // also called by the launch code on the host (table geometry)
 #if defined(__CUDA_ARCH__)
 #define AFC_DEVICE_CODE 1
 #else

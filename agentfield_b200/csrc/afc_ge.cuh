@@ -212,6 +212,31 @@ static_assert(BASE_COLS % BASE_CHUNK == 0 && BASE_COLS >= COMB_COLS, "chunking")
 AFC_HD void sc_recode_base(uint32_t* t, const uint32_t* s) { if (BASE_W == 16) sc_recode65536(t, s); else sc_recode256(t, s); }
 AFC_HD int sc_digit_base(const uint32_t* t, int i) { return BASE_W == 16 ? sc_digit65536(t, i) : sc_digit256(t, i); }
 
+// The fixed-base table the table-driven verify reads (ed25519_keyed_point), radix 2^w for w in 16..22 (sc_recode_wide):
+//   tab[i][j] = (j+1) * 2^(w i) * B     rows i = 0..rows-1 of 2^(w-1) entries each; the top row holds only as many entries as its
+//   digit can reach (base_table_entries rounds them up to whole build chunks).
+// At w = 16 this is the radix-65536 table above, shared with signing; wider tables are verify-only, allocated per context at its
+// first table-driven verify.  Passed to the kernels by value: the recoding offset is a kernel parameter, not a register.
+struct base_table { const ge_precomp* tab; uint32_t offset[8]; int w, rows; };
+AFC_HHD base_table base_table_make(const ge_precomp* tab, int w) {
+    base_table b;
+    b.tab = tab; b.w = w; b.rows = sc_wide_rows(w);
+    sc_wide_offset(b.offset, w);
+    return b;
+}
+// largest top-row digit of any S < 2^253 (every canonical S < L): what the top row must hold
+AFC_HHD int base_table_top_max(int w) {
+    uint32_t c[8], s[8], t[8];
+    sc_wide_offset(c, w);
+    for (int i = 0; i < 8; i++) s[i] = i < 7 ? 0xffffffffu : 0x1fffffffu;
+    sc_recode_wide(t, s, c);
+    return sc_digit_wide(t, sc_wide_rows(w) - 1, w, sc_wide_rows(w));
+}
+AFC_HHD size_t base_table_entries(int w) {
+    const size_t top = ((size_t)base_table_top_max(w) + BASE_CHUNK - 1) / BASE_CHUNK * BASE_CHUNK;
+    return (size_t)(sc_wide_rows(w) - 1) * ((size_t)1 << (w - 1)) + top;
+}
+
 // out[j] = affine precomputed form of M + j P for j = 0..CH-1, with ONE field inversion (Montgomery's trick); on return
 // M has advanced to M + CH P.  c = P in cached form.  Scratch: 4 CH field elements of thread-local memory.
 template <class F, int CH>
@@ -237,14 +262,14 @@ AFC_HD void ge_affine_run(ge_precomp* out, ge_p3& M, const ge_cached& c) {
     }
 }
 
-// M = m P for 1 <= m < 2^17, left-to-right double-and-add.  c = P in cached form.
+// M = m P for 1 <= m < 2^22, left-to-right double-and-add.  c = P in cached form.
 template <class F = FeInline>
 AFC_HD void ge_small_multiple(ge_p3& M, const ge_p3& P, const ge_cached& c, uint32_t m) {
     ge_p1p1 t;
     int started = 0;
     M = P;
 #pragma unroll 1
-    for (int bit = 16; bit >= 0; bit--) {
+    for (int bit = 21; bit >= 0; bit--) {
         if (started) { ge_dbl<F>(t, M.X, M.Y, M.Z); ge_p1p1_to_p3<F>(M, t); }
         if ((m >> bit) & 1) {
             if (started) { ge_addsub<F>(t, M, c, 0); ge_p1p1_to_p3<F>(M, t); }
@@ -253,14 +278,14 @@ AFC_HD void ge_small_multiple(ge_p3& M, const ge_p3& P, const ge_cached& c, uint
     }
 }
 
-// One chunk of the base-point table per thread at init: out[0..BASE_CHUNK) = (j0+1 .. j0+BASE_CHUNK) * 2^(W i) * B.
+// One chunk of a base-point table of radix 2^w per thread: out[0..BASE_CHUNK) = (j0+1 .. j0+BASE_CHUNK) * 2^(w i) * B.
 template <class F = FeInline>
-AFC_HD void ge_build_base_chunk(ge_precomp* out, int i, int j0) {
+AFC_HD void ge_build_base_chunk(ge_precomp* out, int i, int j0, int w = BASE_W) {
     ge_p3 P, M;
     fe_const(P.X, AFC_BX_32); fe_const(P.Y, AFC_BY_32); fe_1(P.Z); F::mul(P.T, P.X, P.Y);
     ge_p1p1 t;
 #pragma unroll 1
-    for (int k = 0; k < BASE_W * i; k++) { ge_dbl<F>(t, P.X, P.Y, P.Z); ge_p1p1_to_p3<F>(P, t); }
+    for (int k = 0; k < w * i; k++) { ge_dbl<F>(t, P.X, P.Y, P.Z); ge_p1p1_to_p3<F>(P, t); }
     ge_cached c;
     ge_p3_to_cached<F>(c, P);
     ge_small_multiple<F>(M, P, c, (uint32_t)j0 + 1);
@@ -624,26 +649,35 @@ AFC_HD int ge_build_key_row(ge_precomp* row, const uint32_t* pk, int i) {
 #define AFC_PREFETCH_B(p) AFC_PF_L1(p)
 #endif
 // R' = [S]B + [k](-A) through the two tables, left in projective form (X : Y : Z): 32 mixed additions from the key's
-// radix-256 table of -A and 256/W from the base-point table, no doublings.
+// radix-256 table of -A and base.rows (12..16) from the base-point table, no doublings.  Base row j is added at key row
+// floor(32 j / rows), so the two kinds of gather stay interleaved whatever the window.
 template <class F = FeInline>
-AFC_HD void ed25519_keyed_point(fe& X, fe& Y, fe& Z, const uint32_t* sig, const uint32_t* k, const ge_precomp* atab, const ge_precomp* base) {
+AFC_HD void ed25519_keyed_point(fe& X, fe& Y, fe& Z, const uint32_t* sig, const uint32_t* k, const ge_precomp* atab, const base_table& base) {
     uint32_t kt[8], st[8];
     sc_recode256(kt, k);
-    sc_recode_base(st, sig + 8);
-    constexpr int SH = BASE_W == 16 ? 1 : 0;            // the base table advances one row every 2^SH rows of the key table
+    sc_recode_wide(st, sig + 8, base.offset);
+    const int w = base.w, rows = base.rows;
     ge_p3 h; ge_p3_0(h);
     ge_p1p1 t;
+    int j = 0, at = 0;                                   // next base row, and the key row it is added at
 #pragma unroll 1
     for (int i = 0; i < COMB_ROWS; i++) {
         int dk = sc_digit256(kt, i);
-        int ds = (i & ((1 << SH) - 1)) ? 0 : sc_digit_base(st, i >> SH);
+        int ds = 0;
+        size_t brow = 0;
+        if (i == at) {
+            ds = sc_digit_wide(st, j, w, rows);
+            brow = (size_t)j << (w - 1);
+            j++;
+            at = j < rows ? (j * COMB_ROWS) / rows : COMB_ROWS;
+        }
 #if AFC_DEVICE_CODE && AFC_KP_PREFETCH
         if (i + 1 < COMB_ROWS) {       // the next rows' entries are random 96-byte reads (HBM / L2): start them now
             int nk = sc_digit256(kt, i + 1), mk = nk < 0 ? -nk : nk;
             if (mk) { const char* p = (const char*)&atab[(i + 1) * COMB_COLS + (mk - 1)]; AFC_PREFETCH_A(p); AFC_PREFETCH_A(p + 95); }
-            if (!((i + 1) & ((1 << SH) - 1))) {
-                int ns = sc_digit_base(st, (i + 1) >> SH), ms = ns < 0 ? -ns : ns;
-                if (ms) { const char* p = (const char*)&base[(size_t)((i + 1) >> SH) * BASE_COLS + (ms - 1)]; AFC_PREFETCH_B(p); AFC_PREFETCH_B(p + 95); }
+            if (at == i + 1) {
+                int ns = sc_digit_wide(st, j, w, rows), ms = ns < 0 ? -ns : ns;
+                if (ms) { const char* p = (const char*)&base.tab[((size_t)j << (w - 1)) + (ms - 1)]; AFC_PREFETCH_B(p); AFC_PREFETCH_B(p + 95); }
             }
         }
 #endif
@@ -663,10 +697,10 @@ AFC_HD void ed25519_keyed_point(fe& X, fe& Y, fe& Z, const uint32_t* sig, const 
             int neg = ds < 0, m = neg ? -ds : ds;
             ge_precomp e;
 #if AFC_KP_ARRANGED
-            ge_load_precomp_arranged(e, &base[(size_t)(i >> SH) * BASE_COLS + (m - 1)], neg);
+            ge_load_precomp_arranged(e, &base.tab[brow + (m - 1)], neg);
             ge_madd_arranged<F>(t, h, e, neg);
 #else
-            ge_load_precomp(e, &base[(size_t)(i >> SH) * BASE_COLS + (m - 1)]);
+            ge_load_precomp(e, &base.tab[brow + (m - 1)]);
             ge_maddsub<F>(t, h, e, neg);
 #endif
             ge_p1p1_to_p3<F>(h, t);
@@ -679,7 +713,9 @@ AFC_HD void ed25519_keyed_point(fe& X, fe& Y, fe& Z, const uint32_t* sig, const 
 template <class F = FeInline>
 AFC_HD int ed25519_verify_keyed_core(int pk_ok, const uint32_t* sig, const uint32_t* k, const ge_precomp* atab, const ge_precomp* comb) {
     fe X, Y, Z;
-    ed25519_keyed_point<F>(X, Y, Z, sig, k, atab, comb);
+    fe_0(X); fe_1(Y); fe_1(Z);
+    // only a canonical S (< L < 2^253) keeps the top digit inside the base table's top row, as in the kernels
+    if (ed25519_sig_wellformed(sig)) ed25519_keyed_point<F>(X, Y, Z, sig, k, atab, base_table_make(comb, BASE_W));
     uint32_t enc[1][8];
     if (!pk_ok) { fe_0(X); fe_1(Y); fe_1(Z); }          // garbage table: keep the arithmetic well defined, result is forced to 0
     ge_encode_many<F, 1>(enc, &X, &Y, &Z);

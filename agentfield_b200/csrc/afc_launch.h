@@ -216,6 +216,10 @@ uint64_t didrr_per_reg_fixed();
 // comb: 32 x 128 ge_precomp (row 0 = the 128 small multiples of B)
 size_t ed_tables_bytes();
 cudaError_t ed_build_tables(void* comb, cudaStream_t s, LaunchLog* lg);
+// The fixed-base table of the table-driven verify: radix 2^w, w in 16..22 (w = 16: comb itself; wider: ed_build_wide_table)
+struct VerifyBase { const void* tab; int w; };
+size_t ed_wide_table_bytes(int w);
+cudaError_t ed_build_wide_table(void* tab, int w, cudaStream_t s, LaunchLog* lg);
 // Device buffers of the transparent issuer-key cache used by ed_verify_batch (see k_ed25519.cu); owned by afcrypto.cu.
 // state words (uint32 each)
 enum KcState {
@@ -265,7 +269,7 @@ struct KeyCache {
 };
 cudaError_t ed_keycache_clear(const KeyCache& kc, cudaStream_t s, LaunchLog* lg);     // empties the persistent table (slots, counters)
 // scratch_k: n * 32 bytes; kc: nullable (nullptr = always the generic Straus kernel)
-cudaError_t ed_verify_batch(const void* comb, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off,
+cudaError_t ed_verify_batch(const void* comb, const VerifyBase& vb, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off,
                             uint32_t n, uint8_t* ok, uint32_t* scratch_k, const KeyCache* kc, cudaStream_t s, LaunchLog* lg);
 size_t ed_key_table_bytes(uint32_t n_keys);
 size_t ed_key_bases_bytes(uint32_t n_keys);     // scratch for ed_build_key_tables
@@ -273,7 +277,7 @@ cudaError_t ed_build_key_tables(const uint8_t* pks, uint32_t n_keys, void* tabs,
 size_t ed_keyed_scratch_bytes(uint32_t n_keys, uint32_t n);
 size_t ed_verify_pts_bytes(uint64_t n);         // KeyCache::pts for a call of n credentials (0 unless AFC_VERIFY_QUAD is set)
 // scratch_perm: ed_keyed_scratch_bytes() bytes, 32-byte aligned: projective results, then the issuer-bucketed order (nullptr = credential order, one-thread kernel)
-cudaError_t ed_verify_keyed_batch(const void* comb, const void* tabs, const uint8_t* valid, const uint8_t* key_pks, uint32_t n_keys,
+cudaError_t ed_verify_keyed_batch(const void* comb, const VerifyBase& vb, const void* tabs, const uint8_t* valid, const uint8_t* key_pks, uint32_t n_keys,
                                   const uint32_t* key_index, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off, uint32_t n,
                                   uint8_t* ok, uint32_t* scratch_k, uint32_t* scratch_perm, cudaStream_t s, LaunchLog* lg);
 // ct16: the 48 KB constant-time table (ed_build_ct_table) or nullptr for the fast, variable-time fixed-base multiplication

@@ -112,4 +112,25 @@ AFC_HD void sc_recode65536(uint32_t* t, const uint32_t* s) {
 }
 AFC_HD int sc_digit65536(const uint32_t* t, int i) { return (int)((t[i >> 1] >> ((i & 1) * 16)) & 65535u) - 32768; }
 
+// Signed radix-2^w recoding of s < L for any w in 16..22 (the verify-only fixed-base table): rows = ceil(254 / w);
+// t = s + C with C = 2^(w-1) (1 + 2^w + ... + 2^(w (rows-2))); digit_i = field_i(t) - 2^(w-1) in [-2^(w-1), 2^(w-1)) for
+// i < rows - 1; the top digit is everything above, t >> (w (rows-1)), with no offset: s < L < 2^253 bounds it by 2^(w-1)
+// (it is 0 or 1 when w (rows-1) = 252).  At w = 16 the digits are those of sc_recode65536.
+AFC_HHD int sc_wide_rows(int w) { return (254 + w - 1) / w; }
+AFC_HHD void sc_wide_offset(uint32_t* c, int w) {
+    for (int i = 0; i < 8; i++) c[i] = 0;
+    for (int i = 0; i + 1 < sc_wide_rows(w); i++) { const int b = w * i + w - 1; c[b >> 5] |= 1u << (b & 31); }
+}
+AFC_HHD void sc_recode_wide(uint32_t* t, const uint32_t* s, const uint32_t* offset) {
+    uint64_t c = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) { c += (uint64_t)s[i] + offset[i]; t[i] = (uint32_t)c; c >>= 32; }
+}
+AFC_HHD int sc_digit_wide(const uint32_t* t, int i, int w, int rows) {
+    const int p = w * i, lo = p >> 5;
+    const uint64_t v = (uint64_t)t[lo] | (lo < 7 ? (uint64_t)t[lo + 1] << 32 : 0ull);
+    const uint32_t f = (uint32_t)(v >> (p & 31));
+    return i + 1 == rows ? (int)f : (int)(f & ((1u << w) - 1u)) - (1 << (w - 1));
+}
+
 }  // namespace afc

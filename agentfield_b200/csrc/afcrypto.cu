@@ -9,6 +9,7 @@
 #include "afc_launch.h"
 
 #include <atomic>
+#include <chrono>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -28,6 +29,11 @@ constexpr int kSlots = 4;                 // chunks in flight per call: copies k
 constexpr uint32_t kChunkItems = 1u << 17;  // items per pipeline chunk for host-buffer calls (one full wave of the table-driven verify at G = 2)
 constexpr size_t kChunkBytes = 96u << 20;   // and at most this many message bytes per chunk
 constexpr uint32_t kMinChunkItems = 1u << 16;   // the tail of a call tapers down to this (fewer, larger copies than 16 k)
+// Window of the table-driven verify's fixed-base table (16..22; env AFC_VERIFY_BASE_WINDOW overrides it per context): 16 reads the
+// radix-65536 table every context builds at init; a wider one costs 2^(w-1) x 96 B per row of device memory, built once per context.
+#ifndef AFC_VERIFY_BASE_WINDOW
+#define AFC_VERIFY_BASE_WINDOW 22
+#endif
 
 struct DevBuf {
     uint8_t* p = nullptr;
@@ -99,6 +105,13 @@ struct afc_ctx {
     bool kc_ready = false;
     uint32_t kc_max_keys = 4096;        // AFC_KEYCACHE_MAX_KEYS / afc_keycache_configure; 0 disables (4096 keys = 1.6 GB of an H100's 80 GB)
     uint32_t kc_call_cap = 0;           // per-call scratch capacity (items)
+    // the table-driven verify's fixed-base table (verify_base): radix 2^vb_want, built at the first table-driven verify
+    std::mutex vb_mu;
+    int vb_want = AFC_VERIFY_BASE_WINDOW;
+    bool vb_ready = false;
+    void* vb_tab = nullptr;             // nullptr: the radix-65536 table (comb) serves
+    int vb_w = 16;
+    uint32_t vb_build_us = 0;
     std::mutex kc_mu;
     cudaEvent_t kc_event = nullptr;     // orders successive users of the cache across streams
     // per-kernel CUDA-event profiling (afc_profile_begin / afc_profile_end)
@@ -237,13 +250,43 @@ const launch::KeyCache* kc_prepare(afc_ctx* ctx, uint32_t n) {
     }
     return &k;
 }
+// The fixed-base table of the table-driven verify.  A context's first call that needs it allocates and builds the radix-2^w table
+// (w = AFC_VERIFY_BASE_WINDOW; 16 = the radix-65536 table every context already has), synchronously and once; when the memory cannot
+// be had the radix-65536 table serves instead, with the same results.
+cudaError_t verify_base(afc_ctx* ctx, launch::VerifyBase& vb) {
+    std::lock_guard<std::mutex> g(ctx->vb_mu);
+    if (!ctx->vb_ready && ctx->vb_want != 16) {
+        const auto t0 = std::chrono::steady_clock::now();
+        void* tab = nullptr;
+        if (cudaMalloc(&tab, launch::ed_wide_table_bytes(ctx->vb_want)) != cudaSuccess) { cudaGetLastError(); tab = nullptr; }
+        if (tab) {
+            cudaStream_t s = nullptr;
+            cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+            if (e == cudaSuccess) { CallLog lc(ctx); e = launch::ed_build_wide_table(tab, ctx->vb_want, s, lc); }
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+            if (s) cudaStreamDestroy(s);
+            if (e != cudaSuccess) { cudaFree(tab); return e; }
+            ctx->vb_tab = tab; ctx->vb_w = ctx->vb_want;
+            ctx->vb_build_us = (uint32_t)std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
+        }
+    }
+    ctx->vb_ready = true;
+    vb = ctx->vb_tab ? launch::VerifyBase{ctx->vb_tab, ctx->vb_w} : launch::VerifyBase{ctx->comb, 16};
+    return cudaSuccess;
+}
+
 // verify through the cache when possible; serialises cache users across streams with an event
 cudaError_t verify_with_cache(afc_ctx* ctx, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off, uint32_t n,
                               uint8_t* ok, uint32_t* scratch_k, cudaStream_t st, launch::LaunchLog* lg) {
     std::lock_guard<std::mutex> g(ctx->kc_mu);
     const launch::KeyCache* kc = kc_prepare(ctx, n);
-    if (kc) { cudaError_t e = cudaStreamWaitEvent(st, ctx->kc_event, 0); if (e != cudaSuccess) return e; }
-    cudaError_t e = launch::ed_verify_batch(ctx->comb, pks, sigs, msgs, off, n, ok, scratch_k, kc, st, lg);
+    launch::VerifyBase vb{ctx->comb, 16};
+    if (kc) {
+        cudaError_t e = verify_base(ctx, vb);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(st, ctx->kc_event, 0);
+        if (e != cudaSuccess) return e;
+    }
+    cudaError_t e = launch::ed_verify_batch(ctx->comb, vb, pks, sigs, msgs, off, n, ok, scratch_k, kc, st, lg);
     if (kc && e == cudaSuccess) e = cudaEventRecord(ctx->kc_event, st);
     return e;
 }
@@ -348,7 +391,9 @@ cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, cons
     if (e == cudaSuccess) e = launch::offsets_from_lengths(S.msg_off, n, S.scan, st, lg);
     if (e == cudaSuccess) e = json ? launch::vcj_emit(jschema, docs, doc_off, n, S.msg_off, S.msgs, st, lg)
                                    : launch::vc_emit(schema, docs, doc_off, n, S.msg_off, S.msgs, st, lg);
-    if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, S.kidx, S.sigs, S.msgs,
+    launch::VerifyBase vb;
+    if (e == cudaSuccess) e = verify_base(ctx, vb);
+    if (e == cudaSuccess) e = launch::ed_verify_keyed_batch(ctx->comb, vb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, S.kidx, S.sigs, S.msgs,
                                                             S.msg_off, n, S.ok, S.kscr, S.kscr + (size_t)n * 8, st, lg);
     if (e == cudaSuccess) e = launch::vc_fold(status, S.ok, n, st, lg);
     return e;
@@ -673,6 +718,7 @@ int afc_init(int device, afc_ctx** out) {
     if (!ctx) return AFC_ENOMEM;
     ctx->device = device;
     if (const char* e = getenv("AFC_KEYCACHE_MAX_KEYS")) ctx->kc_max_keys = (uint32_t)strtoul(e, nullptr, 10);
+    if (const char* e = getenv("AFC_VERIFY_BASE_WINDOW")) { const int w = atoi(e); if (w >= 16 && w <= 22) ctx->vb_want = w; }
     auto fail = [&](cudaError_t e, const char* what) { set_err(ctx, e, what); fprintf(stderr, "afc_init: %s\n", ctx->last_error.c_str()); afc_destroy(ctx); return AFC_ECUDA; };
     cudaError_t e;
     if ((e = cudaSetDevice(device)) != cudaSuccess) return fail(e, "cudaSetDevice");
@@ -718,6 +764,7 @@ void afc_destroy(afc_ctx* ctx) {
     kc_free(ctx);
     if (ctx->kc_event) cudaEventDestroy(ctx->kc_event);
     if (ctx->comb) cudaFree(ctx->comb);
+    if (ctx->vb_tab) cudaFree(ctx->vb_tab);
     if (ctx->ct16) cudaFree(ctx->ct16);
     for (auto& r : ctx->prof_recs) { if (r.e0) cudaEventDestroy(r.e0); if (r.e1) cudaEventDestroy(r.e1); }
     delete ctx;
@@ -1099,6 +1146,10 @@ int afc_keycache_stats(afc_ctx* ctx, afc_keycache_stats_t* out) {
     out->last_hot = st[launch::KS_NHOT]; out->last_cold = st[launch::KS_NCOLD]; out->last_distinct = st[launch::KS_DISTINCT];
     out->last_built = st[launch::KS_NBUILD]; out->last_evicted = st[launch::KS_EVICTED];
     out->total_built = st[launch::KS_TOTAL_BUILT]; out->total_evicted = st[launch::KS_TOTAL_EVICTED]; out->calls = st[launch::KS_CALLS];
+    std::lock_guard<std::mutex> gv(ctx->vb_mu);
+    out->base_window = (uint32_t)(!ctx->vb_ready ? ctx->vb_want : ctx->vb_tab ? ctx->vb_w : 16);
+    out->base_build_us = ctx->vb_build_us;
+    out->base_table_bytes = ctx->vb_tab ? launch::ed_wide_table_bytes(ctx->vb_w) : 0;
     return AFC_OK;
 }
 
@@ -1165,7 +1216,9 @@ int afc_ed25519_verify_keyed_batch(afc_ctx* ctx, afc_keyset* ks, const uint32_t*
             d_ok = k.take((size_t)r.cnt + 16);
             d_k = (uint32_t*)k.take((size_t)r.cnt * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, r.cnt));
         }));
-        CK(launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_ki, d_sigs, M.d, M.off, r.cnt, d_ok, d_k,
+        launch::VerifyBase vb;
+        CK(verify_base(ctx, vb));
+        CK(launch::ed_verify_keyed_batch(ctx->comb, vb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_ki, d_sigs, M.d, M.off, r.cnt, d_ok, d_k,
                                          d_k + (size_t)r.cnt * 8, r.st, r.lc));
         return r.copy_back({{ok, r.i0, d_ok, r.cnt}});
     });
@@ -1178,8 +1231,10 @@ int afc_ed25519_verify_keyed_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint3
     CallLog lc(ctx);
     cudaStream_t st = (cudaStream_t)stream;
     uint32_t* d_k = nullptr;
+    launch::VerifyBase vb;
+    CK(verify_base(ctx, vb));
     if (n) CK(cudaMallocAsync((void**)&d_k, (size_t)n * 32 + launch::ed_keyed_scratch_bytes(ks->n_keys, n), st));
-    cudaError_t e = launch::ed_verify_keyed_batch(ctx->comb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_key_index, d_sigs, d_msgs,
+    cudaError_t e = launch::ed_verify_keyed_batch(ctx->comb, vb, ks->d_tabs, ks->d_valid, ks->d_pks, ks->n_keys, d_key_index, d_sigs, d_msgs,
                                                   d_msg_off, n, d_ok, d_k, n ? d_k + (size_t)n * 8 : nullptr, st, lc);
     if (n) cudaFreeAsync(d_k, st);
     CK(e);

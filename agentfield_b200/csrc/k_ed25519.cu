@@ -60,6 +60,12 @@ k_ed_build_tables(ge_precomp* base) {
     int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t < BASE_ROWS * CPR) ge_build_base_chunk<FeCall>(base + (size_t)t * BASE_CHUNK, t / CPR, (t % CPR) * BASE_CHUNK);
 }
+// the same for the verify-only table of radix 2^w (base_table_entries(w) entries; at a context's first table-driven verify)
+__global__ void __launch_bounds__(32)
+k_ed_build_wide(ge_precomp* tab, int w, uint32_t chunks) {
+    const uint32_t cpr = (1u << (w - 1)) / BASE_CHUNK, t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < chunks) ge_build_base_chunk<FeCall>(tab + (size_t)t * BASE_CHUNK, (int)(t / cpr), (int)(t % cpr) * BASE_CHUNK, w);
+}
 
 // the 512 entries of the constant-time signing table, copied out of the radix-65536 table (afc_init, once per context)
 __global__ void __launch_bounds__(256)
@@ -139,7 +145,7 @@ constexpr int KC_THREADS = AFC_CACHED_THREADS;
 // gather from ONE 12 KB table row per step instead of 32 different 384 KB tables (in credential order the gathers miss L2
 // far more often).  lookup(i, atab) -> false when credential i's key is unknown or does not decode (ok = 0).
 template <class Item, class Lookup>
-__device__ __forceinline__ void table_verify_group(Item item, Lookup lookup, const ge_precomp* __restrict__ base, const uint8_t* __restrict__ sigs,
+__device__ __forceinline__ void table_verify_group(Item item, Lookup lookup, const base_table& base, const uint8_t* __restrict__ sigs,
                                                    const uint32_t* __restrict__ ks, uint32_t n, uint32_t T, int G, uint8_t* __restrict__ ok) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
@@ -188,7 +194,7 @@ __device__ __forceinline__ void table_verify_group(Item item, Lookup lookup, con
 // tile, and an inversion per credential would be a third of the work.
 template <class F, int NT> __device__ __forceinline__ void fe_invert_cta(fe& inv, const fe& q, fe* tree);
 template <int NT, class Item, class Lookup>
-__device__ __forceinline__ void table_verify_dynamic(Item item, Lookup lookup, const ge_precomp* __restrict__ base, const uint8_t* __restrict__ sigs,
+__device__ __forceinline__ void table_verify_dynamic(Item item, Lookup lookup, const base_table& base, const uint8_t* __restrict__ sigs,
                                                      const uint32_t* __restrict__ ks, uint32_t n, uint32_t* __restrict__ counter,
                                                      uint8_t* __restrict__ ok, int share_inv) {
     __shared__ fe tree[2 * NT];
@@ -464,7 +470,7 @@ k_ks_scatter(const uint32_t* __restrict__ key_index, uint32_t n_keys, uint32_t n
 }
 
 __global__ void __launch_bounds__(ED_THREADS, AFC_CACHED_MINB)
-k_ed_verify_keyed(const ge_precomp* __restrict__ comb, const ge_precomp* __restrict__ tabs, const uint8_t* __restrict__ valid,
+k_ed_verify_keyed(const base_table base, const ge_precomp* __restrict__ tabs, const uint8_t* __restrict__ valid,
                   const uint32_t* __restrict__ key_index, uint32_t n_keys, const uint8_t* __restrict__ sigs,
                   const uint32_t* __restrict__ ks, uint32_t n, uint32_t T, int G, uint8_t* __restrict__ ok, const uint32_t* __restrict__ perm) {
     table_verify_group([&](uint32_t p) { return perm ? perm[p] : p; }, [&](uint32_t i, const ge_precomp*& atab) {
@@ -472,11 +478,11 @@ k_ed_verify_keyed(const ge_precomp* __restrict__ comb, const ge_precomp* __restr
         if (key >= n_keys || !valid[key]) return false;      // unknown index or undecodable key: ok = 0
         atab = tabs + (size_t)key * COMB_ROWS * COMB_COLS;
         return true;
-    }, comb, sigs, ks, n, T, G, ok);
+    }, base, sigs, ks, n, T, G, ok);
 }
 
 __global__ void __launch_bounds__(ED_THREADS, AFC_CACHED_MINB)
-k_ed_verify_keyed_dyn(const ge_precomp* __restrict__ comb, const ge_precomp* __restrict__ tabs, const uint8_t* __restrict__ valid,
+k_ed_verify_keyed_dyn(const base_table base, const ge_precomp* __restrict__ tabs, const uint8_t* __restrict__ valid,
                       const uint32_t* __restrict__ key_index, uint32_t n_keys, const uint8_t* __restrict__ sigs,
                       const uint32_t* __restrict__ ks, uint32_t n, uint8_t* __restrict__ ok, const uint32_t* __restrict__ perm,
                       uint32_t* __restrict__ counter, int share_inv) {
@@ -485,7 +491,7 @@ k_ed_verify_keyed_dyn(const ge_precomp* __restrict__ comb, const ge_precomp* __r
         if (key >= n_keys || !valid[key]) return false;
         atab = tabs + (size_t)key * COMB_ROWS * COMB_COLS;
         return true;
-    }, comb, sigs, ks, n, counter, ok, share_inv);
+    }, base, sigs, ks, n, counter, ok, share_inv);
 }
 
 // ---- transparent issuer-key cache behind afc_ed25519_verify_batch -----------------------------------------------
@@ -700,7 +706,7 @@ k_kc_scatter(KeyCacheDev kc, uint32_t n) {
 // (Fusing k_ed_hram into this kernel was tried and dropped: the SHA-512 state pushes the register allocation of the curve loop
 // around and nothing overlaps that did not already.)
 __global__ void __launch_bounds__(KC_THREADS, AFC_CACHED_MINB)
-k_ed_verify_cached(KeyCacheDev kc, const ge_precomp* __restrict__ comb, const uint8_t* __restrict__ sigs, const uint32_t* __restrict__ ks,
+k_ed_verify_cached(KeyCacheDev kc, const base_table base, const uint8_t* __restrict__ sigs, const uint32_t* __restrict__ ks,
                    int G, uint8_t* __restrict__ ok) {
     const uint32_t n_hot = kc.state[KS_NHOT];
     if (!n_hot) return;
@@ -710,7 +716,7 @@ k_ed_verify_cached(KeyCacheDev kc, const ge_precomp* __restrict__ comb, const ui
         if (!kc.valid[id]) return false;                     // key does not decode: ok = 0
         atab = (const ge_precomp*)kc.tabs + (size_t)id * COMB_ROWS * COMB_COLS;
         return true;
-    }, comb, sigs, ks, n_hot, T, G, ok);
+    }, base, sigs, ks, n_hot, T, G, ok);
 }
 
 // ---- table-driven verification on FOUR lanes per credential (experiment, AFC_VERIFY_QUAD=1|2) --------------------------------
@@ -932,7 +938,7 @@ k_ed_quad_finish(Src src, const fe* __restrict__ pts, const uint8_t* __restrict_
 }
 
 __global__ void __launch_bounds__(KC_THREADS, AFC_CACHED_MINB)
-k_ed_verify_cached_dyn(KeyCacheDev kc, const ge_precomp* __restrict__ comb, const uint8_t* __restrict__ sigs, const uint32_t* __restrict__ ks,
+k_ed_verify_cached_dyn(KeyCacheDev kc, const base_table base, const uint8_t* __restrict__ sigs, const uint32_t* __restrict__ ks,
                        uint8_t* __restrict__ ok, int share_inv) {
     const uint32_t n_hot = kc.state[KS_NHOT];
     if (!n_hot) return;
@@ -941,7 +947,7 @@ k_ed_verify_cached_dyn(KeyCacheDev kc, const ge_precomp* __restrict__ comb, cons
         if (!kc.valid[id]) return false;
         atab = (const ge_precomp*)kc.tabs + (size_t)id * COMB_ROWS * COMB_COLS;
         return true;
-    }, comb, sigs, ks, n_hot, kc.state + KS_QTILE, ok, share_inv);
+    }, base, sigs, ks, n_hot, kc.state + KS_QTILE, ok, share_inv);
 }
 
 // mode 0: seeds (32 B each) -> expand then sign;  mode 1: expanded keys (96 B each) selected by key_index.
@@ -1254,6 +1260,13 @@ cudaError_t ed_build_tables(void* comb, cudaStream_t s, LaunchLog* lg) {
     AFC_LAUNCH(lg, "k_ed_build_tables", s, k_ed_build_tables<<<blocks_for((uint64_t)BASE_ROWS * BASE_COLS / BASE_CHUNK, 32), 32, 0, s>>>((ge_precomp*)comb));
     return cudaGetLastError();
 }
+size_t ed_wide_table_bytes(int w) { return sizeof(ge_precomp) * base_table_entries(w); }
+cudaError_t ed_build_wide_table(void* tab, int w, cudaStream_t s, LaunchLog* lg) {
+    const uint32_t chunks = (uint32_t)(base_table_entries(w) / BASE_CHUNK);
+    AFC_LAUNCH(lg, "k_ed_build_wide", s, k_ed_build_wide<<<blocks_for(chunks, 32), 32, 0, s>>>((ge_precomp*)tab, w, chunks));
+    return cudaGetLastError();
+}
+static base_table verify_table(const VerifyBase& vb) { return base_table_make((const ge_precomp*)vb.tab, vb.w); }
 // AFC_VERIFY_QUAD: 0 = one thread per credential (k_ed_verify_cached_dyn / _keyed_dyn; default), 1 = four lanes per credential after
 // k_ed_hram, 2 = four lanes per credential with the hashing fused.  The four-lane form spends 8 multiplication slots on the 7
 // products of a mixed addition and more of the same pipe on register moves (DESIGN.md §4).  Kept as an experiment; same results.
@@ -1333,7 +1346,7 @@ static void launch_key_build(const KeyBuild& b, uint32_t max_build, cudaStream_t
         AFC_LAUNCH(lg, "k_kc_rows", rows, k_kc_rows<<<blocks_for((uint64_t)max_build * nr * KR_PARTS, KR_NT), KR_NT, 0, rows>>>(b, st * nr, nr));
     }
 }
-cudaError_t ed_verify_batch(const void* comb, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off,
+cudaError_t ed_verify_batch(const void* comb, const VerifyBase& vb, const uint8_t* pks, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off,
                             uint32_t n, uint8_t* ok, uint32_t* scratch_k, const KeyCache* kcp, cudaStream_t s, LaunchLog* lg) {
     if (n == 0) return cudaSuccess;
     const ge_precomp* cb = (const ge_precomp*)comb;
@@ -1389,11 +1402,11 @@ cudaError_t ed_verify_batch(const void* comb, const uint8_t* pks, const uint8_t*
         AFC_LAUNCH(lg, "k_ed_quad_finish", s, k_ed_quad_finish<QuadCached><<<blocks_for(((uint64_t)n + QF_G - 1) / QF_G, QF_THREADS), QF_THREADS, 0, s>>>(src, (const fe*)kc.pts, sigs, ok));
     } else {
         if (dynamic_mode()) {
-            AFC_LAUNCH(lg, "k_ed_verify_cached_dyn", s, k_ed_verify_cached_dyn<<<dynamic_grid(n, (const void*)k_ed_verify_cached_dyn, KC_THREADS), KC_THREADS, 0, s>>>(kc, cb, sigs, scratch_k, ok, dynamic_share_inv(n)));
+            AFC_LAUNCH(lg, "k_ed_verify_cached_dyn", s, k_ed_verify_cached_dyn<<<dynamic_grid(n, (const void*)k_ed_verify_cached_dyn, KC_THREADS), KC_THREADS, 0, s>>>(kc, verify_table(vb), sigs, scratch_k, ok, dynamic_share_inv(n)));
         } else {
             const int G = pick_group(n, (const void*)k_ed_verify_cached);
             const uint32_t Tmax = (uint32_t)(((uint64_t)n + G - 1) / G);
-            AFC_LAUNCH(lg, "k_ed_verify_cached", s, k_ed_verify_cached<<<blocks_for(Tmax, KC_THREADS), KC_THREADS, 0, s>>>(kc, cb, sigs, scratch_k, G, ok));
+            AFC_LAUNCH(lg, "k_ed_verify_cached", s, k_ed_verify_cached<<<blocks_for(Tmax, KC_THREADS), KC_THREADS, 0, s>>>(kc, verify_table(vb), sigs, scratch_k, G, ok));
         }
     }
     launch_generic_verify(cb, pks, sigs, scratch_k, n, ok, kc.cold, kc.state + KS_NCOLD, s, lg);
@@ -1413,7 +1426,7 @@ size_t ed_verify_pts_bytes(uint64_t n) { return quad_mode() ? (size_t)n * 96 : 0
 size_t ed_keyed_scratch_bytes(uint32_t n_keys, uint32_t n) { return ed_verify_pts_bytes(n) + (4 + keyed_bucket_words(n_keys) + (size_t)n) * 4; }
 // scratch_perm: ed_keyed_scratch_bytes(n_keys, n) bytes, 32-byte aligned ([pts[3 n] field elements,] 4 counter words, bucket[n_keys + 1], perm[n]), or
 // nullptr = credential order and the one-thread kernel
-cudaError_t ed_verify_keyed_batch(const void* comb, const void* tabs, const uint8_t* valid, const uint8_t* key_pks, uint32_t n_keys,
+cudaError_t ed_verify_keyed_batch(const void* comb, const VerifyBase& vb, const void* tabs, const uint8_t* valid, const uint8_t* key_pks, uint32_t n_keys,
                                   const uint32_t* key_index, const uint8_t* sigs, const uint8_t* msgs, const uint64_t* off, uint32_t n,
                                   uint8_t* ok, uint32_t* scratch_k, uint32_t* scratch_perm, cudaStream_t s, LaunchLog* lg) {
     if (n == 0) return cudaSuccess;
@@ -1445,12 +1458,12 @@ cudaError_t ed_verify_keyed_batch(const void* comb, const void* tabs, const uint
     if (scratch_perm && dynamic_mode()) {
         uint32_t* tile_ctr = scratch_perm + ed_verify_pts_bytes(n) / 4;
         AFC_LAUNCH(lg, "k_fill_u32", s, k_fill_u32<<<1, 256, 0, s>>>(tile_ctr, 0u, 4));
-        AFC_LAUNCH(lg, "k_ed_verify_keyed_dyn", s, k_ed_verify_keyed_dyn<<<dynamic_grid(n, (const void*)k_ed_verify_keyed_dyn, ED_THREADS), ED_THREADS, 0, s>>>((const ge_precomp*)comb, (const ge_precomp*)tabs, valid, key_index, n_keys, sigs, scratch_k, n, ok, perm, tile_ctr, dynamic_share_inv(n)));
+        AFC_LAUNCH(lg, "k_ed_verify_keyed_dyn", s, k_ed_verify_keyed_dyn<<<dynamic_grid(n, (const void*)k_ed_verify_keyed_dyn, ED_THREADS), ED_THREADS, 0, s>>>(verify_table(vb), (const ge_precomp*)tabs, valid, key_index, n_keys, sigs, scratch_k, n, ok, perm, tile_ctr, dynamic_share_inv(n)));
         return cudaGetLastError();
     }
     const int G = pick_group(n, (const void*)k_ed_verify_keyed);
     const uint32_t T = (uint32_t)(((uint64_t)n + G - 1) / G);
-    AFC_LAUNCH(lg, "k_ed_verify_keyed", s, k_ed_verify_keyed<<<blocks_for(T, ED_THREADS), ED_THREADS, 0, s>>>((const ge_precomp*)comb, (const ge_precomp*)tabs, valid, key_index, n_keys, sigs, scratch_k, n, T, G, ok, perm));
+    AFC_LAUNCH(lg, "k_ed_verify_keyed", s, k_ed_verify_keyed<<<blocks_for(T, ED_THREADS), ED_THREADS, 0, s>>>(verify_table(vb), (const ge_precomp*)tabs, valid, key_index, n_keys, sigs, scratch_k, n, T, G, ok, perm));
     return cudaGetLastError();
 }
 // ct16 != nullptr selects the constant-time kernels (48 KB of dynamic shared memory for the table)

@@ -110,12 +110,17 @@ int afc_ed25519_verify_batch_dev(afc_ctx* ctx, const uint8_t* d_pks, const uint8
  * issuer.  Decisions are taken on the device, nothing synchronises, results are bit-identical whichever way a credential goes.
  * max_keys = 0 disables (always the generic kernel); default 4096 (1.6 GB), or env AFC_KEYCACHE_MAX_KEYS.
  * afc_keycache_info: cached_keys = tables currently held, last_mode = 1 if the last verify call sent any credential through
- * tables.  afc_keycache_stats: the split of the last call and the running totals. */
+ * tables.  afc_keycache_stats: the split of the last call and the running totals, and the fixed-base table the table-driven
+ * verify reads: base_window = its radix 2^w (16 = the radix-65536 table shared with signing, also what serves when a wider table
+ * cannot be allocated), base_table_bytes / base_build_us = the context's verify-only wider table (0 until its first
+ * table-driven verify builds it). */
 typedef struct afc_keycache_stats_t {
     uint32_t max_keys, cached_keys;
     uint32_t last_hot, last_cold;          /* credentials of the last call verified through tables / by the generic kernel */
     uint32_t last_distinct, last_built, last_evicted;
     uint32_t total_built, total_evicted, calls;
+    uint32_t base_window, base_build_us;
+    uint64_t base_table_bytes;
 } afc_keycache_stats_t;
 int afc_keycache_configure(afc_ctx* ctx, uint32_t max_keys);
 int afc_keycache_info(afc_ctx* ctx, uint32_t* max_keys, uint32_t* cached_keys, uint32_t* last_mode);
