@@ -25,6 +25,11 @@ ISSUE_HASH_DATA = 1
 WORKFLOW_COLUMNS = ("workflow_id", "session_id", "issuer_did", "vc_id", "issuance_date", "snapshot_time", "proof_created")
 WORKFLOW_RECORD_COLUMNS = ("vc_id", "status")
 WORKFLOW_BUILT, WORKFLOW_HOST = 0, 1
+CHAIN_WORKFLOW_COLUMNS = ("workflow_vc_id", "resolved_at")
+CHAIN_RECORD_COLUMNS = ("execution_id", "workflow_id", "session_id", "agent_node_id", "workflow_name", "issuer_did", "target_did", "caller_did",
+                        "vc_document", "signature", "storage_uri", "input_hash", "output_hash")
+CHAIN_AGENT_NODE_ID_NIL, CHAIN_WORKFLOW_NAME_NIL, CHAIN_VC_DOCUMENT_NIL = 1, 2, 4
+CHAIN_BUILT, CHAIN_HOST = 0, 1
 WEBHOOK_COLUMNS = ("execution_id", "run_id", "status", "node_id", "reasoner_id", "target_type", "timestamp", "error_message")
 WEBHOOK_HAS_DURATION, WEBHOOK_HAS_ERROR_MESSAGE, WEBHOOK_HAS_SECRET = 1, 2, 4
 WEBHOOK_BUILT, WEBHOOK_HOST = 0, 1
@@ -100,6 +105,11 @@ SYMBOLS = {
     "afc_vc_workflow_bound": (C.c_uint64, [vp, vp, vp, C.c_uint32]),
     "afc_vc_issue_workflow_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),
     "afc_vc_issue_workflow_batch_dev": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, vp]),
+    "afc_did_directory_new": (C.c_int, [vp, vp, vp, vp, C.c_uint32, C.POINTER(vp)]),
+    "afc_did_directory_free": (None, [vp]),
+    "afc_vc_workflow_chain_bound": (C.c_uint64, [vp, vp, vp, vp, vp, C.c_uint32]),
+    "afc_vc_workflow_chain_batch": (C.c_int, [vp, vp, C.c_uint32] + [vp] * 16 + [C.c_uint32, vp, C.c_uint64, vp, vp]),
+    "afc_vc_workflow_chain_batch_dev": (C.c_int, [vp, vp, C.c_uint32] + [vp] * 16 + [C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_bound": (C.c_uint64, [vp, vp, C.c_uint32]),
     "afc_webhook_sign_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_sign_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),

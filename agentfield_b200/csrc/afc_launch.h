@@ -157,6 +157,38 @@ cudaError_t vcw_proof(const uint8_t* sigs, const uint8_t* state, uint32_t n, con
                       cudaStream_t s, LaunchLog* lg);
 uint64_t vcw_literal_bytes();          // constant text of both document forms together
 
+// ---- k_vcchain.cu: workflow VC chains served on the device (afc_vcchain.cuh).  The issue call's inputs as for vcw_*; chain_col_off: 2
+// absolute offsets per workflow + 1; clock: 3 per workflow; chain_rec_col_off (13 per record + 1), rec_flags, doc_size and created_off are
+// indexed by absolute record.  The batch's m records and O = 3 m + n DID occurrence slots have per-item scratch.
+struct VccArgs {
+    const uint8_t* cols; const uint64_t* col_off; const uint64_t* rec_off; const uint8_t* rec_cols; const uint64_t* rec_col_off;
+    const int64_t* created_at;
+    const uint8_t* chain_cols; const uint64_t* chain_col_off; const int64_t* clock;
+    const uint8_t* chain_rec_cols; const uint64_t* chain_rec_col_off; const uint8_t* rec_flags; const int64_t* doc_size; const int32_t* created_off;
+    // the directory: DID bytes and uint32 offsets, its slot table, each DID's rank in byte order and the DID of each rank, its keys (16-byte aligned)
+    const uint8_t* dir_dids; const uint32_t* dir_off; const uint32_t* dir_slots; uint32_t dir_mask; const uint32_t* dir_rank; const uint32_t* dir_order;
+    const uint8_t* dir_pks;
+    uint32_t n, m;
+    // what the workflow-credential passes left: documents and offsets, proof values, states, summaries, scanned id lengths, array places
+    const uint8_t* docs; const uint64_t* doc_off; const uint8_t* pv; const uint8_t* wstate; const uint32_t* summary; const uint64_t* id_off;
+    const uint64_t* arr;
+    // outputs
+    uint8_t* bodies; uint64_t* body_off; uint8_t* state;
+    // scratch: rlen m + 1; rank, dlist O; elen O + 1; hset 2 O; host, ndist n; lay vcc_lay_words() per workflow; scan
+    // json_scan_scratch_bytes(max(n, m, O))
+    uint64_t* rlen; uint32_t* rank; uint32_t* dlist; uint64_t* elen; uint32_t* hset; uint32_t* host; uint32_t* ndist; uint64_t* lay; uint64_t* scan;
+};
+size_t vcc_lay_words();
+// out: the six ends of vcw_ends, chain_col_off[0], chain_col_off[2 n], chain_rec_col_off at 13 rec_off[0] and 13 rec_off[n] (one thread)
+cudaError_t vcc_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
+                     const uint64_t* chain_rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
+// after the workflow-credential passes: states, body offsets (complete when this has run) and the layout; then the bodies
+cudaError_t vcc_sizes(const VccArgs& A, cudaStream_t s, LaunchLog* lg);
+cudaError_t vcc_emit(const VccArgs& A, cudaStream_t s, LaunchLog* lg);
+uint64_t vcc_frame_fixed();            // the body bound's constant per workflow, per record and per DID occurrence (afc_vcchain.cuh)
+uint64_t vcc_record_fixed();
+uint64_t vcc_entry_fixed();
+
 // ---- k_didreg.cu: agent DIDs registered on the device (afc_didreg.cuh).  node_off: n + 1 absolute offsets; id_idx: 2n + 1 absolute id
 // indices (request i's reasoners [id_idx[2i], id_idx[2i+1]), skills [id_idx[2i+1], id_idx[2i+2])); id_off: absolute, indexed by absolute id.
 // The m = id_idx[2n] - id_idx[0] ids have per-id scratch; the component outputs hold n + m entries (the components, then zeros).

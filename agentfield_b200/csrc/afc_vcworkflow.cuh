@@ -10,7 +10,8 @@
 //                      form): the constant text of types.WorkflowVCDocument interleaved with the workflow's columns, Go-escaped, all but
 //                      the ids inside the componentVcIds array: each record writes its own id there (vcw_put_id), in both forms, since the
 //                      prefix through "proof": is common to them.
-//   vcw_put_time       time.Time.UTC().Format(time.RFC3339) of Unix seconds: integer civil-from-days arithmetic, 20 characters.
+//   vcw_put_time       time.Time.UTC().Format(time.RFC3339) of Unix seconds: integer civil-from-days arithmetic, 20 characters (vcw_put_civil
+//                      writes the first 19, which the chain call's RFC3339Nano writer shares).
 //
 // Deliberate deviation: a workflow with no records starts at time.Now() in the reference (:563), read a second time for snapshotTime.  Here
 // its startTime is the snapshot_time column's text, as the host mirror (services.generate_workflow_vc_batch) writes it.
@@ -171,8 +172,9 @@ struct VcwItem {
 // Two decimal digits, and time.Time.UTC().Format(time.RFC3339) of Unix seconds in [VCW_SEC_MIN, VCW_SEC_MAX]
 template <class Sink>
 AFC_HD void vcw_put2(Sink& out, uint32_t v) { out.put('0' + v / 10); out.put('0' + v % 10); }
+// The civil date and time of Unix seconds without a zone designator: 2006-01-02T15:04:05 (19 characters)
 template <class Sink>
-AFC_HD void vcw_put_time(Sink& out, int64_t sec) {
+AFC_HD void vcw_put_civil(Sink& out, int64_t sec) {
     const int64_t days = (sec >= 0 ? sec : sec - 86399) / 86400;  // floor division
     const uint32_t sod = (uint32_t)(sec - days * 86400);
     // civil from days (proleptic Gregorian, eras of 400 years = 146097 days from 0000-03-01)
@@ -185,7 +187,12 @@ AFC_HD void vcw_put_time(Sink& out, int64_t sec) {
     const uint32_t d = doy - (153 * mp + 2) / 5 + 1, m = mp < 10 ? mp + 3 : mp - 9;
     const uint32_t y = (uint32_t)(yoe + era * 400 + (m <= 2));
     vcw_put2(out, y / 100); vcw_put2(out, y % 100); out.put('-'); vcw_put2(out, m); out.put('-'); vcw_put2(out, d);
-    out.put('T'); vcw_put2(out, sod / 3600); out.put(':'); vcw_put2(out, sod / 60 % 60); out.put(':'); vcw_put2(out, sod % 60); out.put('Z');
+    out.put('T'); vcw_put2(out, sod / 3600); out.put(':'); vcw_put2(out, sod / 60 % 60); out.put(':'); vcw_put2(out, sod % 60);
+}
+template <class Sink>
+AFC_HD void vcw_put_time(Sink& out, int64_t sec) {
+    vcw_put_civil(out, sec);
+    out.put('Z');
 }
 
 template <class Sink>

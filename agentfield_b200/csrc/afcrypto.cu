@@ -8,6 +8,7 @@
 #include "afc_internal.h"
 #include "afc_launch.h"
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -142,6 +143,20 @@ struct afc_keyset {
     uint32_t slot_mask = 0;
     uint8_t* d_schemas = nullptr;  // 2 x launch::vc_schema_bytes(): execution VC, workflow VC
     uint8_t* d_vcj_schemas = nullptr;  // 2 x launch::vcj_schema_bytes(): the same for documents in any spelling (afc_vcjson.cuh)
+};
+
+// The public half of a DID registry (afc_did_directory_new): DIDs, their slot table (as in a named key set), each DID's rank in byte order
+// and the DID of each rank, and the public keys
+struct afc_did_directory {
+    afc_ctx* ctx = nullptr;
+    uint32_t n = 0;
+    uint8_t* d_dids = nullptr;     // DID bytes back to back
+    uint32_t* d_did_off = nullptr; // n + 1
+    uint32_t* d_slots = nullptr;   // slot_mask + 1 entries, 0xffffffff = empty
+    uint32_t slot_mask = 0;
+    uint32_t* d_rank = nullptr;    // n: DID -> rank
+    uint32_t* d_order = nullptr;   // n: rank -> DID
+    uint8_t* d_pks = nullptr;      // n x 32
 };
 
 struct afc_merkle_tree {
@@ -1247,16 +1262,17 @@ static uint32_t did_hash(const uint8_t* p, uint64_t n) {
     for (uint64_t j = 0; j < n; j++) h = (h ^ p[j]) * 16777619u;          // = vc_did_hash_byte (afc_vcdoc.cuh)
     return h;
 }
-int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, const uint64_t* did_off, uint32_t n_keys, afc_keyset** out) {
-    if (!ctx || !out || !pks || !dids || !did_off || n_keys == 0) return AFC_EINVAL;
-    *out = nullptr;
-    const uint64_t base = did_off[0], total = did_off[n_keys] - base;
-    for (uint32_t k = 0; k < n_keys; k++) if (did_off[k + 1] < did_off[k]) return AFC_EINVAL;
-    if (total >= 0xffffffffull) return AFC_EINVAL;
-    uint32_t cap = 2; while (cap < 2ull * n_keys) cap <<= 1;
-    std::vector<uint32_t> slots(cap, 0xffffffffu), off(n_keys + 1);
-    for (uint32_t k = 0; k <= n_keys; k++) off[k] = (uint32_t)(did_off[k] - base);
-    for (uint32_t k = 0; k < n_keys; k++) {
+// The DID -> index table of named key sets and DID directories: FNV-1a, linear probing, 2^k >= 2n slots (0xffffffff = empty), and the
+// DIDs' offsets relative to did_off[0] (uint32).  AFC_EINVAL for offsets that run backwards, 4 GB of DIDs or more, or a DID named twice.
+static int did_slot_table(const uint8_t* dids, const uint64_t* did_off, uint32_t n, std::vector<uint32_t>& slots, std::vector<uint32_t>& off) {
+    const uint64_t base = did_off[0];
+    for (uint32_t k = 0; k < n; k++) if (did_off[k + 1] < did_off[k]) return AFC_EINVAL;
+    if (did_off[n] - base >= 0xffffffffull) return AFC_EINVAL;
+    uint32_t cap = 2; while (cap < 2ull * n) cap <<= 1;
+    slots.assign(cap, 0xffffffffu);
+    off.resize((size_t)n + 1);
+    for (uint32_t k = 0; k <= n; k++) off[k] = (uint32_t)(did_off[k] - base);
+    for (uint32_t k = 0; k < n; k++) {
         const uint8_t* d = dids + did_off[k];
         const uint64_t len = did_off[k + 1] - did_off[k];
         uint32_t s = did_hash(d, len) & (cap - 1);
@@ -1266,6 +1282,15 @@ int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, 
         }
         slots[s] = k;
     }
+    return AFC_OK;
+}
+int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, const uint64_t* did_off, uint32_t n_keys, afc_keyset** out) {
+    if (!ctx || !out || !pks || !dids || !did_off || n_keys == 0) return AFC_EINVAL;
+    *out = nullptr;
+    const uint64_t base = did_off[0], total = did_off[n_keys] - base;
+    std::vector<uint32_t> slots, off;
+    RC(did_slot_table(dids, did_off, n_keys, slots, off));
+    const uint32_t cap = (uint32_t)slots.size();
     int rc = afc_keyset_new(ctx, pks, n_keys, out);
     if (rc != AFC_OK) return rc;
     afc_keyset* ks = *out;
@@ -1743,6 +1768,249 @@ int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
                          r.lc));
             RC(r.copy_back({offsets_out(doc_off, i0, d_doff, (size_t)cnt + 1, base), {proof_values, (size_t)i0 * 86, d_pv, (size_t)cnt * 86},
                             {state, i0, d_st, cnt}, {summary, (size_t)i0 * 16, d_sum, (size_t)cnt * 16}, {docs, base, d_docs, bytes}}));
+            base += bytes;
+            return AFC_OK;
+        });
+    });
+}
+
+// ---------------------------------------------------------------------------------- workflow VC chains
+int afc_did_directory_new(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, const uint64_t* did_off, uint32_t n, afc_did_directory** out) {
+    if (!ctx || !out || !pks || !dids || !did_off) return AFC_EINVAL;
+    *out = nullptr;
+    std::vector<uint32_t> slots, off;
+    RC(did_slot_table(dids, did_off, n, slots, off));
+    const uint8_t* d0 = dids + did_off[0];
+    std::vector<uint32_t> order(n), rank(n);
+    for (uint32_t k = 0; k < n; k++) order[k] = k;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {      // strings.Compare: bytes, then length
+        const uint32_t la = off[a + 1] - off[a], lb = off[b + 1] - off[b];
+        const int c = memcmp(d0 + off[a], d0 + off[b], la < lb ? la : lb);
+        return c != 0 ? c < 0 : la < lb;
+    });
+    for (uint32_t k = 0; k < n; k++) rank[order[k]] = k;
+    CK(cudaSetDevice(ctx->device));
+    afc_did_directory* dir = new (std::nothrow) afc_did_directory();
+    if (!dir) return AFC_ENOMEM;
+    dir->ctx = ctx; dir->n = n; dir->slot_mask = (uint32_t)slots.size() - 1;
+    const size_t total = off[n], words = (size_t)n + 1;
+    cudaError_t e = cudaMalloc((void**)&dir->d_dids, total + 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_did_off, words * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_slots, slots.size() * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_rank, words * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_order, words * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_pks, (size_t)n * 32 + 16);
+    if (e == cudaSuccess && total) e = cudaMemcpy(dir->d_dids, d0, total, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dir->d_did_off, off.data(), words * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dir->d_slots, slots.data(), slots.size() * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n) e = cudaMemcpy(dir->d_rank, rank.data(), (size_t)n * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n) e = cudaMemcpy(dir->d_order, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n) e = cudaMemcpy(dir->d_pks, pks, (size_t)n * 32, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        set_err(ctx, e, "afc_did_directory_new");
+        afc_did_directory_free(dir);
+        return e == cudaErrorMemoryAllocation ? AFC_ENOMEM : AFC_ECUDA;
+    }
+    *out = dir;
+    return AFC_OK;
+}
+void afc_did_directory_free(afc_did_directory* dir) {
+    if (!dir) return;
+    cudaSetDevice(dir->ctx->device);
+    void* bufs[] = {dir->d_dids, dir->d_did_off, dir->d_slots, dir->d_rank, dir->d_order, dir->d_pks};
+    for (void* p : bufs) if (p) cudaFree(p);
+    delete dir;
+}
+
+// Bound from the ends of the five offset arrays: the workflow credential (wf_doc_bound), the frame's constant text, at most 6 bytes per
+// escaped byte — a workflow column appears at most twice in the frame (workflow_id), an issue record column twice (vc_id in both component
+// lists), a chain record column once (a compacted document grows at most 6 times too) — and per record and per DID occurrence their
+// constant text (a bundle member's DID, at most VCC_DID_MAX bytes, twice, and resolved_at, at most VCC_RESOLVED_MAX bytes).
+static uint64_t vcc_bound(uint32_t n, uint64_t col_bytes, uint64_t m, uint64_t rec_bytes, uint64_t chain_col_bytes, uint64_t chain_rec_bytes) {
+    return wf_doc_bound(n, col_bytes, m, rec_bytes) + (uint64_t)n * launch::vcc_frame_fixed() + 12 * col_bytes + 6 * chain_col_bytes +
+           m * (launch::vcc_record_fixed() + 4) + 12 * rec_bytes + 6 * chain_rec_bytes + (3 * m + n) * launch::vcc_entry_fixed();
+}
+static uint64_t span(uint64_t a, uint64_t b) { return b >= a ? b - a : 0; }
+// The DID occurrence slots (3 per record, 1 per workflow) are counted and scanned in 32 bits, and each workflow's hash set has twice its
+// slots: a batch holds at most 2^31 - 1 slots, so neither count can wrap
+static bool vcc_slots_fit(uint64_t m, uint32_t n) { return m <= 0x7fffffffull && 3 * m + n <= 0x7fffffffull; }
+uint64_t afc_vc_workflow_chain_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
+                                     const uint64_t* chain_rec_col_off, uint32_t n) {
+    if (!col_off || !rec_off || !rec_col_off || !chain_col_off || !chain_rec_col_off || n == 0) return 0;
+    const uint64_t cb = span(col_off[0], col_off[(size_t)n * AFC_WORKFLOW_COLUMNS]), ccb = span(chain_col_off[0], chain_col_off[(size_t)n * AFC_CHAIN_WORKFLOW_COLUMNS]);
+    const uint64_t r0 = rec_off[0], r1 = rec_off[n];
+    if (r1 < r0) return vcc_bound(n, cb, 0, 0, ccb, 0);
+    return vcc_bound(n, cb, r1 - r0, span(rec_col_off[2 * r0], rec_col_off[2 * r1]), ccb,
+                     span(chain_rec_col_off[AFC_CHAIN_RECORD_COLUMNS * r0], chain_rec_col_off[AFC_CHAIN_RECORD_COLUMNS * r1]));
+}
+
+// per-call device scratch: the workflow-credential call's outputs and scratch, then the chain's (launch::VccArgs)
+struct ChainScratch {
+    WorkflowScratch W;
+    uint8_t* docs; uint64_t* doc_off; uint8_t* pv; uint8_t* wstate; uint32_t* summary;
+};
+static void vcc_scratch(Carve& k, ChainScratch& s, launch::VccArgs& A, uint32_t n, uint32_t m, uint64_t doc_bound) {
+    const uint64_t O = 3 * (uint64_t)m + n, most = O > n ? O : n;
+    s.docs = k.take(doc_bound + 64);
+    s.doc_off = k.take<uint64_t>((size_t)n + 1);
+    s.pv = k.take((size_t)n * 86);
+    s.wstate = k.take(n);
+    s.summary = k.take<uint32_t>((size_t)n * 4);
+    wf_scratch(k, s.W, n, m, doc_bound);
+    A.rlen = k.take<uint64_t>((size_t)m + 1);
+    A.rank = k.take<uint32_t>(O);
+    A.dlist = k.take<uint32_t>(O);
+    A.elen = k.take<uint64_t>(O + 1);
+    A.hset = k.take<uint32_t>(2 * O);
+    A.host = k.take<uint32_t>(n);
+    A.ndist = k.take<uint32_t>(n);
+    A.lay = k.take<uint64_t>((size_t)n * launch::vcc_lay_words());
+    A.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes((uint32_t)most));
+}
+static void vcc_bind(launch::VccArgs& A, const ChainScratch& s, const afc_did_directory* dir, uint32_t n, uint32_t m) {
+    A.dir_dids = dir->d_dids; A.dir_off = dir->d_did_off; A.dir_slots = dir->d_slots; A.dir_mask = dir->slot_mask; A.dir_rank = dir->d_rank;
+    A.dir_order = dir->d_order; A.dir_pks = dir->d_pks;
+    A.n = n; A.m = m;
+    A.docs = s.docs; A.doc_off = s.doc_off; A.pv = s.pv; A.wstate = s.wstate; A.summary = s.summary; A.id_off = s.W.id_off; A.arr = s.W.arr;
+}
+static int vcc_check(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
+                     const uint64_t* rec_off, const uint64_t* rec_col_off, const uint8_t* chain_cols, const uint64_t* chain_col_off, const int64_t* clock,
+                     const uint64_t* chain_rec_col_off, const afc_did_directory* dir, uint32_t n, const uint8_t* bodies, const uint64_t* body_off,
+                     const uint8_t* state) {
+    if (!ctx || !dir || dir->ctx != ctx || !col_off || !rec_off || !rec_col_off || !chain_col_off || !chain_rec_col_off || !body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!expanded96 || n_keys == 0 || !key_index || !cols || !chain_cols || !clock || !bodies || !state) return AFC_EINVAL;
+    return AFC_OK;
+}
+
+int afc_vc_workflow_chain_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                    const uint64_t* d_col_off, const uint64_t* d_rec_off, const uint8_t* d_rec_cols, const uint64_t* d_rec_col_off,
+                                    const int64_t* d_created_at, const uint8_t* d_chain_cols, const uint64_t* d_chain_col_off, const int64_t* d_clock,
+                                    const uint8_t* d_chain_rec_cols, const uint64_t* d_chain_rec_col_off, const uint8_t* d_rec_flags,
+                                    const int64_t* d_doc_size, const int32_t* d_created_off, const afc_did_directory* dir, uint32_t n,
+                                    uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream) {
+    int rc = vcc_check(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_col_off, d_chain_cols, d_chain_col_off, d_clock,
+                       d_chain_rec_col_off, dir, n, d_bodies, d_body_off, d_state);
+    if (rc != AFC_OK || n == 0) return rc;
+    if (!aligned16(d_expanded96)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies: gathered by one thread, read once
+    {
+        uint64_t* d_ends = nullptr;
+        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
+        cudaError_t e = launch::vcc_ends(d_col_off, d_rec_off, d_rec_col_off, d_chain_col_off, d_chain_rec_col_off, n, d_ends, st, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(d_ends, st);
+        CK(e);
+        CK(cudaStreamSynchronize(st));
+    }
+    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[7] < ends[6] || ends[9] < ends[8] || !vcc_slots_fit(ends[3] - ends[2], n))
+        return AFC_EINVAL;
+    const uint32_t m = (uint32_t)(ends[3] - ends[2]);
+    if (m && (!d_rec_cols || !d_created_at || !d_chain_rec_cols || !d_rec_flags || !d_doc_size || !d_created_off)) return AFC_EINVAL;
+    if (bodies_cap < vcc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4], ends[7] - ends[6], ends[9] - ends[8])) return AFC_EINVAL;
+    const uint64_t dbound = wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4]);
+    launch::VccArgs A{};
+    ChainScratch S;
+    uint8_t* scratch = nullptr;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { vcc_scratch(k, S, A, n, m, dbound); }));
+    vcc_bind(A, S, dir, n, m);
+    A.cols = d_cols; A.col_off = d_col_off; A.rec_off = d_rec_off; A.rec_cols = d_rec_cols; A.rec_col_off = d_rec_col_off; A.created_at = d_created_at;
+    A.chain_cols = d_chain_cols; A.chain_col_off = d_chain_col_off; A.clock = d_clock; A.chain_rec_cols = d_chain_rec_cols;
+    A.chain_rec_col_off = d_chain_rec_col_off; A.rec_flags = d_rec_flags; A.doc_size = d_doc_size; A.created_off = d_created_off;
+    A.bodies = d_bodies; A.body_off = d_body_off; A.state = d_state;
+    cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, S.doc_off, S.summary, S.wstate, S.W, st, lc);
+    if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m,
+                                        S.docs, S.doc_off, S.pv, S.wstate, S.summary, S.W, st, lc);
+    if (e == cudaSuccess) e = launch::vcc_sizes(A, st, lc);
+    if (e == cudaSuccess) e = launch::vcc_emit(A, st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                const uint64_t* col_off, const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off,
+                                const int64_t* created_at, const uint8_t* chain_cols, const uint64_t* chain_col_off, const int64_t* clock,
+                                const uint8_t* chain_rec_cols, const uint64_t* chain_rec_col_off, const uint8_t* rec_flags, const int64_t* doc_size,
+                                const int32_t* created_off, const afc_did_directory* dir, uint32_t n, uint8_t* bodies, uint64_t bodies_cap,
+                                uint64_t* body_off, uint8_t* state) {
+    int rc = vcc_check(ctx, expanded96, n_keys, key_index, cols, col_off, rec_off, rec_col_off, chain_cols, chain_col_off, clock, chain_rec_col_off,
+                       dir, n, bodies, body_off, state);
+    if (rc != AFC_OK) return rc;
+    if (n == 0) { body_off[0] = 0; return AFC_OK; }
+    for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
+    const uint32_t C = AFC_WORKFLOW_COLUMNS, CC = AFC_CHAIN_WORKFLOW_COLUMNS, RC_ = AFC_CHAIN_RECORD_COLUMNS;
+    uint64_t bad = 0;
+    for (size_t k = 0; k < (size_t)n * C; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
+    for (size_t k = 0; k < (size_t)n * CC; k++) bad |= (uint64_t)(chain_col_off[k + 1] < chain_col_off[k]);
+    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(rec_off[i + 1] < rec_off[i]);
+    if (bad || !vcc_slots_fit(rec_off[n] - rec_off[0], n)) return AFC_EINVAL;
+    for (uint64_t k = 2 * rec_off[0]; k < 2 * rec_off[n]; k++) bad |= (uint64_t)(rec_col_off[k + 1] < rec_col_off[k]);
+    for (uint64_t k = RC_ * rec_off[0]; k < RC_ * rec_off[n]; k++) bad |= (uint64_t)(chain_rec_col_off[k + 1] < chain_rec_col_off[k]);
+    if (bad || bodies_cap < afc_vc_workflow_chain_bound(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off, n)) return AFC_EINVAL;
+    if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at || !chain_rec_cols || !rec_flags || !doc_size || !created_off)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    // Chunks of whole workflows through the ring, as for workflow credentials: the record arrays are staged for the chunk's records and
+    // addressed from a shifted base, so absolute record indices stay valid; a workflow larger than a chunk's byte budget goes alone.
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        const uint64_t r0 = rec_off[i0], r = rec_off[i + 1];
+        return (col_off[(size_t)(i + 1) * C] - col_off[(size_t)i0 * C]) + (chain_col_off[(size_t)(i + 1) * CC] - chain_col_off[(size_t)i0 * CC]) +
+               (rec_col_off[2 * r] - rec_col_off[2 * r0]) + (chain_rec_col_off[RC_ * r] - chain_rec_col_off[RC_ * r0]) + 64 * (r - r0);
+    };
+    uint64_t base = 0;
+    return with_device_keys(ctx, expanded96, n_keys, [&](const uint8_t* d_keys) {
+        Ring ring(ctx);
+        return ring.walk(n, measure, [&](Ring& r) {
+            const uint32_t i0 = r.i0, cnt = r.cnt;
+            const uint64_t cbase = col_off[(size_t)i0 * C], cbytes = col_off[(size_t)(i0 + cnt) * C] - cbase;
+            const uint64_t ccbase = chain_col_off[(size_t)i0 * CC], ccbytes = chain_col_off[(size_t)(i0 + cnt) * CC] - ccbase;
+            const uint64_t r0 = rec_off[i0], r1 = rec_off[i0 + cnt];
+            const uint64_t rbase = rec_col_off[2 * r0], rbytes = rec_col_off[2 * r1] - rbase;
+            const uint64_t crbase = chain_rec_col_off[RC_ * r0], crbytes = chain_rec_col_off[RC_ * r1] - crbase;
+            const uint32_t m = (uint32_t)(r1 - r0);
+            const uint64_t dbound = wf_doc_bound(cnt, cbytes, m, rbytes), bbound = vcc_bound(cnt, cbytes, m, rbytes, ccbytes, crbytes);
+            const uint32_t* d_ki;
+            launch::VccArgs A{};
+            ChainScratch S;
+            RC(r.stage([&](Stager& k) {
+                A.cols = k.in_at(cols, cbase, cbytes, 16);
+                A.col_off = k.in(col_off, (size_t)i0 * C, (size_t)cnt * C + 1);
+                d_ki = k.in(key_index, i0, cnt);
+                A.rec_off = k.in(rec_off, i0, (size_t)cnt + 1);
+                A.rec_cols = k.in_at(rec_cols, rbase, rbytes, 16);
+                A.rec_col_off = k.in(rec_col_off, 2 * r0, m ? 2 * (size_t)m + 1 : 0);
+                A.created_at = k.in(created_at, 2 * r0, 2 * (size_t)m);
+                A.chain_cols = k.in_at(chain_cols, ccbase, ccbytes, 16);
+                A.chain_col_off = k.in(chain_col_off, (size_t)i0 * CC, (size_t)cnt * CC + 1);
+                A.clock = k.in(clock, 3 * (size_t)i0, 3 * (size_t)cnt);
+                A.chain_rec_cols = k.in_at(chain_rec_cols, crbase, crbytes, 16);
+                A.chain_rec_col_off = k.in(chain_rec_col_off, RC_ * r0, m ? RC_ * (size_t)m + 1 : 0);
+                A.rec_flags = k.in(rec_flags, r0, m);
+                A.doc_size = k.in(doc_size, r0, m);
+                A.created_off = k.in(created_off, r0, m);
+                A.bodies = k.take(bbound + 64);
+                A.body_off = k.take<uint64_t>((size_t)cnt + 1);
+                A.state = k.take(cnt);
+                vcc_scratch(k, S, A, cnt, m, dbound);
+            }));
+            A.rec_col_off -= 2 * r0;                // absolute record indices stay valid
+            A.created_at -= 2 * r0;
+            A.chain_rec_col_off -= RC_ * r0;
+            A.rec_flags -= r0;
+            A.doc_size -= r0;
+            A.created_off -= r0;
+            vcc_bind(A, S, dir, cnt, m);
+            CK(wf_sizes(A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, cnt, m, S.doc_off, S.summary, S.wstate, S.W, r.st, r.lc));
+            CK(wf_finish(ctx, d_keys, n_keys, d_ki, A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, cnt, m, S.docs, S.doc_off,
+                         S.pv, S.wstate, S.summary, S.W, r.st, r.lc));
+            CK(launch::vcc_sizes(A, r.st, r.lc));
+            uint64_t bytes;
+            RC(r.read(&bytes, {A.body_off + cnt}));
+            CK(launch::vcc_emit(A, r.st, r.lc));
+            RC(r.copy_back({offsets_out(body_off, i0, A.body_off, (size_t)cnt + 1, base), {state, i0, A.state, cnt}, {bodies, base, A.bodies, bytes}}));
             base += bytes;
             return AFC_OK;
         });

@@ -269,6 +269,123 @@ class ExpandedKeys:
         return [{"vc_document": buf[int(off[i]):int(off[i + 1])], "signature": pv[i].tobytes().decode() if state[i] == _abi.WORKFLOW_BUILT else "",
                  "state": int(state[i]), "summary": [int(x) for x in summ[i]]} for i in range(n)]
 
+    # -- workflow VC chains (afc_vc_workflow_chain_batch)
+    @staticmethod
+    def pack_chain_requests(workflows):
+        """GetWorkflowVCChain inputs: the dicts of services.VCService.get_workflow_vc_chain_batch (those of issue_workflow_vc_batch, each
+        ExecutionVC record complete: execution_id, workflow_id, session_id, agent_node_id / workflow_name (None = nil), issuer_did,
+        target_did, caller_did, vc_document (bytes, None = nil), signature, storage_uri, document_size_bytes, input_hash, output_hash,
+        status, created_at (an aware datetime); plus workflow_vc_id, resolved_at and snapshot, an aware datetime) -> the host arrays of
+        afc_vc_workflow_chain_batch after key_index: pack_workflow_requests's six, then chain_cols, chain_col_off, clock, chain_rec_cols,
+        chain_rec_col_off, rec_flags, doc_size, created_off."""
+        def b(v):
+            return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+        wcols, rcols, clock, flags, size, zone = [], [], [], [], [], []
+        for w in workflows:
+            wcols += [b(w["workflow_vc_id"]), b(w["resolved_at"])]
+            clock += unix_pair(w["snapshot"]) + [zone_seconds(w["snapshot"])]
+            for v in w["execution_vcs"]:
+                f = 0
+                for key, bit in (("agent_node_id", _abi.CHAIN_AGENT_NODE_ID_NIL), ("workflow_name", _abi.CHAIN_WORKFLOW_NAME_NIL),
+                                 ("vc_document", _abi.CHAIN_VC_DOCUMENT_NIL)):
+                    if v.get(key) is None:
+                        f |= bit
+                rcols += [b(v.get(k) or b"") for k in _abi.CHAIN_RECORD_COLUMNS]
+                flags.append(f)
+                size.append(int(v["document_size_bytes"]))
+                zone.append(zone_seconds(v["created_at"]))
+        chain_cols, chain_col_off = pack(wcols)
+        chain_rec_cols, chain_rec_col_off = pack(rcols)
+        return (*ExpandedKeys.pack_workflow_requests(workflows), chain_cols, chain_col_off, np.array(clock, dtype=np.int64), chain_rec_cols,
+                chain_rec_col_off, np.array(flags + [0], dtype=np.uint8), np.array(size + [0], dtype=np.int64), np.array(zone + [0], dtype=np.int32))
+
+    _chain_coef = None
+
+    @classmethod
+    def _chain_bound(cls, n, col_bytes, records, rec_bytes, chain_col_bytes, chain_rec_bytes):
+        """afc_vc_workflow_chain_bound for n workflows with these totals.  The library needs offset arrays that span the batch's records,
+        which the device call only has on the device; the bound is linear in the six totals, so its coefficients are read off the library
+        once, with one-workflow arrays (tests/test_vcchain_hostsim.py holds this equal to the library's bound)."""
+        if cls._chain_coef is None:
+            lib = _abi.load()
+            a = [np.zeros(len(_abi.WORKFLOW_COLUMNS) + 1, dtype=np.uint64), np.zeros(2, dtype=np.uint64), np.zeros(3, dtype=np.uint64),
+                 np.zeros(3, dtype=np.uint64), np.zeros(len(_abi.CHAIN_RECORD_COLUMNS) + 1, dtype=np.uint64)]
+
+            def f(k=None, at=None):
+                if k is not None:
+                    a[k][at] = 1
+                v = lib.afc_vc_workflow_chain_bound(*[_abi.ptr(x) for x in a], 1)
+                if k is not None and k != 1:
+                    a[k][at] = 0
+                return v
+            fixed = f()
+            per_col, per_ccol = f(0, -1) - fixed, f(3, -1) - fixed
+            per_rec = f(1, 1) - fixed                                  # rec_off stays [0, 1] for the two per-record-byte probes
+            cls._chain_coef = (fixed, per_col, per_rec, f(2, 2) - fixed - per_rec, per_ccol, f(4, -1) - fixed - per_rec)
+        c = cls._chain_coef
+        return n * c[0] + c[1] * col_bytes + c[2] * records + c[3] * rec_bytes + c[4] * chain_col_bytes + c[5] * chain_rec_bytes if n else 0
+
+    @classmethod
+    def _chain_bound_dev(cls, n, d_col_off, d_rec_off, d_rec_col_off, d_ccol_off, d_crcol_off):
+        """_chain_bound of device offset arrays: their ten ends in one device-to-host copy."""
+        import torch
+        C, RC = len(_abi.WORKFLOW_COLUMNS), len(_abi.CHAIN_RECORD_COLUMNS)
+        at = lambda t, k: t[k:k + 1]                                # views: no index tensor crosses to the device
+        r = torch.cat([at(d_rec_off, 0), at(d_rec_off, n)])
+        e = [int(x) for x in torch.cat([at(d_col_off, 0), at(d_col_off, C * n), r, d_rec_col_off.index_select(0, 2 * r), at(d_ccol_off, 0),
+                                        at(d_ccol_off, 2 * n), d_crcol_off.index_select(0, RC * r)]).cpu().tolist()]
+        span = lambda lo, hi: max(hi - lo, 0)
+        return cls._chain_bound(n, span(e[0], e[1]), span(e[2], e[3]), span(e[4], e[5]), span(e[6], e[7]), span(e[8], e[9]))
+
+    def workflow_chain_packed(self, directory, key_index, *arrays, expanded=None):
+        """afc_vc_workflow_chain_batch on host arrays (the layout of pack_chain_requests).  Returns (bodies uint8, body_off uint64 [n+1],
+        state uint8 [n])."""
+        n = len(key_index)
+        cols, col_off, rec_off, rec_cols, rec_col_off, created, chain_cols, chain_col_off, clock, crec_cols, crec_col_off, flags, size, zone = arrays
+        created = np.ascontiguousarray(created if len(created) else np.zeros(2, dtype=np.int64))
+        exp = self._expanded if expanded is None else expanded
+        lib = _abi.load()
+        cap = lib.afc_vc_workflow_chain_bound(_abi.ptr(col_off), _abi.ptr(rec_off), _abi.ptr(rec_col_off), _abi.ptr(chain_col_off),
+                                              _abi.ptr(crec_col_off), n)
+        bodies = np.empty(max(cap, 1), dtype=np.uint8)
+        body_off = np.zeros(n + 1, dtype=np.uint64)
+        state = np.empty(max(n, 1), dtype=np.uint8)
+        _abi.check(lib.afc_vc_workflow_chain_batch(self.ctx.handle, _abi.ptr(exp), exp.shape[0], _abi.ptr(key_index), _abi.ptr(cols),
+                                                   _abi.ptr(col_off), _abi.ptr(rec_off), _abi.ptr(rec_cols), _abi.ptr(rec_col_off), _abi.ptr(created),
+                                                   _abi.ptr(chain_cols), _abi.ptr(chain_col_off), _abi.ptr(clock), _abi.ptr(crec_cols),
+                                                   _abi.ptr(crec_col_off), _abi.ptr(flags), _abi.ptr(size), _abi.ptr(zone), directory.handle, n,
+                                                   _abi.ptr(bodies), cap, _abi.ptr(body_off), _abi.ptr(state)), self.ctx.handle)
+        return bodies[:int(body_off[n])], body_off, state[:n]
+
+    def workflow_chain_dev(self, directory, d_key_index, d_arrays, n, stream=None, d_expanded=None):
+        """afc_vc_workflow_chain_batch_dev: d_arrays are the 14 arrays of pack_chain_requests on the device (offsets as int64, uint32
+        arrays as int32).  Returns (d_bodies uint8, d_body_off int64 [n+1], d_state uint8 [n])."""
+        import torch
+        d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created, d_ccols, d_ccol_off, d_clock, d_crcols, d_crcol_off, d_flags, d_size, d_zone = d_arrays
+        dev = d_col_off.device
+        if d_expanded is None:
+            d_expanded = torch.from_numpy(self._expanded).to(dev)
+        lib = _abi.load()
+        cap = self._chain_bound_dev(n, d_col_off, d_rec_off, d_rec_col_off, d_ccol_off, d_crcol_off) if n else 0
+        d_bodies = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        d_body_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_state = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        _abi.check(lib.afc_vc_workflow_chain_batch_dev(self.ctx.handle, _abi.ptr(d_expanded), d_expanded.shape[0], _abi.ptr(d_key_index),
+                                                       *[_abi.ptr(t) for t in d_arrays], directory.handle, n, _abi.ptr(d_bodies), cap,
+                                                       _abi.ptr(d_body_off), _abi.ptr(d_state), self.ctx._stream(stream)), self.ctx.handle)
+        total = int(d_body_off[n]) if n else 0
+        return d_bodies[:total], d_body_off, d_state[:n]
+
+    def workflow_chains(self, workflows, directory):
+        """GetWorkflowVCChain + c.JSON for many workflows in one host-buffer call: [(state, body bytes)] (an AFC_CHAIN_HOST workflow has an
+        empty body)."""
+        if not workflows:
+            return []
+        ki = self.key_index([self.workflow_issuer(w) for w in workflows])
+        bodies, off, state = self.workflow_chain_packed(directory, ki, *self.pack_chain_requests(workflows))
+        buf = bodies.tobytes()
+        return [(int(state[i]), buf[int(off[i]):int(off[i + 1])]) for i in range(len(workflows))]
+
     # -- agent DID registration (afc_did_register_batch)
     def _append(self, expanded, dids):
         base = self._expanded.shape[0]
@@ -551,6 +668,41 @@ def unix_pair(t):
         raise ValueError("created_at must be an aware datetime")
     d = t - _EPOCH
     return [d.days * 86400 + d.seconds, d.microseconds * 1000]
+
+
+def zone_seconds(t):
+    """The UTC offset of an aware datetime in seconds."""
+    return int(t.utcoffset().total_seconds())
+
+
+class DIDDirectory:
+    """afc_did_directory: the public half of a DID registry on the device — DIDs, their public keys and their order — for the DID
+    resolution bundle of workflow chains.  No verify tables are built (a KeySet's are 384 KB per key)."""
+
+    def __init__(self, dids, pks, ctx=None):
+        self.ctx = ctx or default_context()
+        self._lib = _abi.load()
+        if len(dids) != len(pks) or any(len(p) != 32 for p in pks):
+            raise ValueError("one 32-byte public key per DID")
+        self.dids = [d.encode("utf-8", "surrogatepass") if isinstance(d, str) else bytes(d) for d in dids]
+        self.pks = [bytes(p) for p in pks]
+        buf, off = pack(self.dids)
+        arr = np.frombuffer(b"".join(self.pks) or bytes(32), dtype=np.uint8).copy()
+        h = C.c_void_p()
+        _abi.check(self._lib.afc_did_directory_new(self.ctx.handle, _abi.ptr(arr), _abi.ptr(buf), _abi.ptr(off), len(self.dids), C.byref(h)),
+                   self.ctx.handle)
+        self.handle = h
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self._lib.afc_did_directory_free(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class KeySet:

@@ -329,6 +329,24 @@ class VCService:
                         "snapshot_time": w["snapshot_time"], "storage_uri": "", "document_size_bytes": len(vc_bytes)})
         return out
 
+    # -- workflow VC chains (vc_service.go:292-338, 810-870; internal/handlers/ui/did.go:383)
+    def get_workflow_vc_chain_batch(self, workflows, directory):
+        """GetWorkflowVCChain + c.JSON for many workflows, in request order: each body is the bytes the chain endpoint writes.  Each
+        workflow: the inputs of issue_workflow_vc_batch with complete ExecutionVC records (ExpandedKeys.pack_chain_requests), plus
+        workflow_vc_id, resolved_at and snapshot (an aware datetime).  directory: an identity.DIDDirectory (DIDService.did_directory).
+        One device call (ExpandedKeys.workflow_chains); workflows it declines (AFC_CHAIN_HOST) are built by the host mirror,
+        workflow_chain_body over issue_workflow_vc_batch's output, which raises ValueError where json.Marshal fails in Go."""
+        if not workflows:
+            return []
+        res = self.keys.workflow_chains(workflows, directory)
+        out = [body for _, body in res]
+        host = [i for i, (st, _) in enumerate(res) if st == _abi.CHAIN_HOST]
+        if host:
+            keys = dict(zip(directory.dids, directory.pks))
+            for i, wvc in zip(host, self.issue_workflow_vc_batch([workflows[i] for i in host])):
+                out[i] = workflow_chain_body(workflows[i], wvc, keys)
+        return out
+
     def _keyed_verify(self, dids, msgs, proof_values):
         """ed25519.Verify for many (issuer DID, canonical bytes, base64url signature) through one keyed GPU batch.  A DID the
         cache cannot resolve or a signature that does not decode gives None (the reference reports those as errors, not False)."""
@@ -669,6 +687,100 @@ class VCService:
         return out
 
 
+def _marshal_time(t) -> str:
+    """Time.MarshalJSON of an aware datetime (microsecond precision): RFC3339Nano, Z for a zero offset."""
+    off = int(t.utcoffset().total_seconds())
+    text = "%04d-%02d-%02dT%02d:%02d:%02d" % (t.year, t.month, t.day, t.hour, t.minute, t.second)
+    if t.microsecond:
+        text += ("." + "%06d" % t.microsecond).rstrip("0")
+    if off == 0:
+        return text + "Z"
+    a = abs(off) // 60
+    return text + "%s%02d:%02d" % ("-" if off < 0 else "+", a // 60, a % 60)
+
+
+def _compact(raw: bytes) -> bytes:
+    """appendCompact(dst, raw, escapeHTML=true), which json.Marshal runs over a RawMessage; ValueError where it fails."""
+    if not raw:
+        raise ValueError("json: error calling MarshalJSON for type json.RawMessage: unexpected end of JSON input")
+    json.loads(raw.decode("utf-8", "surrogateescape"), parse_constant=_reject_constant)
+    out, in_str, esc, i = bytearray(), False, False, 0
+    while i < len(raw):
+        c = raw[i]
+        if c in b"<>&":
+            out += b"\\u00%02x" % c
+        elif c == 0xE2 and raw[i + 1:i + 3] in (b"\x80\xa8", b"\x80\xa9") and i + 2 < len(raw):
+            out += b"\\u202" + (b"8" if raw[i + 2] == 0xA8 else b"9")
+            i += 3
+            continue
+        elif in_str:
+            out.append(c)
+            esc, in_str = (False, in_str) if esc else (c == 0x5C, c != 0x22)
+        elif c not in b" \t\n\r":
+            out.append(c)
+            in_str = c == 0x22
+        i += 1
+    return bytes(out)
+
+
+def _reject_constant(name):
+    raise ValueError("invalid character %r" % name)
+
+
+def workflow_chain_body(w, wvc, keys) -> bytes:
+    """json.Marshal(types.WorkflowVCChainResponse) for one workflow on the host: w as get_workflow_vc_chain_batch takes it, wvc its
+    issue_workflow_vc_batch result, keys the registry's public keys by DID (bytes)."""
+    S = go_json.any_string
+    evs = w["execution_vcs"]
+    recs = []
+    for v in evs:
+        parts = ['"vc_id":' + S(v["vc_id"]), '"execution_id":' + S(v["execution_id"]), '"workflow_id":' + S(v["workflow_id"]),
+                 '"session_id":' + S(v["session_id"])]
+        for k in ("agent_node_id", "workflow_name"):
+            if v.get(k) is not None:
+                parts.append('"%s":' % k + S(v[k]))
+        doc = "null" if v.get("vc_document") is None else _compact(bytes(v["vc_document"])).decode("utf-8", "surrogateescape")
+        parts += ['"issuer_did":' + S(v["issuer_did"]), '"target_did":' + S(v["target_did"]), '"caller_did":' + S(v["caller_did"]),
+                  '"vc_document":' + doc, '"signature":' + S(v["signature"]), '"storage_uri":' + S(v["storage_uri"]),
+                  '"document_size_bytes":%d' % v["document_size_bytes"], '"input_hash":' + S(v["input_hash"]), '"output_hash":' + S(v["output_hash"]),
+                  '"status":' + S(v["status"]), '"created_at":"%s"' % _marshal_time(v["created_at"])]
+        recs.append("{" + ",".join(parts) + "}")
+    times = [v["created_at"] for v in evs]
+    start = min(times) if evs else w["snapshot"]
+    wf = ['"workflow_id":' + S(w["workflow_id"]), '"session_id":' + S(wvc["session_id"]), '"component_vcs":' + "[" + ",".join(S(x) for x in wvc["component_vcs"]) + "]",
+          '"workflow_vc_id":' + S(w["workflow_vc_id"]), '"status":' + S(wvc["status"]), '"start_time":"%s"' % _marshal_time(evs[times.index(start)]["created_at"] if evs else start)]
+    if wvc["end_time"] is not None:
+        wf.append('"end_time":"%s"' % _marshal_time(evs[times.index(max(times))]["created_at"]))
+    doc = wvc["vc_document"]
+    wf += ['"total_steps":%d' % len(evs), '"completed_steps":%d' % wvc["completed_steps"], '"vc_document":' + doc.decode("utf-8", "surrogateescape")]
+    if wvc["signature"]:
+        wf.append('"signature":' + S(wvc["signature"]))
+    if wvc["issuer_did"]:
+        wf.append('"issuer_did":' + S(wvc["issuer_did"]))
+    wf += ['"snapshot_time":"%s"' % _marshal_time(w["snapshot"]), '"storage_uri":""', '"document_size_bytes":%d' % len(doc)]
+    top = ['"workflow_id":' + S(w["workflow_id"]), '"component_vcs":[' + ",".join(recs) + "]", '"workflow_vc":{' + ",".join(wf) + "}",
+           '"total_steps":%d' % len(evs), '"status":' + S(wvc["status"])]
+    enc = lambda x: x.encode("utf-8", "surrogatepass") if isinstance(x, str) else bytes(x)
+    wanted = set()
+    for d in [x for v in evs for x in (v["issuer_did"], v["caller_did"], v["target_did"])] + [wvc["issuer_did"]]:
+        d = enc(d)
+        if d in (b"", b"did:key:") or not d.decode("utf-8", "replace").strip(_GO_SPACE) or d not in keys:
+            continue
+        wanted.add(d)
+    if wanted:
+        ents = []
+        for d in sorted(wanted):
+            method = d.split(b":")[1] if len(d) > 4 and d[:4] == b"did:" else b"key"
+            x = base64.urlsafe_b64encode(keys[d]).rstrip(b"=").decode()
+            ents.append(S(d) + ':{"method":' + S(method) + ',"public_key_jwk":{"alg":"EdDSA","crv":"Ed25519","kty":"OKP","use":"sig","x":"' + x +
+                        '"},"resolved_from":"bundled","resolved_at":' + S(w["resolved_at"]) + "}")
+        top.append('"did_resolution_bundle":{' + ",".join(ents) + "}")
+    return ("{" + ",".join(top) + "}").encode("utf-8", "surrogateescape")
+
+
+_GO_SPACE = "\t\n\v\f\r \x85\xa0\u1680\u2000\u2001\u2002\u2003\u2004\u2005\u2006\u2007\u2008\u2009\u200a\u2028\u2029\u202f\u205f\u3000"
+
+
 def _issue(kind, severity, component, description, field="", expected="", actual=""):
     """types.VerificationIssue (vc_service.go:880-889)."""
     return {"type": kind, "severity": severity, "component": component, "field": field, "expected": expected, "actual": actual,
@@ -923,6 +1035,30 @@ class DIDService:
             seen.add(k)
             todo.append(r)
         return self._register(todo) if todo else []
+
+    ROOT_PATH = "m/44'/0'"
+
+    @property
+    def root_did(self):
+        """registry.RootDID: generateDIDFromSeed(masterSeed, "m/44'/0'") (did_service.go:61); its key joins `keys`, since the workflow
+        credential of a workflow without records is issued under it (vc_service.go:577-580)."""
+        if getattr(self, "_root_did", None) is None:
+            self._root_did = self.keys.derive(self.master_seed, [self.ROOT_PATH])[0]
+        return self._root_did
+
+    def did_directory(self, ctx=None):
+        """The registry's public half on the device (identity.DIDDirectory): every DID ResolveDID resolves (did_service.go:368-473) with
+        its public key — the root DID (the key at m/44'/0'), then every agent's and component's DID with the key its stored public JWK
+        holds (the JWK's x).  A DID the registry holds twice (re-registration gives every new component of one kind the same DID) is
+        taken once: its key is the same."""
+        from .identity import DIDDirectory
+        keys = {self.root_did: self.keys.public_key(self.root_did)}
+        for a in self.agent_nodes.values():
+            for e in [a] + list(a["reasoners"].values()) + list(a["skills"].values()):
+                if e["did"] not in keys:
+                    x = json.loads(e["public_key_jwk"])["x"]
+                    keys[e["did"]] = base64.urlsafe_b64decode(x + "=" * (-len(x) % 4))
+        return DIDDirectory(list(keys), list(keys.values()), ctx=ctx or self.keys.ctx)
 
     def _reregister(self, requests):
         reqs = []

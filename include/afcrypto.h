@@ -400,6 +400,69 @@ int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
                                     const int64_t* d_created_at, uint32_t n, uint8_t* d_docs, uint64_t docs_cap, uint64_t* d_doc_off,
                                     uint8_t* d_proof_values, uint8_t* d_state, uint32_t* d_summary, void* stream);
 
+/* ---- E4: workflow VC chains served in one call: GetWorkflowVCChain (internal/services/vc_service.go:292-338) with
+ * collectDIDResolutionBundle (:810-870) and the handler's c.JSON (internal/handlers/ui/did.go:383), for n workflows.
+ * afc_did_directory_new: the registry's public half — n DIDs (did i = dids[did_off[i] .. did_off[i+1]), n + 1 offsets) and their public
+ * keys (pks, n x 32), looked up as a named key set looks up its DIDs, with each DID's rank in byte order (strings.Compare) computed once.
+ * No verify tables are built, so a directory of 10^6 DIDs takes tens of MB.  A duplicate DID, a NULL pointer or offsets that run
+ * backwards give AFC_EINVAL.
+ * afc_vc_workflow_chain_batch writes, for workflow i, bodies[body_off[i] .. body_off[i+1]): json.Marshal(types.WorkflowVCChainResponse),
+ * HTML escaping on, byte for byte, and state[i]:
+ *   AFC_CHAIN_BUILT   the body
+ *   AFC_CHAIN_HOST    a zero-length body; the caller builds it itself.  HOST covers every AFC_WORKFLOW_HOST workflow of the issue call;
+ *                     a non-nil vc_document that is empty or not JSON (json.Marshal fails in Go), or nested deeper than 32; a created_at
+ *                     or snapshot time whose UTC offset is not a whole number of minutes or is 24 hours or more, or whose local year
+ *                     falls outside 1..9999; a resolved_at column longer than 64 bytes; a DID longer than 128 bytes that the bundle would hold.
+ * The body: component_vcs holds each record in ExecutionVC field order, agent_node_id / workflow_name omitted when nil, vc_document
+ * compacted as Go's appendCompact does (whitespace outside strings dropped; < > & U+2028 U+2029 escaped), null when nil, created_at as
+ * Time.MarshalJSON writes it; parent_vc_id and child_vc_ids are never set by storage (vc_storage.go:234-263), so they are never written.
+ * workflow_vc is the credential afc_vc_issue_workflow_batch issues on the same inputs (vc_document, signature = its proof value), with
+ * start_time / end_time at full precision from the records summary[2] / [3] names, in their own offsets, and snapshot_time from the clock.
+ * did_resolution_bundle holds the issuer, caller and target DIDs of every record and the credential's issuer, without "", "did:key:" and
+ * DIDs strings.TrimSpace empties, that the directory holds, once each, in byte order; each with its method (strings.Split(did, ":")[1]
+ * after a "did:" prefix and more, "key" otherwise), the public JWK ed25519PublicKeyToJWK writes for the directory's key, "bundled" and
+ * resolved_at.  The member is omitted when the bundle is empty.
+ * Inputs: every argument of afc_vc_issue_workflow_batch, unchanged, and
+ *   chain_cols / chain_col_off      AFC_CHAIN_WORKFLOW_COLUMNS byte strings per workflow, 2n + 1 absolute offsets
+ *   clock                           3 int64 per workflow: the snapshot time as Unix seconds, nanoseconds and UTC offset in seconds; also
+ *                                   StartTime of a workflow without records (the reference reads time.Now() for both)
+ *   chain_rec_cols / chain_rec_col_off   AFC_CHAIN_RECORD_COLUMNS byte strings per record, indexed by absolute record as rec_col_off
+ *   rec_flags                       per record: AFC_CHAIN_AGENT_NODE_ID_NIL, AFC_CHAIN_WORKFLOW_NAME_NIL, AFC_CHAIN_VC_DOCUMENT_NIL
+ *   doc_size                        per record: document_size_bytes
+ *   created_off                     per record: the UTC offset of created_at in seconds
+ * bodies_cap must be at least afc_vc_workflow_chain_bound(...), computed from the ends of the five offset arrays alone and additive over
+ * workflows (else AFC_EINVAL, before any work).  Other AFC_EINVAL: a NULL pointer, n_keys == 0, a directory of another context, more
+ * than 2^31 - 1 DID occurrence slots (3 per record, 1 per workflow); in the host-buffer call also key_index[i] >= n_keys and offsets
+ * that run backwards.  The host-buffer call streams chunks of whole workflows through the context's staging ring; the expanded keys it
+ * stages are wiped from the device when it returns.  The _dev call synchronises `stream` once, to read the ends of the offset arrays; expanded96 must be 16-byte aligned there.
+ * n = 0 writes body_off[0] = 0 in the host-buffer call and nothing in the _dev call. */
+typedef struct afc_did_directory afc_did_directory;
+int afc_did_directory_new(afc_ctx* ctx, const uint8_t* pks /* n x 32 */, const uint8_t* dids, const uint64_t* did_off /* n+1 */, uint32_t n,
+                          afc_did_directory** out);
+void afc_did_directory_free(afc_did_directory* dir);
+#define AFC_CHAIN_WORKFLOW_COLUMNS 2   /* workflow_vc_id, resolved_at */
+#define AFC_CHAIN_RECORD_COLUMNS 13    /* execution_id, workflow_id, session_id, agent_node_id, workflow_name, issuer_did, target_did,
+                                          caller_did, vc_document, signature, storage_uri, input_hash, output_hash */
+#define AFC_CHAIN_AGENT_NODE_ID_NIL 1
+#define AFC_CHAIN_WORKFLOW_NAME_NIL 2
+#define AFC_CHAIN_VC_DOCUMENT_NIL 4
+#define AFC_CHAIN_BUILT 0
+#define AFC_CHAIN_HOST 1
+uint64_t afc_vc_workflow_chain_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
+                                     const uint64_t* chain_rec_col_off, uint32_t n);
+int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
+                                const uint64_t* col_off, const uint64_t* rec_off, const uint8_t* rec_cols, const uint64_t* rec_col_off,
+                                const int64_t* created_at, const uint8_t* chain_cols, const uint64_t* chain_col_off /* 2n+1 */,
+                                const int64_t* clock /* 3n */, const uint8_t* chain_rec_cols, const uint64_t* chain_rec_col_off /* 13 per record +1 */,
+                                const uint8_t* rec_flags, const int64_t* doc_size, const int32_t* created_off, const afc_did_directory* dir, uint32_t n,
+                                uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off /* n+1 */, uint8_t* state /* n */);
+int afc_vc_workflow_chain_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, uint32_t n_keys, const uint32_t* d_key_index, const uint8_t* d_cols,
+                                    const uint64_t* d_col_off, const uint64_t* d_rec_off, const uint8_t* d_rec_cols, const uint64_t* d_rec_col_off,
+                                    const int64_t* d_created_at, const uint8_t* d_chain_cols, const uint64_t* d_chain_col_off, const int64_t* d_clock,
+                                    const uint8_t* d_chain_rec_cols, const uint64_t* d_chain_rec_col_off, const uint8_t* d_rec_flags,
+                                    const int64_t* d_doc_size, const int32_t* d_created_off, const afc_did_directory* dir, uint32_t n,
+                                    uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream);
+
 /* ---- W2: execution webhook deliveries built and signed in one call: determineWebhookEvent + buildPayload + json.Marshal +
  * generateWebhookSignature (internal/services/webhook_dispatcher.go:294-320, 394-474) for n deliveries.  For delivery i:
  *   bodies[body_off[i] .. body_off[i+1])   the request body json.Marshal(types.ExecutionWebhookPayload), the result member being

@@ -734,13 +734,124 @@ def reregister_block(ctx, dev, timed):
                        "note": "tests/didrr_oracle.py: the reference's branch restated in Python, one core; not the Go service"}}
 
 
+def chain_block(ctx, dev, timed):
+    """Workflow VC chains served on the device (afc_vc_workflow_chain_batch): 2^14 workflows of 1-64 records from 1024 issuers (WC.bulk),
+    each record's stored document one of the workflow credentials afc_vc_issue_workflow_batch issued for the first 1024 workflows, callers
+    and targets drawn from 4096 DIDs, a directory of 2^20 DIDs holding the issuers and those 4096; then the same with 1 % of the workflows
+    at 4096 records.  Reported: the _dev call with its per-kernel split, afc_vc_issue_workflow_batch alone on the same inputs (the
+    difference is what the chain costs), the host-buffer call from unpinned numpy arrays, and the host mirror (services.workflow_chain_body
+    over issue_workflow_vc_batch) on 200 workflows."""
+    import datetime as dt
+    import torch
+    import agentfield_b200 as afb
+    from agentfield_b200 import services
+    from agentfield_b200.identity import DIDDirectory
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import workflow_cases as WC
+    n, K, P, D = 1 << 14, 1024, 4096, 1 << 20
+    rng = np.random.default_rng(0xAF3C)
+    cache = afb.ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (8700 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    peers = [b"did:key:zPeer%06d" % k for k in range(P)]
+    names = [d.encode() for d in dids] + peers + [b"did:key:zFill%08d" % k for k in range(D - K - P)]
+    keys = np.frombuffer(rng.integers(0, 256, 32 * D, dtype=np.uint8).tobytes(), dtype=np.uint8).reshape(D, 32)
+    t_0 = time.perf_counter()
+    directory = DIDDirectory(names, [keys[k].tobytes() for k in range(D)], ctx=ctx)
+    ms_directory = (time.perf_counter() - t_0) * 1e3
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a.view(np.int64) if a.dtype == np.uint64 else a)).to(dev)
+    seed_arrays, _ = WC.bulk(K, rng, dids, counts=rng.integers(1, 65, K))
+    sdocs, soff, _, _, _ = cache.issue_workflow_packed(*seed_arrays)
+    sb = sdocs.tobytes()
+    pool = [sb[int(soff[i]):int(soff[i + 1])] for i in range(K)]
+
+    def chain_arrays(arrays):
+        ki, cols, coff, roff, rcols, rcoff, created = arrays
+        m = int(roff[-1])
+        wf_of = np.repeat(np.arange(n), np.diff(roff.astype(np.int64)))
+        caller = rng.integers(0, P, m)
+        target = rng.integers(0, P, m)
+        doc = rng.integers(0, K, m)
+        flat = []
+        for r in range(m):
+            i = int(wf_of[r])
+            flat += [b"exec-%d" % r, b"wf_%08d" % i, b"sess_%08d" % i, b"agent-%d" % (r % 97), b"flow", dids[ki[i]].encode(), peers[target[r]],
+                     peers[caller[r]], pool[doc[r]], b"sig-%d" % r, b"", b"i" * 43, b"o" * 43]
+        crcols, crcoff = afb.crypto.pack(flat)
+        ccols, ccoff = afb.crypto.pack([v for i in range(n) for v in (b"wvc-%d" % i, b"2026-09-21T06:00:07Z")])
+        clock = np.array([x for i in range(n) for x in (1_790_003_700, 5, 0)], dtype=np.int64)
+        size = np.array([len(pool[k]) for k in doc] + [0], dtype=np.int64)
+        return (ki,) + tuple(arrays[1:]) + (ccols, ccoff, clock, crcols, crcoff, np.zeros(m + 1, dtype=np.uint8), size, np.zeros(m + 1, dtype=np.int32))
+
+    def measure(full):
+        ki, rest = full[0], full[1:]
+        D_ = [t(a) for a in rest]
+        d_ki = t(ki.view(np.int32))
+        run = lambda: cache.workflow_chain_dev(directory, d_ki, D_, n, d_expanded=d_exp)
+        bodies, off, state = run()
+        torch.cuda.synchronize()
+        built, total = int((state == 0).sum()), int(off[n])
+        host_bytes = bodies.cpu().numpy().tobytes()
+        del bodies, off, state                                      # each call allocates its bound; keep one at a time
+        ms = timed(run)
+        ctx.profile_begin()
+        timed(run, reps=3)
+        kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+        issue = lambda: cache.issue_workflow_dev(d_ki, *D_[:6], n, d_expanded=d_exp)
+        ms_issue = timed(issue)
+        m = int(rest[2][-1])
+        return {"workflows": n, "records": m, "built": built, "body_bytes": total, "ms": ms, "workflows_per_s": n / (ms * 1e-3),
+                "issue_only_ms": ms_issue, "chain_ms": ms - ms_issue, "kernels_ms": kms}, host_bytes
+    full = chain_arrays(WC.bulk(n, rng, dids, counts=rng.integers(1, 65, n))[0])
+    main_run, dev_bytes = measure(full)
+    torch.cuda.empty_cache()
+    hb, hoff, _ = cache.workflow_chain_packed(directory, *full)
+    host_same = hb.tobytes() == dev_bytes
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        cache.workflow_chain_packed(directory, *full)
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    del hb, dev_bytes
+    # the host mirror on 200 workflows: issue_workflow_vc_batch, then workflow_chain_body
+    svc = services.VCService(cache)
+    ki, cols, coff, roff, rcols, rcoff, created, ccols, ccoff, clock, crcols, crcoff, flags, size, zone = full
+    utc = dt.timezone.utc
+    wfs = []
+    for i in rng.choice(n, 200, replace=False).tolist():
+        evs = []
+        for r in range(int(roff[i]), int(roff[i + 1])):
+            c = [bytes(crcols[int(crcoff[13 * r + k]):int(crcoff[13 * r + k + 1])]) for k in range(13)]
+            v = dict(zip(afb._abi.CHAIN_RECORD_COLUMNS, [x.decode() for x in c[:8]] + [c[8]] + [x.decode() for x in c[9:]]))
+            v.update(vc_id=bytes(rcols[int(rcoff[2 * r]):int(rcoff[2 * r + 1])]).decode(), status=bytes(rcols[int(rcoff[2 * r + 1]):int(rcoff[2 * r + 2])]).decode(),
+                     created_at=dt.datetime.fromtimestamp(int(created[2 * r]), utc), document_size_bytes=int(size[r]))
+            evs.append(v)
+        w = [bytes(cols[int(coff[7 * i + k]):int(coff[7 * i + k + 1])]).decode() for k in range(7)]
+        wfs.append({"workflow_id": w[0], "execution_vcs": evs, "root_did": dids[0], "vc_id": w[3], "workflow_vc_id": "wvc-%d" % i, "issuance_date": w[4],
+                    "snapshot_time": w[5], "proof_created": w[6], "resolved_at": "2026-09-21T06:00:07Z", "snapshot": dt.datetime.fromtimestamp(1_790_003_700, utc)})
+    keys_by_did = dict(zip(directory.dids, directory.pks))
+    t_0 = time.perf_counter()
+    issued = svc.issue_workflow_vc_batch(wfs)
+    mirror = [services.workflow_chain_body(w, v, keys_by_did) for w, v in zip(wfs, issued)]
+    ms_mirror = (time.perf_counter() - t_0) * 1e3
+    torch.cuda.empty_cache()
+    skewed, _ = measure(chain_arrays(WC.bulk(n, rng, dids, counts=rng.integers(1, 65, n), skew=(0.01, 4096))[0]))
+    directory.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "directory": {"dids": D, "build_ms": ms_directory}, "dev_call": main_run, "skewed_1pct_4096": skewed,
+            "host_call": {"ms": ms_host, "workflows_per_s": n / (ms_host * 1e-3), "same_as_dev": bool(host_same), "note": "unpinned numpy buffers"},
+            "host_mirror": {"workflows": len(wfs), "records": sum(len(w["execution_vcs"]) for w in wfs), "ms": ms_mirror,
+                            "workflows_per_s": len(wfs) / (ms_mirror * 1e-3), "body_bytes": sum(len(b) for b in mirror),
+                            "note": "issue_workflow_vc_batch + workflow_chain_body; created_at at whole seconds"}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register",
-                                        "reregister"],
+                                        "reregister", "chain"],
                     default=None,
                     help="run one block")
     args = ap.parse_args()
@@ -757,7 +868,7 @@ def main():
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
               "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block,
-              "reregister": reregister_block}
+              "reregister": reregister_block, "chain": chain_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
