@@ -30,6 +30,10 @@ CHAIN_RECORD_COLUMNS = ("execution_id", "workflow_id", "session_id", "agent_node
                         "vc_document", "signature", "storage_uri", "input_hash", "output_hash")
 CHAIN_AGENT_NODE_ID_NIL, CHAIN_WORKFLOW_NAME_NIL, CHAIN_VC_DOCUMENT_NIL = 1, 2, 4
 CHAIN_BUILT, CHAIN_HOST = 0, 1
+DID_KIND_SERVER, DID_KIND_AGENT, DID_KIND_REASONER, DID_KIND_SKILL = 0, 1, 2, 3
+DID_IDENTITY_COLUMNS = ("derivation_path", "function_name", "public_key_jwk")
+DIDRES_RESOLVE, DIDRES_DOCUMENT = 0, 1
+DIDRES_FOUND, DIDRES_NOT_FOUND, DIDRES_BAD_REQUEST, DIDRES_HOST = 0, 1, 2, 3
 WEBHOOK_COLUMNS = ("execution_id", "run_id", "status", "node_id", "reasoner_id", "target_type", "timestamp", "error_message")
 WEBHOOK_HAS_DURATION, WEBHOOK_HAS_ERROR_MESSAGE, WEBHOOK_HAS_SECRET = 1, 2, 4
 WEBHOOK_BUILT, WEBHOOK_HOST = 0, 1
@@ -110,6 +114,10 @@ SYMBOLS = {
     "afc_vc_workflow_chain_bound": (C.c_uint64, [vp, vp, vp, vp, vp, C.c_uint32]),
     "afc_vc_workflow_chain_batch": (C.c_int, [vp, vp, C.c_uint32] + [vp] * 16 + [C.c_uint32, vp, C.c_uint64, vp, vp]),
     "afc_vc_workflow_chain_batch_dev": (C.c_int, [vp, vp, C.c_uint32] + [vp] * 16 + [C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
+    "afc_did_directory_set_identities": (C.c_int, [vp, vp, vp, vp]),
+    "afc_did_resolve_bound": (C.c_uint64, [vp, vp, C.c_uint32]),
+    "afc_did_resolve_batch": (C.c_int, [vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp]),
+    "afc_did_resolve_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_bound": (C.c_uint64, [vp, vp, C.c_uint32]),
     "afc_webhook_sign_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_webhook_sign_batch_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp]),

@@ -189,6 +189,29 @@ uint64_t vcc_frame_fixed();            // the body bound's constant per workflow
 uint64_t vcc_record_fixed();
 uint64_t vcc_entry_fixed();
 
+// ---- k_didresolve.cu: DIDs resolved and DID documents served on the device (afc_didresolve.cuh).  A directory's identities: per DID a
+// kind and three columns (derivation_path, function_name, public_key_jwk) at icol_off[3 k .. 3 k + 3] (relative offsets), both body
+// lengths (0 = HOST) and the canonical JWK text of the entries whose stored text is not (side_off: n + 1 offsets, an empty range = the
+// stored text is canonical).
+struct DresDir {
+    const uint8_t* dids; const uint32_t* did_off; const uint32_t* slots; uint32_t mask; uint32_t n;
+    const uint8_t* kind; const uint8_t* icols; const uint64_t* icol_off;
+    uint32_t* rlen; uint32_t* dlen; uint64_t* side_off; uint8_t* side;
+};
+// attach: both lengths, each entry's side length in side_off[k + 1] and the largest body in *largest (zeroed by the caller); tape:
+// icol_off[3 n] / 2 + n + 1 entries.  Then, once side_off holds offsets and side its buffer, dres_canon writes the side texts.
+cudaError_t dres_entries(const DresDir& D, uint32_t* tape, uint32_t* largest, cudaStream_t s, LaunchLog* lg);
+cudaError_t dres_canon(const DresDir& D, uint32_t* tape, cudaStream_t s, LaunchLog* lg);
+// n requests: kinds, bytes at req_off[i] .. req_off[i + 1] (absolute).  out: req_off[0], req_off[n], and bit 0 set for offsets that run
+// backwards, bit 1 for a request of DRES_REQ_MAX + 1 bytes or more (out[2] zeroed by the caller)
+cudaError_t dres_ends(const uint64_t* req_off, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
+// states, entries (ent: n) and body lengths in body_off[1..n]; the scan; then the bodies
+cudaError_t dres_probe(const DresDir& D, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, uint8_t* state,
+                       uint32_t* ent, uint64_t* body_off, uint64_t* scan, cudaStream_t s, LaunchLog* lg);
+cudaError_t dres_emit(const DresDir& D, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const uint8_t* state,
+                      const uint32_t* ent, const uint64_t* body_off, uint8_t* bodies, cudaStream_t s, LaunchLog* lg);
+uint64_t dres_request_fixed();         // the bound's constant per request besides the directory's largest body (afc_didresolve.cuh)
+
 // ---- k_didreg.cu: agent DIDs registered on the device (afc_didreg.cuh).  node_off: n + 1 absolute offsets; id_idx: 2n + 1 absolute id
 // indices (request i's reasoners [id_idx[2i], id_idx[2i+1]), skills [id_idx[2i+1], id_idx[2i+2])); id_off: absolute, indexed by absolute id.
 // The m = id_idx[2n] - id_idx[0] ids have per-id scratch; the component outputs hold n + m entries (the components, then zeros).

@@ -157,6 +157,16 @@ struct afc_did_directory {
     uint32_t* d_rank = nullptr;    // n: DID -> rank
     uint32_t* d_order = nullptr;   // n: rank -> DID
     uint8_t* d_pks = nullptr;      // n x 32
+    // identities (afc_did_directory_set_identities): what DID resolution and DID documents need
+    bool has_ids = false;
+    uint32_t largest = 0;          // the longest body any entry gives (HOST entries aside)
+    uint8_t* d_kind = nullptr;     // n
+    uint8_t* d_icols = nullptr;    // derivation_path, function_name, public_key_jwk of each DID back to back
+    uint64_t* d_icol_off = nullptr;// 3n + 1, relative
+    uint32_t* d_rlen = nullptr;    // n: resolve body length, 0 = HOST
+    uint32_t* d_dlen = nullptr;    // n: document body length, 0 = HOST
+    uint64_t* d_side_off = nullptr;// n + 1: the canonical JWK text of entries whose stored text is not canonical
+    uint8_t* d_side = nullptr;
 };
 
 struct afc_merkle_tree {
@@ -1185,7 +1195,7 @@ int afc_keyset_new(afc_ctx* ctx, const uint8_t* pks, uint32_t n_keys, afc_keyset
     if (e == cudaSuccess) {
         CallLog lc(ctx);
         e = launch::ed_build_key_tables(ks->d_pks, n_keys, ks->d_tabs, ks->d_valid, d_bases, 0, lc);
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+        if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
     }
     if (d_bases) cudaFree(d_bases);
     if (e != cudaSuccess) {
@@ -1817,7 +1827,8 @@ int afc_did_directory_new(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids,
 void afc_did_directory_free(afc_did_directory* dir) {
     if (!dir) return;
     cudaSetDevice(dir->ctx->device);
-    void* bufs[] = {dir->d_dids, dir->d_did_off, dir->d_slots, dir->d_rank, dir->d_order, dir->d_pks};
+    void* bufs[] = {dir->d_dids, dir->d_did_off, dir->d_slots, dir->d_rank, dir->d_order, dir->d_pks, dir->d_kind, dir->d_icols, dir->d_icol_off,
+                    dir->d_rlen, dir->d_dlen, dir->d_side_off, dir->d_side};
     for (void* p : bufs) if (p) cudaFree(p);
     delete dir;
 }
@@ -2014,6 +2025,166 @@ int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
             base += bytes;
             return AFC_OK;
         });
+    });
+}
+
+// ---------------------------------------------------------------------------------- DID resolution and DID documents
+static launch::DresDir dres_dir(const afc_did_directory* dir) {
+    launch::DresDir D{};
+    D.dids = dir->d_dids; D.did_off = dir->d_did_off; D.slots = dir->d_slots; D.mask = dir->slot_mask; D.n = dir->n;
+    D.kind = dir->d_kind; D.icols = dir->d_icols; D.icol_off = dir->d_icol_off;
+    D.rlen = dir->d_rlen; D.dlen = dir->d_dlen; D.side_off = dir->d_side_off; D.side = dir->d_side;
+    return D;
+}
+
+int afc_did_directory_set_identities(afc_did_directory* dir, const uint8_t* kinds, const uint8_t* cols, const uint64_t* col_off) {
+    if (!dir || !kinds || !col_off || dir->has_ids) return AFC_EINVAL;
+    afc_ctx* ctx = dir->ctx;
+    const uint32_t n = dir->n;
+    const size_t words = 3 * (size_t)n;
+    for (uint32_t k = 0; k < n; k++) if (kinds[k] > AFC_DID_KIND_SKILL) return AFC_EINVAL;
+    for (size_t k = 0; k < words; k++) if (col_off[k + 1] < col_off[k]) return AFC_EINVAL;
+    const uint64_t base = col_off[0], total = col_off[words] - base;
+    if (total && !cols) return AFC_EINVAL;
+    std::vector<uint64_t> off(words + 1);
+    for (size_t k = 0; k <= words; k++) off[k] = col_off[k] - base;
+    CK(cudaSetDevice(ctx->device));
+    // on any failure the directory keeps no identities, and serves workflow chains as before
+    auto drop = [&](cudaError_t e) {
+        set_err(ctx, e, "afc_did_directory_set_identities");
+        void* bufs[] = {dir->d_kind, dir->d_icols, dir->d_icol_off, dir->d_rlen, dir->d_dlen, dir->d_side_off, dir->d_side};
+        for (void* p : bufs) if (p) cudaFree(p);
+        dir->d_kind = dir->d_icols = dir->d_side = nullptr; dir->d_icol_off = dir->d_side_off = nullptr; dir->d_rlen = dir->d_dlen = nullptr;
+        return e == cudaErrorMemoryAllocation ? AFC_ENOMEM : AFC_ECUDA;
+    };
+    cudaError_t e = cudaMalloc((void**)&dir->d_kind, (size_t)n + 16);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_icols, total + 64);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_icol_off, (words + 1) * 8);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_rlen, (size_t)n * 4 + 16);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_dlen, (size_t)n * 4 + 16);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_side_off, ((size_t)n + 1) * 8);
+    if (e == cudaSuccess && n) e = cudaMemcpy(dir->d_kind, kinds, n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && total) e = cudaMemcpy(dir->d_icols, cols + base, total, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dir->d_icol_off, off.data(), (words + 1) * 8, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return drop(e);
+    // the jv_emit tapes (afc_didresolve.cuh: jwk.len / 2 + 1 entries per entry), the largest body and the scan's scratch
+    const size_t tape_bytes = vc_align((total / 2 + n + 1) * 4), scan_bytes = launch::json_scan_scratch_bytes(n);
+    uint8_t* scratch = nullptr;
+    if ((e = cudaMalloc((void**)&scratch, tape_bytes + 256 + scan_bytes)) != cudaSuccess) return drop(e);
+    uint32_t* tape = (uint32_t*)scratch;
+    uint32_t* d_largest = (uint32_t*)(scratch + tape_bytes);
+    uint64_t* scan = (uint64_t*)(scratch + tape_bytes + 256);     // 256-aligned, as the scan's words need
+    uint64_t side_total = 0;
+    launch::DresDir D = dres_dir(dir);
+    {
+        CallLog lc(ctx);
+        e = cudaMemset(d_largest, 0, 4);
+        if (e == cudaSuccess) e = launch::dres_entries(D, tape, d_largest, nullptr, lc);
+        if (e == cudaSuccess) e = launch::offsets_from_lengths(dir->d_side_off, n, scan, nullptr, lc);
+        if (e == cudaSuccess) e = cudaMemcpy(&dir->largest, d_largest, 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(&side_total, dir->d_side_off + n, 8, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMalloc((void**)&dir->d_side, side_total + 64);
+        D.side = dir->d_side;
+        if (e == cudaSuccess) e = launch::dres_canon(D, tape, nullptr, lc);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    }
+    cudaFree(scratch);
+    if (e != cudaSuccess) return drop(e);
+    dir->has_ids = true;
+    return AFC_OK;
+}
+
+// Per request: the directory's largest body or a 404 document's constant text, whichever is larger, plus at most 6 bytes per request
+// byte (the 404 document's escaped details)
+static uint64_t dres_bound(const afc_did_directory* dir, uint32_t n, uint64_t req_bytes) {
+    const uint64_t per = std::max<uint64_t>(dir->largest, launch::dres_request_fixed());
+    return (uint64_t)n * per + 6 * req_bytes;
+}
+uint64_t afc_did_resolve_bound(const afc_did_directory* dir, const uint64_t* req_off, uint32_t n) {
+    if (!dir || !dir->has_ids || !req_off || n == 0) return 0;
+    return dres_bound(dir, n, span(req_off[0], req_off[n]));
+}
+
+static int dres_check(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n,
+                      const uint8_t* bodies, const uint64_t* body_off, const uint8_t* state) {
+    if (!ctx || !dir || dir->ctx != ctx || !dir->has_ids || !req_off || !body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!kinds || !reqs || !bodies || !state) return AFC_EINVAL;
+    return AFC_OK;
+}
+
+int afc_did_resolve_batch_dev(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* d_kinds, const uint8_t* d_reqs, const uint64_t* d_req_off,
+                              uint32_t n, uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream) {
+    RC(dres_check(ctx, dir, d_kinds, d_reqs, d_req_off, n, d_bodies, d_body_off, d_state));
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[3];                       // req_off[0], req_off[n] and the offsets' flags: gathered on the device, read once
+    {
+        uint64_t* d_ends = nullptr;
+        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
+        cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
+        if (e == cudaSuccess) e = launch::dres_ends(d_req_off, n, d_ends, st, lc);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(d_ends, st);
+        CK(e);
+        CK(cudaStreamSynchronize(st));
+    }
+    if (ends[2] || bodies_cap < dres_bound(dir, n, ends[1] - ends[0])) return AFC_EINVAL;
+    const launch::DresDir D = dres_dir(dir);
+    uint32_t* ent = nullptr;
+    uint64_t* scan = nullptr;
+    uint8_t* scratch = nullptr;
+    CK(pool_carve(&scratch, st, [&](Carve& k) {
+        ent = k.take<uint32_t>(n);
+        scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
+    }));
+    cudaError_t e = launch::dres_probe(D, d_kinds, d_reqs, d_req_off, n, d_state, ent, d_body_off, scan, st, lc);
+    if (e == cudaSuccess) e = launch::dres_emit(D, d_kinds, d_reqs, d_req_off, n, d_state, ent, d_body_off, d_bodies, st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n,
+                          uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off, uint8_t* state) {
+    RC(dres_check(ctx, dir, kinds, reqs, req_off, n, bodies, body_off, state));
+    if (n == 0) { body_off[0] = 0; return AFC_OK; }
+    uint64_t bad = 0;
+    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(req_off[i + 1] < req_off[i] || req_off[i + 1] - req_off[i] > 0x7fffffffull);   // 2^31 bytes
+    if (bad || bodies_cap < afc_did_resolve_bound(dir, req_off, n)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    const launch::DresDir D = dres_dir(dir);
+    const uint64_t per = dres_bound(dir, 1, 0);
+    // chunks of whole requests, sized by what they stage and the most their bodies can take
+    auto measure = [&](uint32_t i0, uint32_t i) { return 7 * (req_off[i + 1] - req_off[i0]) + per * ((uint64_t)i - i0 + 1); };
+    uint64_t base = 0;
+    Ring ring(ctx);
+    return ring.walk(n, measure, [&](Ring& r) {
+        const uint32_t i0 = r.i0, cnt = r.cnt;
+        const uint64_t bbound = dres_bound(dir, cnt, req_off[i0 + cnt] - req_off[i0]);
+        Msgs m;
+        const uint8_t* d_kinds;
+        uint8_t *d_bodies, *d_state;
+        uint64_t *d_off, *scan;
+        uint32_t* ent;
+        RC(r.stage([&](Stager& k) {
+            m = stage_msgs(k, reqs, req_off, i0, cnt);
+            d_kinds = k.in(kinds, i0, cnt);
+            d_bodies = k.take(bbound + 64);
+            d_off = k.take<uint64_t>((size_t)cnt + 1);
+            d_state = k.take(cnt);
+            ent = k.take<uint32_t>(cnt);
+            scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(cnt));
+        }));
+        CK(launch::dres_probe(D, d_kinds, m.d, m.off, cnt, d_state, ent, d_off, scan, r.st, r.lc));
+        uint64_t bytes;
+        RC(r.read(&bytes, {d_off + cnt}));
+        CK(launch::dres_emit(D, d_kinds, m.d, m.off, cnt, d_state, ent, d_off, d_bodies, r.st, r.lc));
+        RC(r.copy_back({offsets_out(body_off, i0, d_off, (size_t)cnt + 1, base), {state, i0, d_state, cnt}, {bodies, base, d_bodies, bytes}}));
+        base += bytes;
+        return AFC_OK;
     });
 }
 

@@ -693,6 +693,73 @@ class DIDDirectory:
                    self.ctx.handle)
         self.handle = h
 
+    @staticmethod
+    def _b(v):
+        return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+
+    def set_identities(self, kinds, paths, function_names, jwks):
+        """afc_did_directory_set_identities: per DID, in the directory's order, its kind (_abi.DID_KIND_*), derivation path, function name
+        and stored public JWK text (str or bytes).  Once per directory."""
+        n = len(self.dids)
+        if not len(kinds) == len(paths) == len(function_names) == len(jwks) == n:
+            raise ValueError("one kind, path, function name and JWK per DID")
+        cols = []
+        for p, f, j in zip(paths, function_names, jwks):
+            cols += [self._b(p), self._b(f), self._b(j)]
+        buf, off = pack(cols)
+        k = np.array(list(kinds) + [0], dtype=np.uint8)
+        _abi.check(self._lib.afc_did_directory_set_identities(self.handle, _abi.ptr(k), _abi.ptr(buf), _abi.ptr(off)), self.ctx.handle)
+
+    @classmethod
+    def pack_requests(cls, requests):
+        """[(kind, did)] (kind _abi.DIDRES_RESOLVE or _DOCUMENT; did str or bytes) -> (kinds uint8, reqs, req_off)."""
+        reqs, req_off = pack([cls._b(d) for _, d in requests])
+        return np.array([k for k, _ in requests] + [0], dtype=np.uint8), reqs, req_off
+
+    def _bound(self, n, req_bytes):
+        """afc_did_resolve_bound for n requests of req_bytes bytes: it is linear in both, read off the library with one-request arrays."""
+        per = self._lib.afc_did_resolve_bound(self.handle, _abi.ptr(np.zeros(2, dtype=np.uint64)), 1)
+        per_byte = self._lib.afc_did_resolve_bound(self.handle, _abi.ptr(np.array([0, 1], dtype=np.uint64)), 1) - per
+        return n * per + per_byte * req_bytes if n else 0
+
+    def resolve_packed(self, kinds, reqs, req_off):
+        """afc_did_resolve_batch on host arrays (pack_requests).  Returns (bodies uint8, body_off uint64 [n+1], state uint8 [n])."""
+        n = len(req_off) - 1
+        cap = self._lib.afc_did_resolve_bound(self.handle, _abi.ptr(req_off), n)
+        bodies = np.empty(max(cap, 1), dtype=np.uint8)
+        body_off = np.zeros(n + 1, dtype=np.uint64)
+        state = np.empty(max(n, 1), dtype=np.uint8)
+        _abi.check(self._lib.afc_did_resolve_batch(self.ctx.handle, self.handle, _abi.ptr(kinds), _abi.ptr(reqs), _abi.ptr(req_off), n,
+                                                   _abi.ptr(bodies), cap, _abi.ptr(body_off), _abi.ptr(state)), self.ctx.handle)
+        return bodies[:int(body_off[n])], body_off, state[:n]
+
+    def resolve_dev(self, d_kinds, d_reqs, d_req_off, n, stream=None):
+        """afc_did_resolve_batch_dev on device tensors (kinds uint8, request bytes uint8, offsets int64 [n+1]).  Returns (d_bodies uint8,
+        d_body_off int64 [n+1], d_state uint8 [n])."""
+        import torch
+        dev = d_req_off.device
+        cap = 0
+        if n:
+            a, b = (int(x) for x in torch.cat([d_req_off[0:1], d_req_off[n:n + 1]]).cpu().tolist())
+            cap = self._bound(n, max(b - a, 0))
+        d_bodies = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        d_body_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_state = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        _abi.check(self._lib.afc_did_resolve_batch_dev(self.ctx.handle, self.handle, _abi.ptr(d_kinds), _abi.ptr(d_reqs), _abi.ptr(d_req_off), n,
+                                                       _abi.ptr(d_bodies), cap, _abi.ptr(d_body_off), _abi.ptr(d_state), self.ctx._stream(stream)),
+                   self.ctx.handle)
+        total = int(d_body_off[n]) if n else 0
+        return d_bodies[:total], d_body_off, d_state[:n]
+
+    def resolve(self, requests):
+        """Both DID handlers for many requests in one host-buffer call: [(state, body bytes)] in request order (an AFC_DIDRES_HOST request
+        has an empty body)."""
+        if not requests:
+            return []
+        bodies, off, state = self.resolve_packed(*self.pack_requests(requests))
+        buf = bodies.tobytes()
+        return [(int(state[i]), buf[int(off[i]):int(off[i + 1])]) for i in range(len(requests))]
+
     def close(self):
         if getattr(self, "handle", None):
             self._lib.afc_did_directory_free(self.handle)

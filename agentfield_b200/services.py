@@ -778,7 +778,69 @@ def workflow_chain_body(w, wvc, keys) -> bytes:
     return ("{" + ",".join(top) + "}").encode("utf-8", "surrogateescape")
 
 
-_GO_SPACE = "\t\n\v\f\r \x85\xa0\u1680\u2000\u2001\u2002\u2003\u2004\u2005\u2006\u2007\u2008\u2009\u200a\u2028\u2029\u202f\u205f\u3000"
+_DID_COMPONENT_TYPES = ("agentfield_server", "agent", "reasoner", "skill")     # by _abi.DID_KIND_*
+
+
+def _did_bytes(v):
+    return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
+
+
+def resolve_body(did, identity):
+    """GET /api/v1/did/resolve/:did on the host (did_handlers.go:73-94): (HTTP status, body).  identity: what ResolveDID returns for did —
+    {"kind" (_abi.DID_KIND_*), "derivation_path", "function_name", "public_key_jwk"} — or None when it finds nothing."""
+    S = lambda v: go_json.string_bytes(_did_bytes(v))
+    did = _did_bytes(did)
+    if not did:
+        return 400, b'{"error":"DID parameter is required"}'
+    if identity is None:
+        return 404, b'{"error":"DID not found"}'
+    body = ('{"component_type":"%s","derivation_path":%s,"did":%s,"function_name":%s,"public_key_jwk":%s}'
+            % (_DID_COMPONENT_TYPES[identity["kind"]], S(identity["derivation_path"]), S(did), S(identity["function_name"]),
+               S(identity["public_key_jwk"])))
+    return 200, body.encode()
+
+
+def _go_unmarshal_jwk(raw: bytes):
+    """json.Unmarshal(raw, &map[string]interface{}): the value (a dict, or None for null), or ValueError with Go's message for a value of
+    another type and for truncated text; other syntax errors carry Python's wording."""
+    v = go_json.decode_execution_payload(raw) if raw.strip(b" \t\r\n") else raw
+    if isinstance(v, (bytes, bytearray)):                       # rejected: a syntax error, or a number outside float64's range
+        try:
+            json.loads(go_json.go_utf8(raw))
+        except ValueError as ex:
+            if getattr(ex, "pos", 0) >= len(raw.rstrip(b" \t\r\n")):
+                raise ValueError("unexpected end of JSON input")
+            raise ValueError(str(ex))
+        raise ValueError("json: cannot unmarshal number into Go value of type float64")
+    if v is None or isinstance(v, dict):
+        return v
+    kind = "array" if isinstance(v, list) else "string" if isinstance(v, str) else "bool" if isinstance(v, bool) else "number"
+    raise ValueError("json: cannot unmarshal %s into Go value of type map[string]interface {}" % kind)
+
+
+def document_body(did, identity):
+    """GET /api/v1/did/document/:did on the host (did_handlers.go:368-429): (HTTP status, body), identity as for resolve_body.  The stored
+    JWK goes through json.Unmarshal into map[string]interface{} and back; a text Go rejects is a 500."""
+    S = lambda v: go_json.string_bytes(_did_bytes(v))
+    did = _did_bytes(did)
+    if not did:
+        return 400, b'{"error":"DID parameter is required"}'
+    if identity is None:
+        return 404, ('{"details":%s,"error":"DID not found"}' % S(b"DID not found: " + did)).encode()
+    try:
+        jwk = _go_unmarshal_jwk(_did_bytes(identity["public_key_jwk"]))
+    except ValueError as ex:
+        return 500, ('{"details":%s,"error":"Failed to parse public key"}' % S(str(ex))).encode()
+    d, key = S(did), S(did + b"#key-1")
+    body = ('{"@context":["https://www.w3.org/ns/did/v1","https://w3id.org/security/suites/ed25519-2020/v1"],"assertionMethod":[%s],'
+            '"authentication":[%s],"id":%s,"service":[{"description":"AgentField Agent Platform Service","id":%s,'
+            '"serviceEndpoint":"https://agentfield.example.com/api/v1","type":"AgentFieldAgentService"}],"verificationMethod":[{"controller":%s,'
+            '"id":%s,"publicKeyJwk":%s,"type":"Ed25519VerificationKey2020"}]}'
+            % (key, key, d, S(did + b"#agentfield-service"), d, key, go_json.value(jwk)))
+    return 200, body.encode("utf-8", "surrogatepass")
+
+
+_GO_SPACE ="\t\n\v\f\r \x85\xa0\u1680\u2000\u2001\u2002\u2003\u2004\u2005\u2006\u2007\u2008\u2009\u200a\u2028\u2029\u202f\u205f\u3000"
 
 
 def _issue(kind, severity, component, description, field="", expected="", actual=""):
@@ -994,12 +1056,14 @@ class DIDService:
         # node id (bytes) -> {"did", "derivation_path", "public_key_jwk", "reasoners": {id: component}, "skills": {id: component}}, a
         # component being {"did", "derivation_path", "public_key_jwk", "function_name"}: what the existing identity package needs
         self.agent_nodes = {}
+        self._resolver = None             # serve_did_requests: (DIDDirectory with identities, DID bytes -> identity)
 
     @staticmethod
     def _node_key(v):
         return v.encode("utf-8", "surrogatepass") if isinstance(v, str) else bytes(v)
 
     def _register(self, requests):
+        self._resolver = None                                     # serve_did_requests rebuilds its directory
         results = self.keys.register(self.master_seed, self.server_id, requests, len(self.agent_nodes))
         for r, res in zip(requests, results):
             comps = res["components"]
@@ -1046,21 +1110,60 @@ class DIDService:
             self._root_did = self.keys.derive(self.master_seed, [self.ROOT_PATH])[0]
         return self._root_did
 
-    def did_directory(self, ctx=None):
-        """The registry's public half on the device (identity.DIDDirectory): every DID ResolveDID resolves (did_service.go:368-473) with
-        its public key — the root DID (the key at m/44'/0'), then every agent's and component's DID with the key its stored public JWK
-        holds (the JWK's x).  A DID the registry holds twice (re-registration gives every new component of one kind the same DID) is
-        taken once: its key is the same."""
-        from .identity import DIDDirectory
-        keys = {self.root_did: self.keys.public_key(self.root_did)}
+    def _identities(self):
+        """Every DID ResolveDID resolves (did_service.go:368-473), each once, in registration order — the root DID, then each agent, its
+        reasoners and its skills in insertion order — as DID -> {"pk", "kind", "derivation_path", "function_name", "public_key_jwk"}.  A DID
+        the registry holds twice (re-registration gives every new component of one kind the same DID) keeps its first holder: Go's
+        randomised map iteration may return any of them, and they differ only in function_name."""
+        root_pk = self.keys.public_key(self.root_did)
+        out = {self.root_did: {"pk": root_pk, "kind": _abi.DID_KIND_SERVER, "derivation_path": self.ROOT_PATH, "function_name": b"",
+                               "public_key_jwk": public_jwk(root_pk)}}
         for a in self.agent_nodes.values():
-            for e in [a] + list(a["reasoners"].values()) + list(a["skills"].values()):
-                if e["did"] not in keys:
+            comps = [(a, _abi.DID_KIND_AGENT)] + [(c, _abi.DID_KIND_REASONER) for c in a["reasoners"].values()] + \
+                    [(c, _abi.DID_KIND_SKILL) for c in a["skills"].values()]
+            for e, kind in comps:
+                if e["did"] not in out:
                     x = json.loads(e["public_key_jwk"])["x"]
-                    keys[e["did"]] = base64.urlsafe_b64decode(x + "=" * (-len(x) % 4))
-        return DIDDirectory(list(keys), list(keys.values()), ctx=ctx or self.keys.ctx)
+                    out[e["did"]] = {"pk": base64.urlsafe_b64decode(x + "=" * (-len(x) % 4)), "kind": kind, "derivation_path": e["derivation_path"],
+                                     "function_name": e.get("function_name", b""), "public_key_jwk": e["public_key_jwk"]}
+        return out
+
+    def did_directory(self, ctx=None, identities=False):
+        """The registry's public half on the device (identity.DIDDirectory): every DID ResolveDID resolves with its public key — the root
+        DID (the key at m/44'/0'), then every agent's and component's DID with the key its stored public JWK holds (the JWK's x), each
+        once (_identities).  With `identities` the directory also holds what DID resolution and DID documents need (set_identities)."""
+        return self._directory(self._identities(), ctx, identities)
+
+    def _directory(self, ids, ctx=None, identities=False):
+        from .identity import DIDDirectory
+        d = DIDDirectory(list(ids), [e["pk"] for e in ids.values()], ctx=ctx or self.keys.ctx)
+        if identities:
+            d.set_identities(*[[e[k] for e in ids.values()] for k in ("kind", "derivation_path", "function_name", "public_key_jwk")])
+        return d
+
+    def serve_did_requests(self, requests):
+        """GET /api/v1/did/resolve/:did and GET /api/v1/did/document/:did for many requests, [(kind, did)] with kind _abi.DIDRES_RESOLVE or
+        _DOCUMENT, in one device call (identity.DIDDirectory.resolve) over a directory with identities, rebuilt after a registration.
+        Returns [(HTTP status, body)] in request order; requests the device leaves to the host go through resolve_body / document_body."""
+        for kind, _ in requests:
+            if kind not in (_abi.DIDRES_RESOLVE, _abi.DIDRES_DOCUMENT):
+                raise ValueError("unknown request kind %r" % kind)
+        if self._resolver is None:
+            ids = self._identities()
+            self._resolver = (self._directory(ids, identities=True), {_did_bytes(k): v for k, v in ids.items()})
+        directory, index = self._resolver
+        status = {_abi.DIDRES_FOUND: 200, _abi.DIDRES_NOT_FOUND: 404, _abi.DIDRES_BAD_REQUEST: 400}
+        out = []
+        for (kind, did), (st, body) in zip(requests, directory.resolve(requests) if requests else []):
+            if st == _abi.DIDRES_HOST:
+                host = resolve_body if kind == _abi.DIDRES_RESOLVE else document_body
+                out.append(host(did, index.get(_did_bytes(did))))
+            else:
+                out.append((status[st], body))
+        return out
 
     def _reregister(self, requests):
+        self._resolver = None
         reqs = []
         for r in requests:
             a = self.agent_nodes[self._node_key(r["agent_node_id"])]

@@ -463,6 +463,51 @@ int afc_vc_workflow_chain_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
                                     const int64_t* d_doc_size, const int32_t* d_created_off, const afc_did_directory* dir, uint32_t n,
                                     uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream);
 
+/* ---- N1: DIDs resolved and W3C DID documents served in one call: DIDService.ResolveDID (internal/services/did_service.go:368-473) and
+ * the c.JSON of GET /api/v1/did/resolve/:did and GET /api/v1/did/document/:did (internal/handlers/did_handlers.go:73-94, 368-429), for n
+ * requests against a directory.  The handlers' registry checks (DID system disabled, no server registry) stay with the caller.
+ * afc_did_directory_set_identities gives each directory DID, in the order given to afc_did_directory_new, its kind (AFC_DID_KIND_*) and
+ * three byte strings: derivation_path, function_name, public_key_jwk (the stored JWK text; for the root, ed25519PublicKeyToJWK's text of
+ * its key); cols / col_off: 3n + 1 absolute offsets, DID k's strings at col_off[3k .. 3k + 3].  One pass on the device computes each
+ * entry's two body lengths, or HOST, and the directory's longest body.  AFC_EINVAL: a NULL pointer, a kind above AFC_DID_KIND_SKILL,
+ * offsets that run backwards, a directory that already has identities.  A directory without identities serves
+ * afc_vc_workflow_chain_batch as before.
+ * afc_did_resolve_batch writes, for request i = (kinds[i], reqs[req_off[i] .. req_off[i+1])), bodies[body_off[i] .. body_off[i+1]): the
+ * bytes c.JSON writes (json.Marshal, HTML escaping on, map keys sorted), and state[i], which fixes the HTTP status:
+ *   AFC_DIDRES_FOUND        200.  RESOLVE: {"component_type","derivation_path","did","function_name","public_key_jwk"}, the JWK as a
+ *                           JSON string; component_type "agentfield_server", "agent", "reasoner" or "skill" from the kind.  DOCUMENT: the
+ *                           W3C DID document of did_handlers.go:398-425, publicKeyJwk the stored JWK re-marshalled through
+ *                           map[string]interface{} (keys sorted, numbers as float64, strings re-escaped; a stored null stays null).
+ *   AFC_DIDRES_NOT_FOUND    404.  {"error":"DID not found"}, or for DOCUMENT {"details":"DID not found: <the request, escaped>","error":...}.
+ *   AFC_DIDRES_BAD_REQUEST  400.  An empty DID: {"error":"DID parameter is required"}.
+ *   AFC_DIDRES_HOST         a zero-length body; the caller builds it.  A DOCUMENT whose stored JWK json.Unmarshal rejects or holds a
+ *                           value other than an object or null (a 500 in the reference), or one the device does not re-marshal (duplicate
+ *                           or escaped keys, invalid UTF-8 or lone surrogates, nesting deeper than 32, numbers outside float64's normal
+ *                           range); either kind when the found body would exceed 4096 bytes; a kind other than RESOLVE and DOCUMENT.
+ * bodies_cap must be at least afc_did_resolve_bound(dir, req_off, n), additive over requests and computed from the directory and the ends
+ * of req_off alone (else AFC_EINVAL, before any work).  Other AFC_EINVAL: a NULL pointer, a directory without identities or of another
+ * context, a request of 2^31 bytes or more, offsets that run backwards.  The host-buffer call streams chunks of whole requests through
+ * the context's staging ring; the _dev call synchronises `stream` once, to read the ends of req_off and whether any request breaks those
+ * two rules.  n = 0 writes body_off[0] = 0 in the host-buffer call and nothing in the _dev call.  No secret is involved: the call derives
+ * no key and does not rebuild the private JWK ResolveDID regenerates and both handlers discard. */
+#define AFC_DID_KIND_SERVER 0
+#define AFC_DID_KIND_AGENT 1
+#define AFC_DID_KIND_REASONER 2
+#define AFC_DID_KIND_SKILL 3
+#define AFC_DID_IDENTITY_COLUMNS 3   /* derivation_path, function_name, public_key_jwk */
+#define AFC_DIDRES_RESOLVE 0
+#define AFC_DIDRES_DOCUMENT 1
+#define AFC_DIDRES_FOUND 0
+#define AFC_DIDRES_NOT_FOUND 1
+#define AFC_DIDRES_BAD_REQUEST 2
+#define AFC_DIDRES_HOST 3
+int afc_did_directory_set_identities(afc_did_directory* dir, const uint8_t* kinds /* n */, const uint8_t* cols, const uint64_t* col_off /* 3n+1 */);
+uint64_t afc_did_resolve_bound(const afc_did_directory* dir, const uint64_t* req_off, uint32_t n);
+int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off /* n+1 */,
+                          uint32_t n, uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off /* n+1 */, uint8_t* state /* n */);
+int afc_did_resolve_batch_dev(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* d_kinds, const uint8_t* d_reqs, const uint64_t* d_req_off,
+                              uint32_t n, uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream);
+
 /* ---- W2: execution webhook deliveries built and signed in one call: determineWebhookEvent + buildPayload + json.Marshal +
  * generateWebhookSignature (internal/services/webhook_dispatcher.go:294-320, 394-474) for n deliveries.  For delivery i:
  *   bodies[body_off[i] .. body_off[i+1])   the request body json.Marshal(types.ExecutionWebhookPayload), the result member being

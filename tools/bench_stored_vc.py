@@ -9,9 +9,11 @@ issue_execution block measures execution credentials issued in one call (afc_vc_
 measures webhook deliveries built and signed in one call (afc_webhook_sign_batch[_dev]) next to HMAC alone over the same bodies.
 The issue_workflow block measures workflow credentials issued in one call (afc_vc_issue_workflow_batch[_dev]) next to the host-built path.
 The reregister block measures known agents re-registered in one call (afc_did_reregister_batch[_dev]) in a restart storm.
+The resolve block measures DID resolution and DID documents served in one call (afc_did_resolve_batch[_dev]) from a 2^20-DID directory.
 Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -845,13 +847,92 @@ def chain_block(ctx, dev, timed):
                             "note": "issue_workflow_vc_batch + workflow_chain_body; created_at at whole seconds"}}
 
 
+def resolve_block(ctx, dev, timed):
+    """DIDs resolved and DID documents served on the device (afc_did_resolve_batch): a directory of 2^20 + 1 DIDs (the root and 2^14 agents
+    with 63 components each), every 100th stored JWK in a non-canonical spelling; 2^20 requests, half resolve and half document, 5 %
+    unknown DIDs.  Reported: the attach time (afc_did_directory_set_identities, host clock around the synchronous call), the _dev call
+    with its per-kernel split, the bytes it writes over its time against the H100 SXM's 3.35 TB/s, the host-buffer call from pinned
+    buffers, and the host mirror (services.resolve_body / document_body) on 2000 requests."""
+    import base64
+    import torch
+    from agentfield_b200 import _abi, services
+    from agentfield_b200.identity import DIDDirectory, public_jwk
+    A, C_, n = 1 << 14, 63, 1 << 20
+    rng = np.random.default_rng(0xD1DD)
+    did = lambda pk: b"did:key:z" + base64.urlsafe_b64encode(b"\xed\x01" + pk).rstrip(b"=")
+    dids, pks, kinds, paths, fns, jwks = [], [], [], [], [], []
+    for k in range(A * (C_ + 1) + 1):
+        pk = k.to_bytes(32, "little")
+        a, j = (k - 1) // (C_ + 1), (k - 1) % (C_ + 1)
+        kind = _abi.DID_KIND_SERVER if k == 0 else _abi.DID_KIND_AGENT if j == 0 else _abi.DID_KIND_REASONER if j <= 32 else _abi.DID_KIND_SKILL
+        jwk = public_jwk(pk)
+        if k % 100 == 99:
+            jwk = b" " + jwk.replace(b",", b", ")
+        dids.append(did(pk)); pks.append(pk); kinds.append(kind); jwks.append(jwk)
+        paths.append(b"m/44'/0'" if k == 0 else b"m/44'/1234567'/%d'" % a if j == 0 else b"m/44'/1234567'/%d'/%d'/%d'" % (a, int(j > 32), j))
+        fns.append(b"" if kind in (_abi.DID_KIND_SERVER, _abi.DID_KIND_AGENT) else b"function_%d" % j)
+    directory = DIDDirectory(dids, pks, ctx=ctx)
+    t_0 = time.perf_counter()
+    directory.set_identities(kinds, paths, fns, jwks)
+    ms_attach = (time.perf_counter() - t_0) * 1e3
+    pick = rng.integers(0, len(dids), n)
+    unknown = rng.random(n) < 0.05
+    reqs = [(i & 1, b"did:key:zUnknown%07d" % i if unknown[i] else dids[int(pick[i])]) for i in range(n)]
+    kinds_a, reqs_a, off_a = directory.pack_requests(reqs)
+    d_k, d_r, d_o = torch.from_numpy(kinds_a).to(dev), torch.from_numpy(reqs_a).to(dev), torch.from_numpy(off_a.view(np.int64)).to(dev)
+    run = lambda: directory.resolve_dev(d_k, d_r, d_o, n)
+    bodies, off, state = run()
+    torch.cuda.synchronize()
+    total = int(off[n])
+    states = {name: int((state == v).sum()) for name, v in (("found", 0), ("not_found", 1), ("bad_request", 2), ("host", 3))}
+    dev_bytes = bodies.cpu().numpy().tobytes()
+    del bodies, off, state
+    ms = timed(run)
+    ctx.profile_begin()
+    timed(run, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    lib = _abi.load()
+    keep = []
+
+    def pin(a):
+        p = lib.afc_alloc_pinned(max(a.nbytes, 1))
+        h = np.frombuffer((ctypes.c_uint8 * max(a.nbytes, 1)).from_address(p), dtype=np.uint8)[:a.nbytes].view(a.dtype)
+        h[...] = a
+        keep.append(p)
+        return h
+    pk_, pr_, po_ = pin(kinds_a), pin(reqs_a), pin(off_a)
+    hb, _, _ = directory.resolve_packed(pk_, pr_, po_)
+    host_same = hb.tobytes() == dev_bytes
+    del hb, dev_bytes
+    t_0 = time.perf_counter()
+    for _ in range(3):
+        directory.resolve_packed(pk_, pr_, po_)
+    ms_host = (time.perf_counter() - t_0) / 3 * 1e3
+    for p in keep:
+        lib.afc_free_pinned(p)
+    index = {d: {"kind": k, "derivation_path": p, "function_name": f, "public_key_jwk": j} for d, k, p, f, j in zip(dids, kinds, paths, fns, jwks)}
+    sample = [reqs[int(i)] for i in rng.choice(n, 2000, replace=False)]
+    t_0 = time.perf_counter()
+    for k, d in sample:
+        (services.resolve_body if k == 0 else services.document_body)(d, index.get(d))
+    ms_mirror = (time.perf_counter() - t_0) * 1e3
+    directory.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "directory": {"dids": len(dids), "attach_ms": ms_attach},
+            "dev_call": {"requests": n, "states": states, "body_bytes": total, "ms": ms, "requests_per_s": n / (ms * 1e-3),
+                         "bytes_per_s": total / (ms * 1e-3), "share_of_3_35_TBps": total / (ms * 1e-3) / 3.35e12, "kernels_ms": kms},
+            "host_call": {"ms": ms_host, "requests_per_s": n / (ms_host * 1e-3), "same_as_dev": bool(host_same), "note": "pinned buffers"},
+            "host_mirror": {"requests": len(sample), "ms": ms_mirror, "requests_per_s": len(sample) / (ms_mirror * 1e-3)}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register",
-                                        "reregister", "chain"],
+                                        "reregister", "chain", "resolve"],
                     default=None,
                     help="run one block")
     args = ap.parse_args()
@@ -868,7 +949,7 @@ def main():
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
               "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block,
-              "reregister": reregister_block, "chain": chain_block}
+              "reregister": reregister_block, "chain": chain_block, "resolve": resolve_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
