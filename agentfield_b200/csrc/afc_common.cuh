@@ -148,6 +148,20 @@ AFC_HD void ldg_nc_32B(uint32_t* v, const uint32_t* p) {
 }
 #endif
 
+// The ends of a batch's offset arrays, which bound everything a call writes.  Span j writes out[2 j] = off[stride lo] and
+// out[2 j + 1] = off[stride hi]: (lo, hi) = (0, n) when via < 0, else the two words span `via` (an earlier one) wrote, for an array indexed
+// by those words.  A backwards (lo, hi) reads nothing and writes 0 for both words.  Run by one thread of k_offset_ends on the device
+// arrays of a _dev call and on the host arrays by the afc_*_bound functions, so that both read the same words.
+struct OffsetSpan { const uint64_t* off; uint32_t stride; int32_t via; };
+AFC_HHD void offset_ends(const OffsetSpan* s, int k, uint32_t n, uint64_t* out) {
+    for (int j = 0; j < k; j++) {
+        const uint64_t lo = s[j].via < 0 ? 0 : out[2 * s[j].via], hi = s[j].via < 0 ? n : out[2 * s[j].via + 1];
+        const bool ok = hi >= lo;
+        out[2 * j] = ok ? s[j].off[s[j].stride * lo] : 0;
+        out[2 * j + 1] = ok ? s[j].off[s[j].stride * hi] : 0;
+    }
+}
+
 AFC_HD void store_be32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; }
 AFC_HD uint32_t load_le32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 AFC_HD void store_le32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }

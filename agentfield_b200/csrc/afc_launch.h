@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "afc_common.cuh"
+
 namespace afc {
 namespace launch {
 
@@ -67,6 +69,9 @@ cudaError_t json_fill(const uint8_t* segs, const uint32_t* seg_off, const uint8_
                       const uint64_t* field_off, uint32_t n, const uint64_t* out_off, uint8_t* out, cudaStream_t s, LaunchLog* lg);
 // n lengths in out_off[1..n] -> n+1 offsets (out_off[0] = 0); scan_scratch: json_scan_scratch_bytes(n)
 cudaError_t offsets_from_lengths(uint64_t* out_off, uint32_t n, uint64_t* scan_scratch, cudaStream_t s, LaunchLog* lg);
+// The spans of a call's offset arrays (offset_ends, afc_common.cuh); out: their 2 k ends, gathered by one thread
+struct OffsetSpans { OffsetSpan s[5]; int k; };
+cudaError_t offset_ends(const OffsetSpans& S, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
 cudaError_t b64url_encode(const uint8_t* in, uint32_t item, uint32_t n, uint8_t* out, cudaStream_t s, LaunchLog* lg);
 cudaError_t hex_encode(const uint8_t* in, uint64_t total, uint8_t* out, cudaStream_t s, LaunchLog* lg);
 cudaError_t microbench_hash(int which, uint32_t iters, uint32_t blocks, uint32_t threads, uint32_t* sink, cudaStream_t s, LaunchLog* lg);
@@ -134,9 +139,6 @@ uint64_t wh_fixed_bytes();             // the constant text a body can hold at m
 // rec_off: n + 1 absolute record indices; rec_col_off (2 per record + 1) and created_at (2 per record) are indexed by absolute record;
 // the batch's m = rec_off[n] - rec_off[0] records have per-record scratch cls (m bytes) and id lengths / offsets (m + 1 entries);
 // arr: 2 per workflow (where its componentVcIds array starts, its length)
-// out: col_off[0], col_off[7 n], rec_off[0], rec_off[n], rec_col_off[2 rec_off[0]], rec_col_off[2 rec_off[n]] (one thread)
-cudaError_t vcw_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s,
-                     LaunchLog* lg);
 // each record's class and escaped-id length (write them to id_off + 1 for offsets_from_lengths)
 cudaError_t vcw_records(const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created_at, const uint64_t* rec_off, uint32_t m,
                         uint8_t* cls, uint64_t* id_len, cudaStream_t s, LaunchLog* lg);
@@ -179,9 +181,6 @@ struct VccArgs {
     uint64_t* rlen; uint32_t* rank; uint32_t* dlist; uint64_t* elen; uint32_t* hset; uint32_t* host; uint32_t* ndist; uint64_t* lay; uint64_t* scan;
 };
 size_t vcc_lay_words();
-// out: the six ends of vcw_ends, chain_col_off[0], chain_col_off[2 n], chain_rec_col_off at 13 rec_off[0] and 13 rec_off[n] (one thread)
-cudaError_t vcc_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
-                     const uint64_t* chain_rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
 // after the workflow-credential passes: states, body offsets (complete when this has run) and the layout; then the bodies
 cudaError_t vcc_sizes(const VccArgs& A, cudaStream_t s, LaunchLog* lg);
 cudaError_t vcc_emit(const VccArgs& A, cudaStream_t s, LaunchLog* lg);
@@ -229,9 +228,6 @@ struct DidrArgs {
     uint32_t* list; uint8_t* flags; uint64_t* esc; uint64_t* nz; uint32_t* rank; uint64_t* before; uint64_t* map_bytes; uint32_t* map_cnt;
     uint8_t* seeds; uint64_t* scan;
 };
-// out: node_off[0], node_off[n], id_idx[0], id_idx[2n], id_off at both (one thread)
-cudaError_t didr_ends(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t* out, cudaStream_t s,
-                      LaunchLog* lg);
 // every pass; the seeds scratch holds the derived seeds when it has run (the caller wipes it)
 cudaError_t didr_register(const DidrArgs& A, cudaStream_t s, LaunchLog* lg);
 uint64_t didr_req_fixed();             // the body bound's constant per request and per id (afc_didreg.cuh)
@@ -259,9 +255,6 @@ struct DidrrArgs {
     uint8_t* rflags; uint64_t* ebytes; uint8_t* iflags; uint64_t* esc; uint32_t* rank; uint64_t* before; uint32_t* bad; uint64_t* agent_bytes;
     uint64_t* map_bytes; uint32_t* map_cnt; uint8_t* seeds; uint64_t* scan;
 };
-// out: agent_col_off at 0 and 3n, id_idx at 0 and 2n, id_off at both, reg_idx at 0 and 2n, reg_col_off at five times both (one thread)
-cudaError_t didrr_ends(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx, const uint64_t* reg_col_off,
-                       uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg);
 // every pass; the seeds scratch holds the derived seeds when it has run (the caller wipes it)
 cudaError_t didrr_reregister(const DidrrArgs& A, cudaStream_t s, LaunchLog* lg);
 uint64_t didrr_req_fixed();            // the body bound's constant per request and per registered component (afc_didrereg.cuh)

@@ -424,12 +424,47 @@ cudaError_t vc_stored_enqueue(afc_ctx* ctx, const afc_keyset* ks, int kind, cons
     return e;
 }
 
-// offsets must be non-decreasing: a caller's slip would otherwise turn into an out-of-bounds copy from its own buffer
+// offsets must be non-decreasing: a caller's slip would otherwise turn into an out-of-bounds copy from its own buffer.  off[first ..
+// last] is the part of an array indexed by absolute item that a batch uses.
 template <class T>
-bool monotone(const T* off, uint32_t n) {
+bool monotone(const T* off, uint64_t first, uint64_t last) {
     T bad = 0;
-    for (uint32_t i = 0; i < n; i++) bad |= (T)(off[i + 1] < off[i]);
+    for (uint64_t k = first; k < last; k++) bad |= (T)(off[k + 1] < off[k]);
     return bad == 0;
+}
+template <class T>
+bool monotone(const T* off, uint64_t n) { return monotone(off, 0, n); }
+
+// the byte or item count between two ends, 0 for a backwards range
+uint64_t span(uint64_t a, uint64_t b) { return b >= a ? b - a : 0; }
+
+// Runs enq(d_ends) on the stream into `words` words of device scratch, copies them to ends and synchronises once
+template <class F>
+int gather_ends(afc_ctx* ctx, uint64_t* ends, size_t words, cudaStream_t st, F&& enq) {
+    uint64_t* d_ends = nullptr;
+    CK(cudaMallocAsync((void**)&d_ends, words * 8, st));
+    cudaError_t e = enq(d_ends);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, words * 8, cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(d_ends, st);
+    CK(e);
+    CK(cudaStreamSynchronize(st));
+    return AFC_OK;
+}
+// The ends of a _dev call's offset arrays (offset_ends), read with one synchronisation: each word of a call with direct spans only is
+// copied as it is; a call with an indirect span, whose indices are device words too, gathers them with one thread of k_offset_ends.
+int read_ends(afc_ctx* ctx, const launch::OffsetSpans& S, uint32_t n, uint64_t* ends, cudaStream_t st) {
+    bool direct = true;
+    for (int j = 0; j < S.k; j++) direct = direct && S.s[j].via < 0;
+    if (!direct) {
+        CallLog lc(ctx);
+        return gather_ends(ctx, ends, 2 * (size_t)S.k, st, [&](uint64_t* d_ends) { return launch::offset_ends(S, n, d_ends, st, lc); });
+    }
+    for (int j = 0; j < S.k; j++) {
+        CK(cudaMemcpyAsync(&ends[2 * j], S.s[j].off, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&ends[2 * j + 1], S.s[j].off + (size_t)S.s[j].stride * n, 8, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    return AFC_OK;
 }
 
 // AFC_CHUNK_ITEMS / AFC_MIN_CHUNK_ITEMS: tuning knobs for experiments (read once per process)
@@ -1363,6 +1398,8 @@ int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const
                                uint8_t* status, uint32_t* fields) {
     return vc_verify_host(ctx, ks, doc_kind, docs, doc_off, n, status, fields, false);
 }
+// the offset arrays whose ends bound a stored, JSON or audit call
+static launch::OffsetSpans doc_spans(const uint64_t* doc_off) { return {{{doc_off, 1, -1}}, 1}; }
 // the _dev form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
 static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n, uint8_t* d_status,
                          uint32_t* d_fields, void* stream, bool json) {
@@ -1372,10 +1409,8 @@ static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8
     CK(cudaSetDevice(ctx->device));
     CallLog lc(ctx);
     cudaStream_t st = (cudaStream_t)stream;
-    uint64_t ends[2];                       // the batch's byte size bounds the message buffer: read it once (one synchronisation)
-    CK(cudaMemcpyAsync(&ends[0], d_doc_off, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[1], d_doc_off + n, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    uint64_t ends[2];                       // the batch's byte size bounds the message buffer
+    RC(read_ends(ctx, doc_spans(d_doc_off), n, ends, st));
     if (ends[1] < ends[0]) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     VcScratch S;
@@ -1449,10 +1484,8 @@ int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, co
     CK(cudaSetDevice(ctx->device));
     CallLog lc(ctx);
     cudaStream_t st = (cudaStream_t)stream;
-    uint64_t ends[2];                       // the batch's byte size bounds the message buffer: read it once (one synchronisation)
-    CK(cudaMemcpyAsync(&ends[0], d_doc_off, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[1], d_doc_off + n, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    uint64_t ends[2];                       // the batch's byte size bounds the message buffer
+    RC(read_ends(ctx, doc_spans(d_doc_off), n, ends, st));
     if (ends[1] < ends[0]) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     VcScratch S;
@@ -1472,10 +1505,14 @@ static uint64_t issue_fixed_bytes() { return launch::vci_literal_bytes() + 4 * 4
 static uint64_t issue_doc_bound(uint32_t n, uint64_t col_bytes) { return (uint64_t)n * issue_fixed_bytes() + 18 * col_bytes; }
 static uint64_t issue_msg_bound(uint32_t n, uint64_t col_bytes) { return (uint64_t)n * issue_fixed_bytes() + 12 * col_bytes; }
 
+static launch::OffsetSpans issue_spans(const uint64_t* col_off) { return {{{col_off, AFC_ISSUE_COLUMNS, -1}}, 1}; }
+
 uint64_t afc_vc_issue_bound(const uint64_t* col_off, uint32_t n) {
     if (!col_off || n == 0) return 0;
-    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_ISSUE_COLUMNS];
-    return issue_doc_bound(n, b >= a ? b - a : 0);
+    const launch::OffsetSpans S = issue_spans(col_off);
+    uint64_t e[2];
+    offset_ends(S.s, S.k, n, e);
+    return issue_doc_bound(n, span(e[0], e[1]));
 }
 
 // per-call device scratch: signing messages and their offsets, signatures, scan tiles
@@ -1529,12 +1566,10 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
     if (!aligned16(d_expanded96)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
-    uint64_t ends[2];                       // the column bytes bound the documents: read them once (one synchronisation)
-    CK(cudaMemcpyAsync(&ends[0], d_col_off, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[1], d_col_off + (size_t)n * AFC_ISSUE_COLUMNS, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (ends[1] < ends[0] || docs_cap < issue_doc_bound(n, ends[1] - ends[0])) return AFC_EINVAL;
-    const uint64_t cb = ends[1] - ends[0];
+    uint64_t ends[2];                       // the column bytes bound the documents
+    RC(read_ends(ctx, issue_spans(d_col_off), n, ends, st));
+    const uint64_t cb = span(ends[0], ends[1]);
+    if (ends[1] < ends[0] || docs_cap < issue_doc_bound(n, cb)) return AFC_EINVAL;
     uint8_t* hashes = (flags & AFC_ISSUE_HASH_DATA) ? d_hashes : nullptr;
     {
         CallLog lc(ctx);
@@ -1560,10 +1595,9 @@ int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32
     if (n == 0) { doc_off[0] = 0; return AFC_OK; }
     const bool hash = (flags & AFC_ISSUE_HASH_DATA) != 0;
     for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
-    uint64_t bad = 0;
-    for (size_t k = 0; k < (size_t)n * AFC_ISSUE_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
-    if (hash) for (size_t k = 0; k < (size_t)2 * n; k++) bad |= (uint64_t)(payload_off[k + 1] < payload_off[k]);
-    if (bad || docs_cap < afc_vc_issue_bound(col_off, n)) return AFC_EINVAL;
+    if (!monotone(col_off, (uint64_t)n * AFC_ISSUE_COLUMNS) || (hash && !monotone(payload_off, 2 * (uint64_t)n)) ||
+        docs_cap < afc_vc_issue_bound(col_off, n))
+        return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of credentials through the ring.  A chunk's documents land at their final offsets, so its stream is synchronised once after
     // the sizes pass to learn where the chunk ends (the next chunk's copies are enqueued after that).
@@ -1624,12 +1658,17 @@ static uint64_t wf_doc_bound(uint32_t n, uint64_t col_bytes, uint64_t records, u
     return (uint64_t)n * wf_fixed_bytes() + 24 * col_bytes + 6 * rec_bytes + 3 * records;
 }
 
+// ends: col_off at 0 and 7 n, rec_off at 0 and n, rec_col_off at twice those
+static launch::OffsetSpans wf_spans(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off) {
+    return {{{col_off, AFC_WORKFLOW_COLUMNS, -1}, {rec_off, 1, -1}, {rec_col_off, 2, 1}}, 3};
+}
+
 uint64_t afc_vc_workflow_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n) {
     if (!col_off || !rec_off || !rec_col_off || n == 0) return 0;
-    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_WORKFLOW_COLUMNS], r0 = rec_off[0], r1 = rec_off[n];
-    if (r1 < r0) return wf_doc_bound(n, b >= a ? b - a : 0, 0, 0);
-    const uint64_t c = rec_col_off[2 * r0], d = rec_col_off[2 * r1];
-    return wf_doc_bound(n, b >= a ? b - a : 0, r1 - r0, d >= c ? d - c : 0);
+    const launch::OffsetSpans S = wf_spans(col_off, rec_off, rec_col_off);
+    uint64_t e[6];
+    offset_ends(S.s, S.k, n, e);
+    return wf_doc_bound(n, span(e[0], e[1]), span(e[2], e[3]), span(e[4], e[5]));
 }
 
 // per-call device scratch: signing messages and their offsets, signatures, scan tiles, record classes, record id offsets, array places
@@ -1687,20 +1726,12 @@ int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
-    uint64_t ends[6];                       // the ends of the three offset arrays bound the documents: gathered by one thread, read once
-    {
-        uint64_t* d_ends = nullptr;
-        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
-        cudaError_t e = launch::vcw_ends(d_col_off, d_rec_off, d_rec_col_off, n, d_ends, st, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
-        cudaFreeAsync(d_ends, st);
-        CK(e);
-        CK(cudaStreamSynchronize(st));
-    }
+    uint64_t ends[6];                       // the ends of the three offset arrays bound the documents
+    RC(read_ends(ctx, wf_spans(d_col_off, d_rec_off, d_rec_col_off), n, ends, st));
     if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] > 0xffffffffull) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
     if (m && (!d_rec_cols || !d_created_at)) return AFC_EINVAL;
-    const uint64_t bound = wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4]);
+    const uint64_t bound = wf_doc_bound(n, span(ends[0], ends[1]), m, span(ends[4], ends[5]));
     if (docs_cap < bound) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     WorkflowScratch S;
@@ -1721,12 +1752,9 @@ int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
     if (rc != AFC_OK) return rc;
     if (n == 0) { doc_off[0] = 0; return AFC_OK; }
     for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
-    uint64_t bad = 0;
-    for (size_t k = 0; k < (size_t)n * AFC_WORKFLOW_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
-    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(rec_off[i + 1] < rec_off[i]) | (uint64_t)(rec_off[i + 1] - rec_off[i] > 0xffffffffull);
-    if (bad) return AFC_EINVAL;
-    for (uint64_t k = 2 * rec_off[0]; k < 2 * rec_off[n]; k++) bad |= (uint64_t)(rec_col_off[k + 1] < rec_col_off[k]);
-    if (bad || docs_cap < afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n)) return AFC_EINVAL;
+    if (!monotone(col_off, (uint64_t)n * AFC_WORKFLOW_COLUMNS) || !monotone(rec_off, n)) return AFC_EINVAL;
+    for (uint32_t i = 0; i < n; i++) if (rec_off[i + 1] - rec_off[i] > 0xffffffffull) return AFC_EINVAL;      // a chunk's records are counted in 32 bits
+    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n]) || docs_cap < afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n)) return AFC_EINVAL;
     if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of whole workflows through the ring, as for execution credentials.  A chunk's records travel with it (the kernels index them
@@ -1841,18 +1869,25 @@ static uint64_t vcc_bound(uint32_t n, uint64_t col_bytes, uint64_t m, uint64_t r
     return wf_doc_bound(n, col_bytes, m, rec_bytes) + (uint64_t)n * launch::vcc_frame_fixed() + 12 * col_bytes + 6 * chain_col_bytes +
            m * (launch::vcc_record_fixed() + 4) + 12 * rec_bytes + 6 * chain_rec_bytes + (3 * m + n) * launch::vcc_entry_fixed();
 }
-static uint64_t span(uint64_t a, uint64_t b) { return b >= a ? b - a : 0; }
 // The DID occurrence slots (3 per record, 1 per workflow) are counted and scanned in 32 bits, and each workflow's hash set has twice its
 // slots: a batch holds at most 2^31 - 1 slots, so neither count can wrap
 static bool vcc_slots_fit(uint64_t m, uint32_t n) { return m <= 0x7fffffffull && 3 * m + n <= 0x7fffffffull; }
+// ends: those of wf_spans, then chain_col_off at 0 and 2 n and chain_rec_col_off at 13 times the record ends
+static launch::OffsetSpans vcc_spans(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
+                                     const uint64_t* chain_rec_col_off) {
+    launch::OffsetSpans S = wf_spans(col_off, rec_off, rec_col_off);
+    S.s[3] = {chain_col_off, AFC_CHAIN_WORKFLOW_COLUMNS, -1};
+    S.s[4] = {chain_rec_col_off, AFC_CHAIN_RECORD_COLUMNS, 1};
+    S.k = 5;
+    return S;
+}
 uint64_t afc_vc_workflow_chain_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
                                      const uint64_t* chain_rec_col_off, uint32_t n) {
     if (!col_off || !rec_off || !rec_col_off || !chain_col_off || !chain_rec_col_off || n == 0) return 0;
-    const uint64_t cb = span(col_off[0], col_off[(size_t)n * AFC_WORKFLOW_COLUMNS]), ccb = span(chain_col_off[0], chain_col_off[(size_t)n * AFC_CHAIN_WORKFLOW_COLUMNS]);
-    const uint64_t r0 = rec_off[0], r1 = rec_off[n];
-    if (r1 < r0) return vcc_bound(n, cb, 0, 0, ccb, 0);
-    return vcc_bound(n, cb, r1 - r0, span(rec_col_off[2 * r0], rec_col_off[2 * r1]), ccb,
-                     span(chain_rec_col_off[AFC_CHAIN_RECORD_COLUMNS * r0], chain_rec_col_off[AFC_CHAIN_RECORD_COLUMNS * r1]));
+    const launch::OffsetSpans S = vcc_spans(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off);
+    uint64_t e[10];
+    offset_ends(S.s, S.k, n, e);
+    return vcc_bound(n, span(e[0], e[1]), span(e[2], e[3]), span(e[4], e[5]), span(e[6], e[7]), span(e[8], e[9]));
 }
 
 // per-call device scratch: the workflow-credential call's outputs and scratch, then the chain's (launch::VccArgs)
@@ -1907,22 +1942,15 @@ int afc_vc_workflow_chain_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
-    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies: gathered by one thread, read once
-    {
-        uint64_t* d_ends = nullptr;
-        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
-        cudaError_t e = launch::vcc_ends(d_col_off, d_rec_off, d_rec_col_off, d_chain_col_off, d_chain_rec_col_off, n, d_ends, st, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
-        cudaFreeAsync(d_ends, st);
-        CK(e);
-        CK(cudaStreamSynchronize(st));
-    }
+    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies
+    RC(read_ends(ctx, vcc_spans(d_col_off, d_rec_off, d_rec_col_off, d_chain_col_off, d_chain_rec_col_off), n, ends, st));
     if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[7] < ends[6] || ends[9] < ends[8] || !vcc_slots_fit(ends[3] - ends[2], n))
         return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
     if (m && (!d_rec_cols || !d_created_at || !d_chain_rec_cols || !d_rec_flags || !d_doc_size || !d_created_off)) return AFC_EINVAL;
-    if (bodies_cap < vcc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4], ends[7] - ends[6], ends[9] - ends[8])) return AFC_EINVAL;
-    const uint64_t dbound = wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4]);
+    const uint64_t cb = span(ends[0], ends[1]), rb = span(ends[4], ends[5]);
+    if (bodies_cap < vcc_bound(n, cb, m, rb, span(ends[6], ends[7]), span(ends[8], ends[9]))) return AFC_EINVAL;
+    const uint64_t dbound = wf_doc_bound(n, cb, m, rb);
     launch::VccArgs A{};
     ChainScratch S;
     uint8_t* scratch = nullptr;
@@ -1954,14 +1982,12 @@ int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
     for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
     const uint32_t C = AFC_WORKFLOW_COLUMNS, CC = AFC_CHAIN_WORKFLOW_COLUMNS, RC_ = AFC_CHAIN_RECORD_COLUMNS;
-    uint64_t bad = 0;
-    for (size_t k = 0; k < (size_t)n * C; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
-    for (size_t k = 0; k < (size_t)n * CC; k++) bad |= (uint64_t)(chain_col_off[k + 1] < chain_col_off[k]);
-    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(rec_off[i + 1] < rec_off[i]);
-    if (bad || !vcc_slots_fit(rec_off[n] - rec_off[0], n)) return AFC_EINVAL;
-    for (uint64_t k = 2 * rec_off[0]; k < 2 * rec_off[n]; k++) bad |= (uint64_t)(rec_col_off[k + 1] < rec_col_off[k]);
-    for (uint64_t k = RC_ * rec_off[0]; k < RC_ * rec_off[n]; k++) bad |= (uint64_t)(chain_rec_col_off[k + 1] < chain_rec_col_off[k]);
-    if (bad || bodies_cap < afc_vc_workflow_chain_bound(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off, n)) return AFC_EINVAL;
+    if (!monotone(col_off, (uint64_t)n * C) || !monotone(chain_col_off, (uint64_t)n * CC) || !monotone(rec_off, n) ||
+        !vcc_slots_fit(rec_off[n] - rec_off[0], n))
+        return AFC_EINVAL;
+    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n]) || !monotone(chain_rec_col_off, RC_ * rec_off[0], RC_ * rec_off[n]) ||
+        bodies_cap < afc_vc_workflow_chain_bound(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off, n))
+        return AFC_EINVAL;
     if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at || !chain_rec_cols || !rec_flags || !doc_size || !created_off)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of whole workflows through the ring, as for workflow credentials: the record arrays are staged for the chunk's records and
@@ -2100,9 +2126,14 @@ static uint64_t dres_bound(const afc_did_directory* dir, uint32_t n, uint64_t re
     const uint64_t per = std::max<uint64_t>(dir->largest, launch::dres_request_fixed());
     return (uint64_t)n * per + 6 * req_bytes;
 }
+// the _dev call reads these ends with k_dres_ends, which also checks every request's offsets
+static launch::OffsetSpans dres_spans(const uint64_t* req_off) { return {{{req_off, 1, -1}}, 1}; }
 uint64_t afc_did_resolve_bound(const afc_did_directory* dir, const uint64_t* req_off, uint32_t n) {
     if (!dir || !dir->has_ids || !req_off || n == 0) return 0;
-    return dres_bound(dir, n, span(req_off[0], req_off[n]));
+    const launch::OffsetSpans S = dres_spans(req_off);
+    uint64_t e[2];
+    offset_ends(S.s, S.k, n, e);
+    return dres_bound(dir, n, span(e[0], e[1]));
 }
 
 static int dres_check(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n,
@@ -2120,18 +2151,12 @@ int afc_did_resolve_batch_dev(afc_ctx* ctx, const afc_did_directory* dir, const 
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
-    uint64_t ends[3];                       // req_off[0], req_off[n] and the offsets' flags: gathered on the device, read once
-    {
-        uint64_t* d_ends = nullptr;
-        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
-        cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
-        if (e == cudaSuccess) e = launch::dres_ends(d_req_off, n, d_ends, st, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
-        cudaFreeAsync(d_ends, st);
-        CK(e);
-        CK(cudaStreamSynchronize(st));
-    }
-    if (ends[2] || bodies_cap < dres_bound(dir, n, ends[1] - ends[0])) return AFC_EINVAL;
+    uint64_t ends[3];                       // req_off[0], req_off[n] and the offsets' flags
+    RC(gather_ends(ctx, ends, 3, st, [&](uint64_t* d_ends) {
+        const cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
+        return e == cudaSuccess ? launch::dres_ends(d_req_off, n, d_ends, st, lc) : e;
+    }));
+    if (ends[2] || bodies_cap < dres_bound(dir, n, span(ends[0], ends[1]))) return AFC_EINVAL;
     const launch::DresDir D = dres_dir(dir);
     uint32_t* ent = nullptr;
     uint64_t* scan = nullptr;
@@ -2151,9 +2176,9 @@ int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint
                           uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off, uint8_t* state) {
     RC(dres_check(ctx, dir, kinds, reqs, req_off, n, bodies, body_off, state));
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
-    uint64_t bad = 0;
-    for (uint32_t i = 0; i < n; i++) bad |= (uint64_t)(req_off[i + 1] < req_off[i] || req_off[i + 1] - req_off[i] > 0x7fffffffull);   // 2^31 bytes
-    if (bad || bodies_cap < afc_did_resolve_bound(dir, req_off, n)) return AFC_EINVAL;
+    if (!monotone(req_off, n)) return AFC_EINVAL;
+    for (uint32_t i = 0; i < n; i++) if (req_off[i + 1] - req_off[i] > 0x7fffffffull) return AFC_EINVAL;     // 2^31 bytes
+    if (bodies_cap < afc_did_resolve_bound(dir, req_off, n)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     const launch::DresDir D = dres_dir(dir);
     const uint64_t per = dres_bound(dir, 1, 0);
@@ -2193,10 +2218,16 @@ int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint
 // backslash-u 00XX or fffd; a number token grows at most 21 / 4 times, 1e20 -> 100000000000000000000).
 static uint64_t wh_bound(uint32_t n, uint64_t bytes) { return (uint64_t)n * launch::wh_fixed_bytes() + 6 * bytes; }
 
+static launch::OffsetSpans wh_spans(const uint64_t* col_off, const uint64_t* result_off) {
+    return {{{col_off, AFC_WEBHOOK_COLUMNS, -1}, {result_off, 1, -1}}, 2};
+}
+
 uint64_t afc_webhook_bound(const uint64_t* col_off, const uint64_t* result_off, uint32_t n) {
     if (!col_off || !result_off || n == 0) return 0;
-    const uint64_t a = col_off[0], b = col_off[(size_t)n * AFC_WEBHOOK_COLUMNS], c = result_off[0], d = result_off[n];
-    return wh_bound(n, (b >= a ? b - a : 0) + (d >= c ? d - c : 0));
+    const launch::OffsetSpans S = wh_spans(col_off, result_off);
+    uint64_t e[4];
+    offset_ends(S.s, S.k, n, e);
+    return wh_bound(n, span(e[0], e[1]) + span(e[2], e[3]));
 }
 
 // per-call device scratch: the result tapes, the plans, the HMACs, scan tiles
@@ -2233,15 +2264,11 @@ int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64
     if (rc != AFC_OK || n == 0) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
-    uint64_t ends[4];                       // the column and result bytes bound the bodies and size the tapes: one synchronisation
-    CK(cudaMemcpyAsync(&ends[0], d_col_off, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[1], d_col_off + (size_t)n * AFC_WEBHOOK_COLUMNS, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[2], d_result_off, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ends[3], d_result_off + n, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (ends[1] < ends[0] || ends[3] < ends[2] || bodies_cap < wh_bound(n, (ends[1] - ends[0]) + (ends[3] - ends[2]))) return AFC_EINVAL;
+    uint64_t ends[4];                       // the column and result bytes bound the bodies and size the tapes
+    RC(read_ends(ctx, wh_spans(d_col_off, d_result_off), n, ends, st));
+    const uint64_t rb = span(ends[2], ends[3]);
+    if (ends[1] < ends[0] || ends[3] < ends[2] || bodies_cap < wh_bound(n, span(ends[0], ends[1]) + rb)) return AFC_EINVAL;
     if ((!d_results && ends[3] != ends[2]) || !d_secrets) return AFC_EINVAL;
-    const uint64_t rb = ends[3] - ends[2];
     CallLog lc(ctx);
     uint8_t* scratch = nullptr;
     WebhookScratch S;
@@ -2259,13 +2286,11 @@ int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* co
     int rc = wh_check(ctx, cols, col_off, duration_ms, flags, results, result_off, secrets, secret_off, n, bodies, body_off, headers, status);
     if (rc != AFC_OK) return rc;
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
-    uint64_t bad = 0;
-    for (size_t k = 0; k < (size_t)n * AFC_WEBHOOK_COLUMNS; k++) bad |= (uint64_t)(col_off[k + 1] < col_off[k]);
-    for (uint32_t i = 0; i < n; i++) {
-        bad |= (uint64_t)(result_off[i + 1] < result_off[i]) | (uint64_t)(secret_off[i + 1] < secret_off[i]);
-        bad |= (uint64_t)(flags[i] & ~(uint32_t)(AFC_WEBHOOK_HAS_DURATION | AFC_WEBHOOK_HAS_ERROR_MESSAGE | AFC_WEBHOOK_HAS_SECRET));
-    }
-    if (bad || bodies_cap < afc_webhook_bound(col_off, result_off, n)) return AFC_EINVAL;
+    uint32_t bad = 0;
+    for (uint32_t i = 0; i < n; i++) bad |= flags[i] & ~(uint32_t)(AFC_WEBHOOK_HAS_DURATION | AFC_WEBHOOK_HAS_ERROR_MESSAGE | AFC_WEBHOOK_HAS_SECRET);
+    if (bad || !monotone(col_off, (uint64_t)n * AFC_WEBHOOK_COLUMNS) || !monotone(result_off, n) || !monotone(secret_off, n) ||
+        bodies_cap < afc_webhook_bound(col_off, result_off, n))
+        return AFC_EINVAL;
     if ((!results && result_off[n] != result_off[0]) || (!secrets && secret_off[n] != secret_off[0])) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of deliveries through the ring, as for execution credentials: a chunk's stream is synchronised once after the sizes pass to
@@ -2323,13 +2348,17 @@ static uint64_t didr_bound(uint32_t n, uint64_t node_bytes, uint64_t server_len,
     return (uint64_t)n * (launch::didr_req_fixed() + 6 * server_len) + 6 * node_bytes + m * launch::didr_per_id_fixed() + 12 * id_bytes;
 }
 
+// ends: node_off at 0 and n, id_idx at 0 and 2 n, id_off at those
+static launch::OffsetSpans didr_spans(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off) {
+    return {{{node_off, 1, -1}, {id_idx, 2, -1}, {id_off, 1, 1}}, 3};
+}
+
 uint64_t afc_did_register_bound(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t server_id_len) {
     if (!node_off || !id_idx || !id_off || n == 0) return 0;
-    const uint64_t a = node_off[0], b = node_off[n], r0 = id_idx[0], r1 = id_idx[2 * (size_t)n];
-    const uint64_t nb = b >= a ? b - a : 0;
-    if (r1 < r0) return didr_bound(n, nb, server_id_len, 0, 0);
-    const uint64_t c = id_off[r0], d = id_off[r1];
-    return didr_bound(n, nb, server_id_len, r1 - r0, d >= c ? d - c : 0);
+    const launch::OffsetSpans S = didr_spans(node_off, id_idx, id_off);
+    uint64_t e[6];
+    offset_ends(S.s, S.k, n, e);
+    return didr_bound(n, span(e[0], e[1]), server_id_len, span(e[2], e[3]), span(e[4], e[5]));
 }
 
 // per-call device scratch (launch::DidrArgs); the derived seeds are secret
@@ -2359,20 +2388,12 @@ int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
-    uint64_t ends[6];                       // the ends of the three offset arrays bound the bodies: gathered by one thread, read once
-    {
-        uint64_t* d_ends = nullptr;
-        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
-        cudaError_t e = launch::didr_ends(d_node_off, d_id_idx, d_id_off, n, d_ends, st, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
-        cudaFreeAsync(d_ends, st);
-        CK(e);
-        CK(cudaStreamSynchronize(st));
-    }
+    uint64_t ends[6];                       // the ends of the three offset arrays bound the bodies
+    RC(read_ends(ctx, didr_spans(d_node_off, d_id_idx, d_id_off), n, ends, st));
     if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] + n > 0xffffffffull) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
     if (ends[5] > ends[4] && !d_ids) return AFC_EINVAL;
-    if (body_cap < didr_bound(n, ends[1] - ends[0], server_id_len, m, ends[5] - ends[4])) return AFC_EINVAL;
+    if (body_cap < didr_bound(n, span(ends[0], ends[1]), server_id_len, m, span(ends[4], ends[5]))) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     launch::DidrArgs A{};
     uint8_t* d_server;
@@ -2416,9 +2437,7 @@ int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8
     if (!monotone(node_off, n) || !monotone(id_idx, 2 * n)) return AFC_EINVAL;
     const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n];
     if (r_last - r_first + n > 0xffffffffull) return AFC_EINVAL;
-    uint64_t bad = 0;
-    for (uint64_t k = r_first; k < r_last; k++) bad |= (uint64_t)(id_off[k + 1] < id_off[k]);
-    if (bad || (id_off[r_last] > id_off[r_first] && !ids)) return AFC_EINVAL;
+    if (!monotone(id_off, r_first, r_last) || (id_off[r_last] > id_off[r_first] && !ids)) return AFC_EINVAL;
     if (body_cap < afc_did_register_bound(node_off, id_idx, id_off, n, server_id_len)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
@@ -2489,21 +2508,19 @@ static uint64_t didrr_bound(uint32_t n, uint64_t agent_bytes, uint64_t server_le
            G * launch::didrr_per_reg_fixed() + 6 * reg_bytes;
 }
 
+// ends: agent_col_off at 0 and 3 n, id_idx at 0 and 2 n, id_off at those, reg_idx at 0 and 2 n, reg_col_off at five times those
+static launch::OffsetSpans didrr_spans(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
+                                       const uint64_t* reg_col_off) {
+    return {{{agent_col_off, 3, -1}, {id_idx, 2, -1}, {id_off, 1, 1}, {reg_idx, 2, -1}, {reg_col_off, 5, 3}}, 5};
+}
+
 uint64_t afc_did_reregister_bound(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
                                   const uint64_t* reg_col_off, uint32_t n, uint64_t server_id_len) {
     if (!agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || n == 0) return 0;
-    const uint64_t a = agent_col_off[0], b = agent_col_off[3 * (size_t)n];
-    const uint64_t r0 = id_idx[0], r1 = id_idx[2 * (size_t)n], g0 = reg_idx[0], g1 = reg_idx[2 * (size_t)n];
-    uint64_t m = 0, ib = 0, G = 0, rb = 0;
-    if (r1 >= r0) {
-        const uint64_t c = id_off[r0], d = id_off[r1];
-        m = r1 - r0; ib = d >= c ? d - c : 0;
-    }
-    if (g1 >= g0) {
-        const uint64_t c = reg_col_off[5 * g0], d = reg_col_off[5 * g1];
-        G = g1 - g0; rb = d >= c ? d - c : 0;
-    }
-    return didrr_bound(n, b >= a ? b - a : 0, server_id_len, m, ib, G, rb);
+    const launch::OffsetSpans S = didrr_spans(agent_col_off, id_idx, id_off, reg_idx, reg_col_off);
+    uint64_t e[10];
+    offset_ends(S.s, S.k, n, e);
+    return didrr_bound(n, span(e[0], e[1]), server_id_len, span(e[2], e[3]), span(e[4], e[5]), span(e[6], e[7]), span(e[8], e[9]));
 }
 
 // per-call device scratch (launch::DidrrArgs); the derived seeds are secret
@@ -2536,22 +2553,14 @@ int afc_did_reregister_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, con
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
-    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies: gathered by one thread, read once
-    {
-        uint64_t* d_ends = nullptr;
-        CK(cudaMallocAsync((void**)&d_ends, sizeof ends, st));
-        cudaError_t e = launch::didrr_ends(d_agent_col_off, d_id_idx, d_id_off, d_reg_idx, d_reg_col_off, n, d_ends, st, lc);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ends, d_ends, sizeof ends, cudaMemcpyDeviceToHost, st);
-        cudaFreeAsync(d_ends, st);
-        CK(e);
-        CK(cudaStreamSynchronize(st));
-    }
+    uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies
+    RC(read_ends(ctx, didrr_spans(d_agent_col_off, d_id_idx, d_id_off, d_reg_idx, d_reg_col_off), n, ends, st));
     for (int k = 0; k < 10; k += 2)
         if (ends[k + 1] < ends[k]) return AFC_EINVAL;
     if ((ends[3] - ends[2]) + (ends[7] - ends[6]) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]), G = (uint32_t)(ends[7] - ends[6]);
     if ((ends[5] > ends[4] && !d_ids) || (ends[9] > ends[8] && !d_reg_cols) || (m && !d_id_flags) || (G && !d_reg_flags)) return AFC_EINVAL;
-    if (body_cap < didrr_bound(n, ends[1] - ends[0], server_id_len, m, ends[5] - ends[4], G, ends[9] - ends[8])) return AFC_EINVAL;
+    if (body_cap < didrr_bound(n, span(ends[0], ends[1]), server_id_len, m, span(ends[4], ends[5]), G, span(ends[8], ends[9]))) return AFC_EINVAL;
     uint8_t* scratch = nullptr;
     launch::DidrrArgs A{};
     uint8_t* d_server;
@@ -2599,10 +2608,8 @@ int afc_did_reregister_batch(afc_ctx* ctx, const uint8_t* master_seed, const uin
     if (!monotone(agent_col_off, 3 * n) || !monotone(id_idx, 2 * n) || !monotone(reg_idx, 2 * n)) return AFC_EINVAL;
     const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n], g_first = reg_idx[0], g_last = reg_idx[2 * (size_t)n];
     if ((r_last - r_first) + (g_last - g_first) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
-    uint64_t bad = 0;
-    for (uint64_t k = r_first; k < r_last; k++) bad |= (uint64_t)(id_off[k + 1] < id_off[k]);
-    for (uint64_t k = 5 * g_first; k < 5 * g_last; k++) bad |= (uint64_t)(reg_col_off[k + 1] < reg_col_off[k]);
-    if (bad || (id_off[r_last] > id_off[r_first] && !ids) || (reg_col_off[5 * g_last] > reg_col_off[5 * g_first] && !reg_cols) ||
+    if (!monotone(id_off, r_first, r_last) || !monotone(reg_col_off, 5 * g_first, 5 * g_last) || (id_off[r_last] > id_off[r_first] && !ids) ||
+        (reg_col_off[5 * g_last] > reg_col_off[5 * g_first] && !reg_cols) ||
         (r_last > r_first && !id_flags) || (g_last > g_first && !reg_flags))
         return AFC_EINVAL;
     if (body_cap < afc_did_reregister_bound(agent_col_off, id_idx, id_off, reg_idx, reg_col_off, n, server_id_len)) return AFC_EINVAL;

@@ -174,24 +174,9 @@ k_didr_frame(const uint8_t* __restrict__ server, uint64_t server_len, const uint
     w.finish();
 }
 
-// node_off[0], node_off[n], id_idx[0], id_idx[2n], and id_off at both (one thread)
-__global__ void k_didr_ends(const uint64_t* __restrict__ node_off, const uint64_t* __restrict__ id_idx, const uint64_t* __restrict__ id_off, uint32_t n,
-                            uint64_t* __restrict__ out) {
-    const uint64_t a = id_idx[0], b = id_idx[2 * (size_t)n];
-    out[0] = node_off[0]; out[1] = node_off[n]; out[2] = a; out[3] = b;
-    const bool ok = b >= a;                                       // id_off is read only where the id range is not backwards
-    out[4] = ok ? id_off[a] : 0; out[5] = ok ? id_off[b] : 0;
-}
-
 namespace launch {
 
 static inline uint32_t didr_blocks(uint64_t n) { return (uint32_t)((n + DIDR_THREADS - 1) / DIDR_THREADS); }
-
-cudaError_t didr_ends(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t* out, cudaStream_t s,
-                      LaunchLog* lg) {
-    AFC_LAUNCH(lg, "k_didr_ends", s, k_didr_ends<<<1, 1, 0, s>>>(node_off, id_idx, id_off, n, out));
-    return cudaGetLastError();
-}
 
 cudaError_t didr_register(const DidrArgs& A, cudaStream_t s, LaunchLog* lg) {
     const uint32_t n = A.n, m = A.m;

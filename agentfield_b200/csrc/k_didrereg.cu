@@ -230,26 +230,9 @@ k_didrr_frame(const uint8_t* __restrict__ agent_cols, const uint64_t* __restrict
     w.finish();
 }
 
-// agent_col_off at 0 and 3n, id_idx at 0 and 2n, id_off at both, reg_idx at 0 and 2n, reg_col_off at five times both (one thread)
-__global__ void k_didrr_ends(const uint64_t* __restrict__ agent_col_off, const uint64_t* __restrict__ id_idx, const uint64_t* __restrict__ id_off,
-                             const uint64_t* __restrict__ reg_idx, const uint64_t* __restrict__ reg_col_off, uint32_t n, uint64_t* __restrict__ out) {
-    const uint64_t a = id_idx[0], b = id_idx[2 * (size_t)n], c = reg_idx[0], d = reg_idx[2 * (size_t)n];
-    out[0] = agent_col_off[0]; out[1] = agent_col_off[3 * (size_t)n]; out[2] = a; out[3] = b;
-    const bool ok = b >= a, okr = d >= c;                         // offsets are read only where the index range is not backwards
-    out[4] = ok ? id_off[a] : 0; out[5] = ok ? id_off[b] : 0;
-    out[6] = c; out[7] = d;
-    out[8] = okr ? reg_col_off[DIDRR_COLS * c] : 0; out[9] = okr ? reg_col_off[DIDRR_COLS * d] : 0;
-}
-
 namespace launch {
 
 static inline uint32_t didrr_blocks(uint64_t n) { return (uint32_t)((n + DIDRR_THREADS - 1) / DIDRR_THREADS); }
-
-cudaError_t didrr_ends(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx, const uint64_t* reg_col_off,
-                       uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg) {
-    AFC_LAUNCH(lg, "k_didrr_ends", s, k_didrr_ends<<<1, 1, 0, s>>>(agent_col_off, id_idx, id_off, reg_idx, reg_col_off, n, out));
-    return cudaGetLastError();
-}
 
 cudaError_t didrr_reregister(const DidrrArgs& A, cudaStream_t s, LaunchLog* lg) {
     const uint32_t n = A.n, m = A.m, G = A.G;

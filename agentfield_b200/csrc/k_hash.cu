@@ -346,6 +346,8 @@ k_scan_add(uint64_t* __restrict__ v, uint64_t n, const uint64_t* __restrict__ ti
 #pragma unroll
     for (int k = 0; k < SCAN_PER_THREAD; k++) if (base + k < n) v[base + k] += add;
 }
+// The ends a _dev call needs before it can size anything (offset_ends): one thread, since an indirect span's indices are device words
+__global__ void k_offset_ends(const launch::OffsetSpans S, uint32_t n, uint64_t* __restrict__ out) { offset_ends(S.s, S.k, n, out); }
 
 // ---- text codecs either side of the kernels (SURVEY.md §8f N3): base64url without padding for signatures / digests
 // (base64.RawURLEncoding in vc_service.go:465,514) and lowercase hex for the webhook header (hex.EncodeToString,
@@ -478,6 +480,10 @@ cudaError_t offsets_from_lengths(uint64_t* out_off, uint32_t n, uint64_t* scan_s
     AFC_LAUNCH(lg, "k_scan_tiles", s, k_scan_tiles<<<tiles, SCAN_THREADS, 0, s>>>(out_off + 1, n, scan_scratch));
     AFC_LAUNCH(lg, "k_scan_tile_sums", s, k_scan_tile_sums<<<1, 1024, 0, s>>>(scan_scratch, tiles));
     AFC_LAUNCH(lg, "k_scan_add", s, k_scan_add<<<tiles, SCAN_THREADS, 0, s>>>(out_off + 1, n, scan_scratch));
+    return cudaGetLastError();
+}
+cudaError_t offset_ends(const OffsetSpans& S, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg) {
+    AFC_LAUNCH(lg, "k_offset_ends", s, k_offset_ends<<<1, 1, 0, s>>>(S, n, out));
     return cudaGetLastError();
 }
 cudaError_t json_fill(const uint8_t* segs, const uint32_t* seg_off, const uint8_t* kinds, uint32_t F, const uint8_t* fields,

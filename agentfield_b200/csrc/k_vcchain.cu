@@ -294,30 +294,11 @@ k_vcc_copy_doc(const launch::VccArgs A) {
     for (uint64_t b = threadIdx.x; b < len; b += blockDim.x) dst[b] = src[b];
 }
 
-// The ends the host needs before it can size anything: those of k_vcw_ends, then chain_col_off[0], [2 n] and chain_rec_col_off at both
-// record ends
-__global__ void k_vcc_ends(const uint64_t* __restrict__ col_off, const uint64_t* __restrict__ rec_off, const uint64_t* __restrict__ rec_col_off,
-                           const uint64_t* __restrict__ chain_col_off, const uint64_t* __restrict__ chain_rec_col_off, uint32_t n,
-                           uint64_t* __restrict__ out) {
-    const uint64_t r0 = rec_off[0], r1 = rec_off[n];
-    const bool ok = r1 >= r0;
-    out[0] = col_off[0]; out[1] = col_off[(size_t)n * VCW_COLUMNS]; out[2] = r0; out[3] = r1;
-    out[4] = ok ? rec_col_off[2 * r0] : 0; out[5] = ok ? rec_col_off[2 * r1] : 0;
-    out[6] = chain_col_off[0]; out[7] = chain_col_off[(size_t)n * VCC_COLUMNS];
-    out[8] = ok ? chain_rec_col_off[VCC_REC_COLUMNS * r0] : 0; out[9] = ok ? chain_rec_col_off[VCC_REC_COLUMNS * r1] : 0;
-}
-
 namespace launch {
 
 static inline uint32_t vcc_blocks(uint64_t n) { return (uint32_t)((n + VCC_THREADS - 1) / VCC_THREADS); }
 
 size_t vcc_lay_words() { return VCC_LAY; }
-
-cudaError_t vcc_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
-                     const uint64_t* chain_rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s, LaunchLog* lg) {
-    AFC_LAUNCH(lg, "k_vcc_ends", s, k_vcc_ends<<<1, 1, 0, s>>>(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off, n, out));
-    return cudaGetLastError();
-}
 
 cudaError_t vcc_sizes(const VccArgs& A, cudaStream_t s, LaunchLog* lg) {
     if (A.n == 0) return cudaSuccess;

@@ -132,15 +132,6 @@ k_vcw_proof(const uint8_t* __restrict__ sigs, const uint8_t* __restrict__ state,
     vci_proof_one(w, docs + doc_off[i + 1] - 3 - VCI_PV_CHARS, pv);
 }
 
-// The ends the host needs before it can size anything: col_off[0], col_off[7 n], rec_off[0], rec_off[n] and rec_col_off at both
-__global__ void k_vcw_ends(const uint64_t* __restrict__ col_off, const uint64_t* __restrict__ rec_off, const uint64_t* __restrict__ rec_col_off,
-                           uint32_t n, uint64_t* __restrict__ out) {
-    const uint64_t r0 = rec_off[0], r1 = rec_off[n];
-    out[0] = col_off[0]; out[1] = col_off[(size_t)n * VCW_COLUMNS]; out[2] = r0; out[3] = r1;
-    const bool ok = r1 >= r0;                                     // rec_col_off is read only where the record range is not backwards
-    out[4] = ok ? rec_col_off[2 * r0] : 0; out[5] = ok ? rec_col_off[2 * r1] : 0;
-}
-
 namespace launch {
 
 static inline uint32_t vcw_blocks(uint64_t n) { return (uint32_t)((n + VCW_THREADS - 1) / VCW_THREADS); }
@@ -149,11 +140,6 @@ static const VcwProgram& vcw_program() {
     return P;
 }
 
-cudaError_t vcw_ends(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n, uint64_t* out, cudaStream_t s,
-                     LaunchLog* lg) {
-    AFC_LAUNCH(lg, "k_vcw_ends", s, k_vcw_ends<<<1, 1, 0, s>>>(col_off, rec_off, rec_col_off, n, out));
-    return cudaGetLastError();
-}
 cudaError_t vcw_records(const uint8_t* rec_cols, const uint64_t* rec_col_off, const int64_t* created_at, const uint64_t* rec_off, uint32_t m,
                         uint8_t* cls, uint64_t* id_len, cudaStream_t s, LaunchLog* lg) {
     if (m == 0) return cudaSuccess;
