@@ -13,6 +13,7 @@ import numpy as np
 AFC_OK, AFC_EINVAL, AFC_ECUDA, AFC_ENOMEM, AFC_ENCCL, AFC_ESTATE = 0, -1, -2, -3, -4, -5
 DOC_EXECUTION_VC, DOC_WORKFLOW_VC = 0, 1
 VC_INVALID, VC_VALID, VC_HOST, VC_UNRESOLVED, VC_BAD_ENCODING = 0, 1, 2, 3, 4
+VREQ_OK, VREQ_BAD_REQUEST, VREQ_HOST = 0, 1, 2
 AUDIT_COLUMNS = ("issuer_did", "execution_id", "workflow_id", "session_id", "caller_did", "target_did", "status", "input_hash", "output_hash",
                  "signature")
 # AFC_AUDIT_*: bit k < 10 = column k of AUDIT_COLUMNS differs from the document
@@ -99,6 +100,9 @@ SYMBOLS = {
     "afc_vc_verify_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_vc_verify_json_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_verify_json_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_uint32, vp, vp, vp]),
+    "afc_vc_verify_request_bound": (C.c_uint64, [vp, C.c_uint32]),
+    "afc_vc_verify_request_batch": (C.c_int, [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp]),
+    "afc_vc_verify_request_batch_dev": (C.c_int, [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp]),
     "afc_vc_audit_stored_batch": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp]),
     "afc_vc_audit_stored_batch_dev": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, C.c_uint32, vp, vp, vp]),
     "afc_vc_issue_bound": (C.c_uint64, [vp, C.c_uint32]),

@@ -211,6 +211,22 @@ cudaError_t dres_emit(const DresDir& D, const uint8_t* kinds, const uint8_t* req
                       const uint32_t* ent, const uint64_t* body_off, uint8_t* bodies, cudaStream_t s, LaunchLog* lg);
 uint64_t dres_request_fixed();         // the bound's constant per request besides the directory's largest body (afc_didresolve.cuh)
 
+// ---- k_vcreq.cu: VC verification requests answered on the device (afc_vcreq.cuh).  n requests at req_off[i] .. req_off[i + 1] (absolute).
+// bind: each request's VRB_* kind; span: where its object value starts in it; doc_off: n + 1 offsets of the object values once gathered
+// (the scan runs here)
+cudaError_t vrq_bind(const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const uint8_t* dids, const uint32_t* did_off, const uint32_t* slots,
+                     uint32_t slot_mask, uint8_t* bind, uint32_t* span, uint64_t* doc_off, uint64_t* scan, cudaStream_t s, LaunchLog* lg);
+cudaError_t vrq_gather(const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const uint32_t* span, const uint64_t* doc_off, uint8_t* docs,
+                       cudaStream_t s, LaunchLog* lg);
+// after the json-verify path on docs (status, fields n x 4): states, base64 error indices (b64_at: n) and body offsets; then the bodies.
+// schema: the execution document's VcjSchema on the device
+cudaError_t vrq_sizes(const void* schema, const uint8_t* bind, const uint8_t* status, const uint32_t* fields, const uint8_t* docs,
+                      const uint64_t* doc_off, uint32_t n, uint32_t* b64_at, uint8_t* state, uint64_t* body_off, uint64_t* scan, cudaStream_t s,
+                      LaunchLog* lg);
+cudaError_t vrq_emit(const uint8_t* bind, const uint8_t* status, const uint32_t* fields, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                     const uint32_t* b64_at, const uint64_t* body_off, uint8_t* bodies, cudaStream_t s, LaunchLog* lg);
+uint64_t vrq_request_fixed();          // the bound's constant per request (afc_vcreq.cuh)
+
 // ---- k_didreg.cu: agent DIDs registered on the device (afc_didreg.cuh).  node_off: n + 1 absolute offsets; id_idx: 2n + 1 absolute id
 // indices (request i's reasoners [id_idx[2i], id_idx[2i+1]), skills [id_idx[2i+1], id_idx[2i+2])); id_off: absolute, indexed by absolute id.
 // The m = id_idx[2n] - id_idx[0] ids have per-id scratch; the component outputs hold n + m entries (the components, then zeros).

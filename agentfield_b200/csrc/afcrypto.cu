@@ -1435,6 +1435,110 @@ int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, con
     return vc_verify_dev(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, stream, true);
 }
 
+// ---------------------------------------------------------------------------------- VC verification requests
+// Per request the longest constant text of a response plus at most 6 bytes per request byte (issuer and issuanceDate re-escaped)
+static uint64_t vrq_bound(uint32_t n, uint64_t req_bytes) { return (uint64_t)n * launch::vrq_request_fixed() + 6 * req_bytes; }
+uint64_t afc_vc_verify_request_bound(const uint64_t* req_off, uint32_t n) {
+    if (!req_off || n == 0) return 0;
+    const launch::OffsetSpans S = doc_spans(req_off);
+    uint64_t e[2];
+    offset_ends(S.s, S.k, n, e);
+    return vrq_bound(n, span(e[0], e[1]));
+}
+static int vrq_check(afc_ctx* ctx, afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const uint8_t* bodies,
+                     const uint64_t* body_off, const uint8_t* state) {
+    if (!ctx || !ks || ks->ctx != ctx || !req_off || !body_off || (n && (!reqs || !bodies || !state))) return AFC_EINVAL;
+    if (!ks->named) return AFC_ESTATE;
+    return AFC_OK;
+}
+// The scratch of a batch of n requests of req_bytes bytes: the gathered object values (never more than the requests), what the bind
+// leaves for the passes after it, and the json-verify path's own scratch over the gathered values
+struct VrqScratch { uint8_t* docs; uint64_t* doc_off; uint8_t* bind; uint32_t* span; uint8_t* status; uint32_t* fields; uint32_t* b64_at; VcScratch vc; };
+static void vrq_scratch(Carve& k, VrqScratch& s, uint32_t n, uint64_t req_bytes, uint32_t n_keys) {
+    s.docs = k.take(req_bytes + 64);
+    s.doc_off = k.take<uint64_t>((size_t)n + 1);
+    s.bind = k.take(n);
+    s.span = k.take<uint32_t>(n);
+    s.status = k.take((size_t)n + 16);
+    s.fields = k.take<uint32_t>((size_t)n * 4 + 4);
+    s.b64_at = k.take<uint32_t>(n);
+    vc_scratch(k, s.vc, n, req_bytes, n_keys, false);
+}
+// bind -> gather -> the json-verify path, unchanged -> sizes (and the body scan); the caller then runs vrq_emit
+static cudaError_t vrq_enqueue(afc_ctx* ctx, const afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const VrqScratch& S,
+                               uint8_t* state, uint64_t* body_off, cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = launch::vrq_bind(reqs, req_off, n, ks->d_dids, ks->d_did_off, ks->d_slots, ks->slot_mask, S.bind, S.span, S.doc_off, S.vc.scan,
+                                     st, lg);
+    if (e == cudaSuccess) e = launch::vrq_gather(reqs, req_off, n, S.span, S.doc_off, S.docs, st, lg);
+    if (e == cudaSuccess) e = vc_stored_enqueue(ctx, ks, AFC_DOC_EXECUTION_VC, S.docs, S.doc_off, n, S.status, S.fields, S.vc, st, lg, nullptr, nullptr,
+                                                nullptr, true);
+    if (e == cudaSuccess) e = launch::vrq_sizes(ks->d_vcj_schemas, S.bind, S.status, S.fields, S.docs, S.doc_off, n, S.b64_at, state, body_off,
+                                                S.vc.scan, st, lg);
+    return e;
+}
+
+int afc_vc_verify_request_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint8_t* d_reqs, const uint64_t* d_req_off, uint32_t n, uint8_t* d_bodies,
+                                    uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream) {
+    RC(vrq_check(ctx, ks, d_reqs, d_req_off, n, d_bodies, d_body_off, d_state));
+    if (n == 0) return AFC_OK;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    CallLog lc(ctx);
+    uint64_t ends[3];                       // req_off[0], req_off[n] and the offsets' flags (k_dres_ends applies the same two rules)
+    RC(gather_ends(ctx, ends, 3, st, [&](uint64_t* d_ends) {
+        const cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
+        return e == cudaSuccess ? launch::dres_ends(d_req_off, n, d_ends, st, lc) : e;
+    }));
+    const uint64_t req_bytes = span(ends[0], ends[1]);
+    if (ends[2] || bodies_cap < vrq_bound(n, req_bytes)) return AFC_EINVAL;
+    uint8_t* scratch = nullptr;
+    VrqScratch S;
+    CK(pool_carve(&scratch, st, [&](Carve& k) { vrq_scratch(k, S, n, req_bytes, ks->n_keys); }));
+    cudaError_t e = vrq_enqueue(ctx, ks, d_reqs, d_req_off, n, S, d_state, d_body_off, st, lc);
+    if (e == cudaSuccess) e = launch::vrq_emit(S.bind, S.status, S.fields, S.docs, S.doc_off, n, S.b64_at, d_body_off, d_bodies, st, lc);
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
+}
+
+int afc_vc_verify_request_batch(afc_ctx* ctx, afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, uint8_t* bodies,
+                                uint64_t bodies_cap, uint64_t* body_off, uint8_t* state) {
+    RC(vrq_check(ctx, ks, reqs, req_off, n, bodies, body_off, state));
+    if (n == 0) { body_off[0] = 0; return AFC_OK; }
+    if (!monotone(req_off, n)) return AFC_EINVAL;
+    for (uint32_t i = 0; i < n; i++) if (req_off[i + 1] - req_off[i] > 0x7fffffffull) return AFC_EINVAL;     // 2^31 bytes
+    if (bodies_cap < afc_vc_verify_request_bound(req_off, n)) return AFC_EINVAL;
+    CK(cudaSetDevice(ctx->device));
+    const uint64_t per = vrq_bound(1, 0);
+    // chunks of whole requests, sized by what they stage (the requests, their gathered values and signing messages) and the most their
+    // bodies can take
+    auto measure = [&](uint32_t i0, uint32_t i) { return 9 * (req_off[i + 1] - req_off[i0]) + per * ((uint64_t)i - i0 + 1); };
+    uint64_t base = 0;
+    Ring ring(ctx);
+    return ring.walk(n, measure, [&](Ring& r) {
+        const uint32_t i0 = r.i0, cnt = r.cnt;
+        const uint64_t req_bytes = req_off[i0 + cnt] - req_off[i0];
+        Msgs m;
+        uint8_t *d_bodies, *d_state;
+        uint64_t* d_off;
+        VrqScratch S;
+        RC(r.stage([&](Stager& k) {
+            m = stage_msgs(k, reqs, req_off, i0, cnt);
+            d_bodies = k.take(vrq_bound(cnt, req_bytes) + 64);
+            d_off = k.take<uint64_t>((size_t)cnt + 1);
+            d_state = k.take(cnt);
+            vrq_scratch(k, S, cnt, req_bytes, ks->n_keys);
+        }));
+        CK(vrq_enqueue(ctx, ks, m.d, m.off, cnt, S, d_state, d_off, r.st, r.lc));
+        uint64_t bytes;
+        RC(r.read(&bytes, {d_off + cnt}));
+        CK(launch::vrq_emit(S.bind, S.status, S.fields, S.docs, S.doc_off, cnt, S.b64_at, d_off, d_bodies, r.st, r.lc));
+        RC(r.copy_back({offsets_out(body_off, i0, d_off, (size_t)cnt + 1, base), {state, i0, d_state, cnt}, {bodies, base, d_bodies, bytes}}));
+        base += bytes;
+        return AFC_OK;
+    });
+}
+
 // audit: the arguments of afc_vc_verify_stored_batch, plus columns exactly for execution documents
 static int vc_audit_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
                           const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {

@@ -888,6 +888,46 @@ class KeySet:
         buf, off = pack(docs)
         return self.verify_json_packed(doc_kind, buf, off)
 
+    def verify_requests_packed(self, reqs, req_off):
+        """afc_vc_verify_request_batch: n raw request bodies of POST /api/v1/did/verify (packed bytes + n+1 offsets) -> (bodies uint8,
+        body_off uint64 [n+1], state uint8 [n] of _abi.VREQ_*)."""
+        n = len(req_off) - 1
+        cap = self._lib.afc_vc_verify_request_bound(_abi.ptr(req_off), n)
+        bodies = np.empty(max(cap, 1), dtype=np.uint8)
+        body_off = np.zeros(n + 1, dtype=np.uint64)
+        state = np.empty(max(n, 1), dtype=np.uint8)
+        _abi.check(self._lib.afc_vc_verify_request_batch(self.ctx.handle, self.handle, _abi.ptr(reqs), _abi.ptr(req_off), n, _abi.ptr(bodies), cap,
+                                                         _abi.ptr(body_off), _abi.ptr(state)), self.ctx.handle)
+        return bodies[:int(body_off[n])], body_off, state[:n]
+
+    def verify_requests_dev(self, d_reqs, d_req_off, n, stream=None):
+        """afc_vc_verify_request_batch_dev on device tensors (request bytes uint8, offsets int64 [n+1]).  Returns (d_bodies uint8,
+        d_body_off int64 [n+1], d_state uint8 [n])."""
+        import torch
+        dev = d_req_off.device
+        cap = 0
+        if n:
+            a, b = (int(x) for x in torch.cat([d_req_off[0:1], d_req_off[n:n + 1]]).cpu().tolist())
+            cap = self._lib.afc_vc_verify_request_bound(_abi.ptr(np.array([a, max(a, b)], dtype=np.uint64)), 1) + \
+                (n - 1) * self._lib.afc_vc_verify_request_bound(_abi.ptr(np.zeros(2, dtype=np.uint64)), 1)
+        d_bodies = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        d_body_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_state = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        _abi.check(self._lib.afc_vc_verify_request_batch_dev(self.ctx.handle, self.handle, _abi.ptr(d_reqs), _abi.ptr(d_req_off), n, _abi.ptr(d_bodies),
+                                                             cap, _abi.ptr(d_body_off), _abi.ptr(d_state), self.ctx._stream(stream)), self.ctx.handle)
+        total = int(d_body_off[n]) if n else 0
+        return d_bodies[:total], d_body_off, d_state[:n]
+
+    def verify_requests(self, bodies):
+        """Many request bodies (bytes) in one host-buffer call: [(state, response body bytes)] in request order (an _abi.VREQ_HOST request
+        has an empty body)."""
+        if not bodies:
+            return []
+        buf, off = pack([bytes(b) for b in bodies])
+        out, body_off, state = self.verify_requests_packed(buf, off)
+        raw = out.tobytes()
+        return [(int(state[i]), raw[int(body_off[i]):int(body_off[i + 1])]) for i in range(len(bodies))]
+
     def audit_stored_packed(self, doc_kind, buf, off, cols=None, col_off=None):
         """afc_vc_audit_stored_batch: n stored documents (packed bytes + n+1 offsets) and, for execution documents, their records'
         _abi.AUDIT_COLUMNS columns (packed bytes + n*10+1 offsets) -> (status uint8 [n], issues uint32 [n] of _abi.AUDIT_* bits)."""

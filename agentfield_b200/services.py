@@ -470,6 +470,54 @@ class VCService:
                     out[i] = _vc_response(False, message="Invalid signature")
         return out
 
+    # -- verification requests answered on the device (afc_vc_verify_request_batch)
+    def serve_verify_requests(self, bodies):
+        """POST /api/v1/did/verify (did_handlers.go:97-111) for many raw request bodies: (http status, response bytes) per body, the bytes
+        c.JSON writes.  Bind, verify and response are built on the GPU in one call; the requests it leaves to the host (AFC_VREQ_HOST) run
+        the handler here: the body bound with Go's rules, go_unmarshal_vc's decoding of the document and _keyed_verify."""
+        bodies = [bytes(b) for b in bodies]
+        ks = self._named_keyset()
+        res = ks.verify_requests(bodies) if ks is not None and bodies else [(_abi.VREQ_HOST, b"")] * len(bodies)
+        out = []
+        for raw, (st, body) in zip(bodies, res):
+            if st == _abi.VREQ_HOST:
+                out.append(self._verify_request_host(raw))
+            else:
+                out.append((400 if st == _abi.VREQ_BAD_REQUEST else 200, body))
+        return out
+
+    def _verify_request_host(self, raw):
+        """One request body through the handler on the host: ShouldBindJSON, VerifyVC, c.JSON."""
+        try:
+            v = _bind_verify_request(raw)
+        except ValueError:
+            return 400, b'{"error":"Invalid request body"}'
+        if v is _ABSENT:
+            return 200, _response_bytes(_vc_response(False, error="failed to parse VC document: unexpected end of JSON input"))
+        if v is None:
+            d = _zero(_VC_DOC)                            # json.Unmarshal of null leaves the zero document
+        elif not isinstance(v, _Obj):
+            what = "string" if isinstance(v, str) else "bool" if isinstance(v, bool) else "array" if isinstance(v, list) else "number"
+            return 200, _response_bytes(_vc_response(
+                False, error="failed to parse VC document: json: cannot unmarshal %s into Go value of type types.VCDocument" % what))
+        else:
+            try:
+                d = _go_into(v, _VC_DOC, _zero(_VC_DOC))
+            except ValueError as ex:
+                return 200, _response_bytes(_vc_response(False, error="failed to parse VC document: %s" % ex))
+        if d["issuer"] not in self.keys._index:
+            return 200, _response_bytes(_vc_response(False, error="failed to resolve issuer DID: DID not found: %s" % d["issuer"]))
+        pv = d["proof"]["proofValue"]
+        v = self._keyed_verify([d["issuer"]], [go_json.vc_document(d)], [pv])[0]
+        if v is None:
+            r = _vc_response(False, error="failed to verify signature: failed to decode signature: illegal base64 data at input byte %d"
+                             % _b64url_error_at(pv))
+        elif v:
+            r = _vc_response(True, message="VC verified successfully", issuer_did=d["issuer"], issued_at=d["issuanceDate"])
+        else:
+            r = _vc_response(False, message="Invalid signature")
+        return 200, _response_bytes(r)
+
     # -- comprehensive audit (vc_service.go:926-1005, 1008-1359, 1386-1644)
     def _audit_component(self, ev, doc, verdict, integrity, security, compliance):
         """The checks of one execution VC against its record (performIntegrityChecks, performSecurityAnalysis with
@@ -922,6 +970,58 @@ def _b64url_error_at(s: str) -> int:
     import re
     m = re.search(r"[^A-Za-z0-9_-]", s)
     return m.start() if m else len(s) - 1
+
+
+def _response_bytes(r) -> bytes:
+    """json.Marshal(types.VCVerificationResponse) of a _vc_response dict: field order, omitempty, Go's escaping."""
+    out = '{"valid":%s' % ("true" if r["valid"] else "false")
+    for key, name in (("issuer_did", "issuer_did"), ("issued_at", "issued_at"), ("message", "message"), ("error", "error")):
+        if r[key]:
+            out += ',"%s":%s' % (name, go_json.string(r[key]))
+    return (out + "}").encode("utf-8", "surrogatepass")
+
+
+_ABSENT = object()
+
+
+def _go_fold(name: str) -> str:
+    """encoding/json's foldName: ASCII letters upper-cased, every other rune mapped through ToUpper(ToLower(r))."""
+    out = []
+    for ch in name:
+        if ch < "\x80":
+            out.append(ch.upper() if "a" <= ch <= "z" else ch)
+        else:
+            f = ch.lower()
+            f = f.upper() if len(f) == 1 else ch
+            out.append(f if len(f) == 1 else ch)
+    return "".join(out)
+
+
+def _bind_verify_request(raw: bytes):
+    """c.ShouldBindJSON(&types.VCVerificationRequest) with gin's default decoder: the first JSON value of the body (what follows it is not
+    read), which must be an object or null.  Returns the decoded vc_document value (the last member whose name matches it exactly or
+    folded), _ABSENT when there is none; raises ValueError where the bind fails."""
+    text = raw.decode("utf-8", "surrogateescape")
+    i = 0
+    while i < len(text) and text[i] in " \t\n\r":
+        i += 1
+
+    def no_constants(name):
+        raise ValueError("invalid character in numeric literal: %s" % name)
+    try:
+        v, _ = json.JSONDecoder(object_pairs_hook=_Obj, parse_constant=no_constants).raw_decode(text, i)
+    except ValueError:
+        raise ValueError("invalid request body")
+    if v is None:
+        return _ABSENT
+    if not isinstance(v, _Obj):
+        raise ValueError("json: cannot unmarshal into Go value of type types.VCVerificationRequest")
+    want = _go_fold("vc_document")
+    found = _ABSENT
+    for k, x in v:
+        if k == "vc_document" or _go_fold(k) == want:
+            found = x
+    return found
 
 
 class _Obj(list):

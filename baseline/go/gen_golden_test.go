@@ -24,6 +24,7 @@
 package afcgolden
 
 import (
+	"bytes"
 	"crypto/ed25519"
 	"crypto/hmac"
 	"crypto/sha256"
@@ -32,6 +33,7 @@ import (
 	"encoding/binary"
 	"encoding/hex"
 	"encoding/json"
+	"fmt"
 	"math"
 	"os"
 	"path/filepath"
@@ -428,6 +430,52 @@ func TestPinGolden(t *testing.T) {
 			m.Write(body)
 			check(t, "webhook_cases.json", c.ExecutionId, "header", "sha256="+hex.EncodeToString(m.Sum(nil)), *c.ExpectHeader)
 		}
+	}
+	// ---------------- verify_request_cases.json: POST /api/v1/did/verify on raw bodies — gin's default ShouldBindJSON
+	// (json.NewDecoder(body).Decode), VCService.VerifyVC (internal/services/vc_service.go:242-289) against the fixture's registry, and
+	// c.JSON's json.Marshal of the response
+	var vr struct {
+		Registry []struct{ Did, Pk string }
+		Cases    []struct {
+			Name         string `json:"name"`
+			BodyHex      string `json:"body_hex"`
+			ExpectStatus int    `json:"expect_status"`
+			ExpectBody   string `json:"expect_body"`
+		}
+	}
+	load(t, "verify_request_cases.json", &vr)
+	vrKeys := map[string][]byte{}
+	for _, r := range vr.Registry {
+		vrKeys[r.Did] = unhex(t, r.Pk)
+	}
+	for _, c := range vr.Cases {
+		status, body := 200, []byte(nil)
+		var req types.VCVerificationRequest
+		if err := json.NewDecoder(bytes.NewReader(unhex(t, c.BodyHex))).Decode(&req); err != nil {
+			status, body = 400, []byte(`{"error":"Invalid request body"}`)
+		} else {
+			res := types.VCVerificationResponse{}
+			var vc types.VCDocument
+			if err := json.Unmarshal(req.VCDocument, &vc); err != nil {
+				res.Error = fmt.Sprintf("failed to parse VC document: %v", err)
+			} else if pk, ok := vrKeys[vc.Issuer]; !ok {
+				res.Error = fmt.Sprintf("failed to resolve issuer DID: DID not found: %s", vc.Issuer)
+			} else {
+				cp := vc
+				cp.Proof = types.VCProof{}
+				canonical, _ := json.Marshal(cp)
+				if sig, err := base64.RawURLEncoding.DecodeString(vc.Proof.ProofValue); err != nil {
+					res.Error = fmt.Sprintf("failed to verify signature: failed to decode signature: %v", err)
+				} else if !verifyRecover(pk, canonical, sig) {
+					res.Message = "Invalid signature"
+				} else {
+					res = types.VCVerificationResponse{Valid: true, IssuerDID: vc.Issuer, IssuedAt: vc.IssuanceDate, Message: "VC verified successfully"}
+				}
+			}
+			body, _ = json.Marshal(res)
+		}
+		check(t, "verify_request_cases.json", c.Name, "status", fmt.Sprint(status), fmt.Sprint(c.ExpectStatus))
+		check(t, "verify_request_cases.json", c.Name, "body", string(body), c.ExpectBody)
 	}
 	// ---------------- write go_pinned.json
 	doc := map[string]interface{}{"go": runtime.Version(), "failed": t.Failed(), "entries": out}

@@ -197,6 +197,42 @@ int afc_vc_verify_json_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const u
 int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                  uint8_t* d_status, uint32_t* d_fields, void* stream);
 
+/* ---- VC verification requests answered in one call: POST /api/v1/did/verify (DIDHandlers.VerifyVC, internal/handlers/did_handlers.go:97-111)
+ * and POST /api/ui/v1/vc/verify (internal/handlers/ui/did.go:442-469), through VCService.VerifyVC (internal/services/vc_service.go:242-289),
+ * for n raw request bodies.  reqs[req_off[i] .. req_off[i+1]) is body i as the client sent it; the call writes state[i], which fixes the HTTP
+ * status, and bodies[body_off[i] .. body_off[i+1]), the bytes c.JSON writes (json.Marshal, HTML escaping on, no trailing newline):
+ *   AFC_VREQ_OK           200.  json.Marshal(types.VCVerificationResponse) for:
+ *                         no vc_document, or a top-level null  {"valid":false,"error":"failed to parse VC document: unexpected end of JSON input"}
+ *                         "vc_document":null                   {"valid":false,"error":"failed to resolve issuer DID: DID not found: "}
+ *                         an object, the verdict of afc_vc_verify_json_batch on exactly its bytes (AFC_DOC_EXECUTION_VC):
+ *                           VALID         {"valid":true,"issuer_did":I,"issued_at":D,"message":"VC verified successfully"}, each of I / D
+ *                                         omitted when empty
+ *                           INVALID       {"valid":false,"message":"Invalid signature"}
+ *                           UNRESOLVED    {"valid":false,"error":"failed to resolve issuer DID: DID not found: " + I}
+ *                           BAD_ENCODING  {"valid":false,"error":"failed to verify signature: failed to decode signature: illegal base64 data at
+ *                                         input byte " + k}, k the first byte of proofValue outside the URL alphabet, else its last byte
+ *   AFC_VREQ_BAD_REQUEST  400.  {"error":"Invalid request body"}: the body holds no JSON value, its first value is not JSON as Go's scanner
+ *                         reads it (the whole value is scanned, bytes after it are not), or that value is an array, string, number or bool.
+ *                         The UI route adds "details": err.Error() to its 400 body; its caller builds that body itself.
+ *   AFC_VREQ_HOST         a zero-length body: the caller runs the handler itself.  A vc_document that is a string, number, array or bool; an
+ *                         object afc_vc_verify_json_batch gives AFC_VC_HOST; a null one when the key set holds the DID ""; a top-level
+ *                         member name with an escape or a byte >= 0x80; nesting deeper than 64.
+ * The member vc_document is matched as Go matches a struct field: the exact name, else any ASCII-case-insensitive spelling; the last one
+ * wins.  I and D are the decoded issuer and issuanceDate written with json.Marshal's escaping.  ks is a named key set (afc_keyset_new_named),
+ * else AFC_ESTATE.  bodies_cap must be at least afc_vc_verify_request_bound(req_off, n), additive over requests and computed from req_off[0]
+ * and req_off[n] alone (a constant per request plus 6 bytes per request byte); else AFC_EINVAL before any work.  Other AFC_EINVAL: a NULL
+ * pointer, a key set of another context, a request of 2^31 bytes or more, offsets that run backwards.  The host-buffer call streams chunks
+ * of whole requests through the context's staging ring; the _dev call synchronises `stream` once, to read the ends of req_off and whether
+ * any request breaks those two rules.  n = 0 writes body_off[0] = 0 in the host-buffer call and nothing in the _dev call. */
+#define AFC_VREQ_OK 0
+#define AFC_VREQ_BAD_REQUEST 1
+#define AFC_VREQ_HOST 2
+uint64_t afc_vc_verify_request_bound(const uint64_t* req_off, uint32_t n);
+int afc_vc_verify_request_batch(afc_ctx* ctx, afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off /* n+1 */, uint32_t n,
+                                uint8_t* bodies, uint64_t bodies_cap, uint64_t* body_off /* n+1 */, uint8_t* state /* n */);
+int afc_vc_verify_request_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint8_t* d_reqs, const uint64_t* d_req_off, uint32_t n,
+                                    uint8_t* d_bodies, uint64_t bodies_cap, uint64_t* d_body_off, uint8_t* d_state, void* stream);
+
 /* ---- stored credentials audited against their records on the device ---------------------------------------------------------
  * replaces, per credential, the checks of VCService.VerifyExecutionVCComprehensive (internal/services/vc_service.go:926-1005):
  * json.Unmarshal, performIntegrityChecks (:1008-1181), performSecurityAnalysis (:1184-1233) and performComplianceChecks

@@ -10,6 +10,8 @@ measures webhook deliveries built and signed in one call (afc_webhook_sign_batch
 The issue_workflow block measures workflow credentials issued in one call (afc_vc_issue_workflow_batch[_dev]) next to the host-built path.
 The reregister block measures known agents re-registered in one call (afc_did_reregister_batch[_dev]) in a restart storm.
 The resolve block measures DID resolution and DID documents served in one call (afc_did_resolve_batch[_dev]) from a 2^20-DID directory.
+The verify_request block measures VC verification requests answered in one call (afc_vc_verify_request_batch[_dev]) next to the
+json-verify call on the same documents.
 Needs a CUDA device; writes nothing.
 usage: python tools/bench_stored_vc.py [--reps R] [--only BLOCK]"""
 import argparse
@@ -926,13 +928,156 @@ def resolve_block(ctx, dev, timed):
             "host_mirror": {"requests": len(sample), "ms": ms_mirror, "requests_per_s": len(sample) / (ms_mirror * 1e-3)}}
 
 
+def _tile_dev(variants, choose, n, dev):
+    """n byte strings on the device without building them on the host: item j is variants[v][j % m] with v = choose(j0, m) for the rep of m
+    items that starts at j0.  variants: lists of m byte strings each.  Returns (d_bytes uint8, d_off int64 [n+1])."""
+    import torch
+    m = len(variants[0])
+    bufs, offs = [], []
+    for v in variants:
+        lens = np.array([len(b) for b in v], dtype=np.int64)
+        off = np.zeros(m + 1, dtype=np.int64)
+        np.cumsum(lens, out=off[1:])
+        bufs.append(torch.from_numpy(np.frombuffer(b"".join(v), dtype=np.uint8).copy()).to(dev))
+        offs.append(off)
+    lens_all = np.empty(n, dtype=np.int64)
+    picks = []
+    for j0 in range(0, n, m):
+        c = choose(j0, m)[:n - j0]
+        picks.append(c)
+        lens_all[j0:j0 + len(c)] = np.stack([np.diff(o) for o in offs])[c, np.arange(len(c))]
+    d_off = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(lens_all, out=d_off[1:])
+    d_bytes = torch.empty(int(d_off[-1]), dtype=torch.uint8, device=dev)
+    for r, c in enumerate(picks):
+        j0 = r * m
+        for v in range(len(variants)):
+            sel = np.nonzero(c == v)[0]
+            if not len(sel):
+                continue
+            src_start = torch.from_numpy(offs[v][sel]).to(dev)
+            ln = torch.from_numpy(np.diff(offs[v])[sel]).to(dev)
+            dst_start = torch.from_numpy(d_off[j0 + sel]).to(dev)
+            owner = torch.repeat_interleave(torch.arange(len(sel), device=dev), ln)
+            first = torch.cumsum(ln, 0) - ln
+            pos = torch.arange(int(ln.sum()), device=dev) - first[owner]
+            d_bytes[dst_start[owner] + pos] = bufs[v][src_start[owner] + pos]
+    return d_bytes, torch.from_numpy(d_off).to(dev)
+
+
+def verify_request_block(ctx, dev, timed):
+    """VC verification requests answered on the device (afc_vc_verify_request_batch): 2^20 raw request bodies of POST /api/v1/did/verify
+    from 1024 issuers, half as the Python SDK sends them (requests' json.dumps of {"vc_document": doc}) and half as the web UI does
+    (JSON.stringify, compact); 1 % with a corrupted signature, 1 % naming an issuer outside the registry, 0.1 % malformed bodies (the
+    opening brace turned into a bracket).  2^14 distinct documents are built on the device, wrapped on the host with every number token
+    kept, and tiled to 2^20 on the device.  Reported: the _dev call with its per-kernel split and the bytes of the bodies it writes,
+    host_fallback (requests left to the host) and all_expected (each state and response class is the planted one), the json-verify
+    call (afc_vc_verify_json_batch_dev) on the unwrapped documents in the same run, and the host-buffer call from pinned memory."""
+    import torch
+    from agentfield_b200 import _abi
+    from agentfield_b200 import canonical as CA
+    from agentfield_b200 import respell as R
+    from agentfield_b200.identity import ExpandedKeys, KeySet
+    n, K, m = 1 << 20, 1024, 1 << 14
+    rng = np.random.default_rng(0xAF0E)
+    cache = ExpandedKeys(ctx)
+    dids = cache.derive(rng.integers(0, 256, 32, dtype=np.uint8).tobytes(), ["m/44'/%d'/0'" % (7000 + a) for a in range(K)])
+    d_exp = torch.from_numpy(cache._expanded).to(dev)
+    d_ki = (torch.arange(m, device=dev) % K).to(torch.int32)
+    d_docs, d_doff, _, _, _ = CA.synthetic_stored_vcs_dev(ctx, d_exp, dids, d_ki, m, seed=0xAF0E)
+    buf, off = d_docs.cpu().numpy(), d_doff.cpu().numpy()
+    docs = [buf[off[i]:off[i + 1]].tobytes() for i in range(m)]
+    del d_docs, d_doff
+
+    def corrupt(d):                                   # one base64 character of proofValue changed: still 86 characters
+        k = d.index(b'"proofValue"') + 20
+        return d[:k] + (b"B" if d[k:k + 1] == b"A" else b"A") + d[k + 1:]
+
+    def foreign(d):                                   # the issuer's last character changed: a DID the registry does not hold
+        k = d.index(b'"issuer":"') + 10
+        e = d.index(b'"', k) - 1
+        return d[:e] + (b"Q" if d[e:e + 1] != b"Q" else b"R") + d[e + 1:]
+    kinds = {"ok": docs, "bad_sig": [corrupt(d) for d in docs], "foreign": [foreign(d) for d in docs]}
+    wrap = lambda d: ("obj", [("vc_document", R.parse_keep(d))])     # noqa: E731
+    sdk = {k: [R.SPELLINGS["dumps"](wrap(d)).encode("utf-8") for d in v] for k, v in kinds.items()}
+    ui = {k: [R.write(wrap(d), esc=R._esc_js).encode("utf-8") for d in v] for k, v in kinds.items()}
+    malformed = [b"[" + b[1:] for b in sdk["ok"]]
+    order = ["ok", "bad_sig", "foreign"]
+    variants = [sdk[k] for k in order] + [ui[k] for k in order] + [malformed]
+
+    def plan(j0, cnt):
+        j = np.arange(j0, j0 + cnt)
+        v = np.where(j % 100 == 37, 1, np.where(j % 100 == 53, 2, 0)) + 3 * ((j // m) % 2)
+        return np.where(j % 1000 == 777, 6, v)
+    d_reqs, d_off = _tile_dev(variants, plan, n, dev)
+    d_vdocs, d_voff = _tile_dev([[s[len(b'{"vc_document": '):-1] for s in sdk[k]] for k in order] * 2 + [kinds["ok"]],
+                                lambda j0, c: plan(j0, c), n, dev)
+    v_all = plan(0, n)
+    ks = KeySet([cache.public_key(d) for d in dids], ctx, dids=dids)
+    run = lambda: ks.verify_requests_dev(d_reqs, d_off, n)             # noqa: E731
+    bodies, body_off, state = run()
+    torch.cuda.synchronize()
+    total = int(body_off[n])
+    st = state.cpu().numpy()
+    want_state = np.where(v_all == 6, _abi.VREQ_BAD_REQUEST, _abi.VREQ_OK)
+    prefixes = [b'{"valid":true,"issuer_did":"di', b'{"valid":false,"message":"Inva', b'{"valid":false,"error":"failed', b'{"error":"Invalid request body']
+    cls = np.where(v_all == 6, 3, v_all % 3)
+    starts = body_off[:-1]
+    head = torch.stack([bodies[starts + k] for k in range(30)], 1).cpu().numpy()
+    want_head = np.frombuffer(b"".join(prefixes), dtype=np.uint8).reshape(4, 30)[cls]
+    all_expected = bool(np.array_equal(st, want_state) and np.array_equal(head, want_head))
+    del bodies, body_off, state, head
+    ms = timed(run)
+    ctx.profile_begin()
+    timed(run, reps=3)
+    kms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    d_vst = torch.empty(n, dtype=torch.uint8, device=dev)
+    jrun = lambda: ks.verify_json_dev(0, d_vdocs, d_voff, n, d_vst)    # noqa: E731
+    ms_json = timed(jrun)
+    ctx.profile_begin()
+    timed(jrun, reps=3)
+    jkms = {k: v["avg_ms"] for k, v in ctx.profile_end().items()}
+    want_json = np.where(v_all % 3 == 1, _abi.VC_INVALID, np.where(v_all % 3 == 2, _abi.VC_UNRESOLVED, _abi.VC_VALID))
+    want_json[v_all == 6] = _abi.VC_VALID
+    json_expected = bool(np.array_equal(d_vst.cpu().numpy(), want_json))
+    lib = _abi.load()
+    keep = []
+
+    def pin(a):
+        p = lib.afc_alloc_pinned(max(a.nbytes, 1))
+        h = np.frombuffer((ctypes.c_uint8 * max(a.nbytes, 1)).from_address(p), dtype=np.uint8)[:a.nbytes].view(a.dtype)
+        h[...] = a
+        keep.append(p)
+        return h
+    h_reqs, h_off = pin(d_reqs.cpu().numpy()), pin(d_off.cpu().numpy().view(np.uint64))
+    ks.verify_requests_packed(h_reqs, h_off)
+    t_0 = time.perf_counter()
+    for _ in range(2):
+        hb, _, hs = ks.verify_requests_packed(h_reqs, h_off)
+    ms_host = (time.perf_counter() - t_0) / 2 * 1e3
+    host_same = bool(np.array_equal(hs, st) and len(hb) == total)
+    del hb
+    for p in keep:
+        lib.afc_free_pinned(p)
+    ks.close()
+    gpu = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    return {"gpu": gpu, "requests": n, "issuers": K, "request_bytes": int(d_off[-1]),
+            "dev_call": {"ms": ms, "requests_per_s": n / (ms * 1e-3), "body_bytes": total, "kernels_ms": kms,
+                         "host_fallback": int((st == _abi.VREQ_HOST).sum()), "bad_request": int((st == _abi.VREQ_BAD_REQUEST).sum()),
+                         "all_expected": all_expected},
+            "verify_json_dev_call": {"ms": ms_json, "docs_per_s": n / (ms_json * 1e-3), "kernels_ms": jkms, "all_expected": json_expected,
+                                     "note": "afc_vc_verify_json_batch_dev on the unwrapped documents"},
+            "host_call": {"ms": ms_host, "requests_per_s": n / (ms_host * 1e-3), "same_as_dev": host_same, "note": "pinned buffers"}}
+
+
 def main():
     import torch
     import agentfield_b200 as afb
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--only", choices=["stored_vc_verify", "audit_stored", "verify_json", "issue_execution", "webhook", "issue_workflow", "register",
-                                        "reregister", "chain", "resolve"],
+                                        "reregister", "chain", "resolve", "verify_request"],
                     default=None,
                     help="run one block")
     args = ap.parse_args()
@@ -949,7 +1094,7 @@ def main():
         return e0.elapsed_time(e1) / reps
     blocks = {"stored_vc_verify": stored_vc_block, "audit_stored": audit_stored_block, "verify_json": verify_json_block,
               "issue_execution": issue_execution_block, "webhook": webhook_block, "issue_workflow": issue_workflow_block, "register": register_block,
-              "reregister": reregister_block, "chain": chain_block, "resolve": resolve_block}
+              "reregister": reregister_block, "chain": chain_block, "resolve": resolve_block, "verify_request": verify_request_block}
     print(json.dumps({k: f(ctx, dev, timed) for k, f in blocks.items() if args.only in (None, k)}), flush=True)
     ctx.close()
 
