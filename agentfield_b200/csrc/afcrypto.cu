@@ -365,16 +365,25 @@ struct Carve {
     }
     template <class T> T* take(size_t count, bool secret = false) { return (T*)take(count * sizeof(T), secret); }
 };
-// A _dev call's scratch: sized by the layout, allocated from the stream-ordered pool, carved by the same layout (the caller frees it)
-template <class Layout> cudaError_t pool_carve(uint8_t** scratch, cudaStream_t st, Layout&& layout) {
+// A _dev call's scratch: sized by the layout, allocated from the stream-ordered pool and carved by the same layout; enq() runs on it, then
+// every region taken as secret is zeroed and the scratch freed, so nothing secret outlives the call.  Returns the first error.
+template <class Layout, class Enq> int dev_scratch(afc_ctx* ctx, cudaStream_t st, Layout&& layout, Enq&& enq) {
     Carve m;
     layout(m);
-    const cudaError_t e = cudaMallocAsync((void**)scratch, m.used, st);
-    if (e != cudaSuccess) return e;
+    uint8_t* scratch = nullptr;
+    CK(cudaMallocAsync((void**)&scratch, m.used, st));
+    Regions secrets;
     Carve k;
-    k.base = *scratch;
+    k.base = scratch; k.secrets = &secrets;
     layout(k);
-    return cudaSuccess;
+    cudaError_t e = enq();
+    for (const auto& s : secrets) {
+        const cudaError_t w = cudaMemsetAsync(s.first, 0, s.second, st);
+        if (e == cudaSuccess) e = w;
+    }
+    cudaFreeAsync(scratch, st);
+    CK(e);
+    return AFC_OK;
 }
 
 // ---- stored credential documents: parse -> scan -> emit -> keyed verify -> fold, in one scratch area
@@ -437,6 +446,11 @@ bool monotone(const T* off, uint64_t n) { return monotone(off, 0, n); }
 
 // the byte or item count between two ends, 0 for a backwards range
 uint64_t span(uint64_t a, uint64_t b) { return b >= a ? b - a : 0; }
+// the ends of a host-buffer call's offset arrays (offset_ends): the words its _dev form reads with read_ends, and its public bound
+const uint64_t* host_ends(const launch::OffsetSpans& S, uint32_t n, uint64_t* ends) {
+    offset_ends(S.s, S.k, n, ends);
+    return ends;
+}
 
 // Runs enq(d_ends) on the stream into `words` words of device scratch, copies them to ends and synchronises once
 template <class F>
@@ -451,19 +465,21 @@ int gather_ends(afc_ctx* ctx, uint64_t* ends, size_t words, cudaStream_t st, F&&
     return AFC_OK;
 }
 // The ends of a _dev call's offset arrays (offset_ends), read with one synchronisation: each word of a call with direct spans only is
-// copied as it is; a call with an indirect span, whose indices are device words too, gathers them with one thread of k_offset_ends.
+// copied as it is; a call with an indirect span, whose indices are device words too, gathers them with one thread of k_offset_ends.  Any
+// backwards range is AFC_EINVAL.
 int read_ends(afc_ctx* ctx, const launch::OffsetSpans& S, uint32_t n, uint64_t* ends, cudaStream_t st) {
     bool direct = true;
     for (int j = 0; j < S.k; j++) direct = direct && S.s[j].via < 0;
     if (!direct) {
         CallLog lc(ctx);
-        return gather_ends(ctx, ends, 2 * (size_t)S.k, st, [&](uint64_t* d_ends) { return launch::offset_ends(S, n, d_ends, st, lc); });
+        RC(gather_ends(ctx, ends, 2 * (size_t)S.k, st, [&](uint64_t* d_ends) { return launch::offset_ends(S, n, d_ends, st, lc); }));
     }
-    for (int j = 0; j < S.k; j++) {
+    for (int j = 0; direct && j < S.k; j++) {
         CK(cudaMemcpyAsync(&ends[2 * j], S.s[j].off, 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(&ends[2 * j + 1], S.s[j].off + (size_t)S.s[j].stride * n, 8, cudaMemcpyDeviceToHost, st));
     }
-    CK(cudaStreamSynchronize(st));
+    if (direct) CK(cudaStreamSynchronize(st));
+    for (int j = 0; j < S.k; j++) if (ends[2 * j + 1] < ends[2 * j]) return AFC_EINVAL;
     return AFC_OK;
 }
 
@@ -1366,44 +1382,59 @@ int afc_keyset_new_named(afc_ctx* ctx, const uint8_t* pks, const uint8_t* dids, 
     ks->named = true;
     return AFC_OK;
 }
-static int vc_stored_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, uint8_t* status) {
+// The stored, JSON and audit calls (how) share their arguments; the audit adds issues, and columns exactly for execution documents.  A keyset
+// without DIDs is AFC_ESTATE, after every AFC_EINVAL.
+enum class Vc { stored, json, audit };
+static int vc_stored_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                           const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues, Vc how) {
     if (!ctx || !ks || ks->ctx != ctx || !doc_off || (n && (!docs || !status))) return AFC_EINVAL;
     if (doc_kind != AFC_DOC_EXECUTION_VC && doc_kind != AFC_DOC_WORKFLOW_VC) return AFC_EINVAL;
+    if (how == Vc::audit && ((n && !issues) || (doc_kind == AFC_DOC_EXECUTION_VC ? (!col_off || (n && !cols)) : (cols || col_off)))) return AFC_EINVAL;
     if (!ks->named) return AFC_ESTATE;
     return AFC_OK;
 }
-// the host-buffer form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
-static int vc_verify_host(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n, uint8_t* status,
-                          uint32_t* fields, bool json) {
-    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
+// the host-buffer form of the stored, JSON and audit calls
+static int vc_stored_host(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                          const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* fields, uint32_t* issues, Vc how) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, cols, col_off, n, status, issues, how);
     if (rc != AFC_OK || n == 0) return rc;
+    const uint32_t C = AFC_AUDIT_COLUMNS;
     CK(cudaSetDevice(ctx->device));
     Ring ring(ctx);
-    return ring.walk(n, msg_bytes(doc_off), [&](Ring& r) {
+    auto measure = [&](uint32_t i0, uint32_t i) {
+        if (col_off) for (uint32_t k = 0; k < C; k++) if (col_off[(size_t)i * C + k + 1] < col_off[(size_t)i * C + k]) return kBadOffsets;
+        return msg_bytes(doc_off)(i0, i);
+    };
+    return ring.walk(n, measure, [&](Ring& r) {
         Msgs D;
+        const uint8_t* d_cols = nullptr;
+        const uint64_t* d_coff = nullptr;
         uint8_t* d_status;
-        uint32_t* d_fields = nullptr;
+        uint32_t *d_fields = nullptr, *d_issues = nullptr;
         VcScratch S;
         RC(r.stage([&](Stager& k) {
             D = stage_msgs(k, docs, doc_off, r.i0, r.cnt);
+            if (col_off) {
+                const uint64_t cbase = col_off[(size_t)r.i0 * C];
+                d_cols = k.in_at(cols, cbase, col_off[(size_t)(r.i0 + r.cnt) * C] - cbase, 16);
+                d_coff = k.in(col_off, (size_t)r.i0 * C, (size_t)r.cnt * C + 1);
+            }
             d_status = k.take((size_t)r.cnt + 16);
             if (fields) d_fields = k.take<uint32_t>((size_t)r.cnt * 4 + 4);
-            vc_scratch(k, S, r.cnt, doc_off[r.i0 + r.cnt] - doc_off[r.i0], ks->n_keys, false);
+            if (how == Vc::audit) d_issues = k.take<uint32_t>((size_t)r.cnt + 4);
+            vc_scratch(k, S, r.cnt, doc_off[r.i0 + r.cnt] - doc_off[r.i0], ks->n_keys, how == Vc::audit);
         }));
-        CK(vc_stored_enqueue(ctx, ks, doc_kind, D.d, D.off, r.cnt, d_status, d_fields, S, r.st, r.lc, nullptr, nullptr, nullptr, json));
-        return r.copy_back({{status, r.i0, d_status, r.cnt}, {fields, (size_t)r.i0 * 16, d_fields, fields ? (size_t)r.cnt * 16 : 0}});
+        CK(vc_stored_enqueue(ctx, ks, doc_kind, D.d, D.off, r.cnt, d_status, d_fields, S, r.st, r.lc, d_issues, d_cols, d_coff, how == Vc::json));
+        return r.copy_back({{status, r.i0, d_status, r.cnt}, {fields, (size_t)r.i0 * 16, d_fields, fields ? (size_t)r.cnt * 16 : 0},
+                            {issues, (size_t)r.i0 * 4, d_issues, d_issues ? (size_t)r.cnt * 4 : 0}});
     });
-}
-int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
-                               uint8_t* status, uint32_t* fields) {
-    return vc_verify_host(ctx, ks, doc_kind, docs, doc_off, n, status, fields, false);
 }
 // the offset arrays whose ends bound a stored, JSON or audit call
 static launch::OffsetSpans doc_spans(const uint64_t* doc_off) { return {{{doc_off, 1, -1}}, 1}; }
-// the _dev form of afc_vc_verify_stored_batch (json = false) and afc_vc_verify_json_batch (json = true)
-static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n, uint8_t* d_status,
-                         uint32_t* d_fields, void* stream, bool json) {
-    int rc = vc_stored_check(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status);
+// the _dev form of the stored, JSON and audit calls
+static int vc_stored_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
+                         const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_fields, uint32_t* d_issues, void* stream, Vc how) {
+    int rc = vc_stored_check(ctx, ks, doc_kind, d_docs, d_doc_off, d_cols, d_col_off, n, d_status, d_issues, how);
     if (rc != AFC_OK || n == 0) return rc;
     if (d_fields && !aligned16(d_fields)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
@@ -1411,38 +1442,49 @@ static int vc_verify_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8
     cudaStream_t st = (cudaStream_t)stream;
     uint64_t ends[2];                       // the batch's byte size bounds the message buffer
     RC(read_ends(ctx, doc_spans(d_doc_off), n, ends, st));
-    if (ends[1] < ends[0]) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
     VcScratch S;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { vc_scratch(k, S, n, ends[1] - ends[0], ks->n_keys, false); }));
-    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, S, st, lc, nullptr, nullptr, nullptr, json);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    return dev_scratch(ctx, st, [&](Carve& k) { vc_scratch(k, S, n, ends[1] - ends[0], ks->n_keys, how == Vc::audit); }, [&] {
+        return vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, S, st, lc, d_issues, d_cols, d_col_off, how == Vc::json);
+    });
+}
+int afc_vc_verify_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                               uint8_t* status, uint32_t* fields) {
+    return vc_stored_host(ctx, ks, doc_kind, docs, doc_off, nullptr, nullptr, n, status, fields, nullptr, Vc::stored);
 }
 int afc_vc_verify_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                    uint8_t* d_status, uint32_t* d_fields, void* stream) {
-    return vc_verify_dev(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, stream, false);
+    return vc_stored_dev(ctx, ks, doc_kind, d_docs, d_doc_off, nullptr, nullptr, n, d_status, d_fields, nullptr, stream, Vc::stored);
 }
 
 // documents in any JSON spelling: the arguments, statuses and fields of afc_vc_verify_stored_batch
 int afc_vc_verify_json_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
                              uint8_t* status, uint32_t* fields) {
-    return vc_verify_host(ctx, ks, doc_kind, docs, doc_off, n, status, fields, true);
+    return vc_stored_host(ctx, ks, doc_kind, docs, doc_off, nullptr, nullptr, n, status, fields, nullptr, Vc::json);
 }
 int afc_vc_verify_json_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, uint32_t n,
                                  uint8_t* d_status, uint32_t* d_fields, void* stream) {
-    return vc_verify_dev(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, d_fields, stream, true);
+    return vc_stored_dev(ctx, ks, doc_kind, d_docs, d_doc_off, nullptr, nullptr, n, d_status, d_fields, nullptr, stream, Vc::json);
+}
+
+// audit: the arguments of afc_vc_verify_stored_batch, plus columns exactly for execution documents
+int afc_vc_audit_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
+                              const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
+    return vc_stored_host(ctx, ks, doc_kind, docs, doc_off, cols, col_off, n, status, nullptr, issues, Vc::audit);
+}
+int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
+                                  const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_issues, void* stream) {
+    return vc_stored_dev(ctx, ks, doc_kind, d_docs, d_doc_off, d_cols, d_col_off, n, d_status, nullptr, d_issues, stream, Vc::audit);
 }
 
 // ---------------------------------------------------------------------------------- VC verification requests
 // Per request the longest constant text of a response plus at most 6 bytes per request byte (issuer and issuanceDate re-escaped)
 static uint64_t vrq_bound(uint32_t n, uint64_t req_bytes) { return (uint64_t)n * launch::vrq_request_fixed() + 6 * req_bytes; }
+// the capacity a batch with these ends (doc_spans) needs
+static bool vrq_fits(const uint64_t* ends, uint32_t n, uint64_t cap) { return cap >= vrq_bound(n, span(ends[0], ends[1])); }
 uint64_t afc_vc_verify_request_bound(const uint64_t* req_off, uint32_t n) {
     if (!req_off || n == 0) return 0;
-    const launch::OffsetSpans S = doc_spans(req_off);
     uint64_t e[2];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(doc_spans(req_off), n, e);
     return vrq_bound(n, span(e[0], e[1]));
 }
 static int vrq_check(afc_ctx* ctx, afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, const uint8_t* bodies,
@@ -1489,16 +1531,13 @@ int afc_vc_verify_request_batch_dev(afc_ctx* ctx, afc_keyset* ks, const uint8_t*
         const cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
         return e == cudaSuccess ? launch::dres_ends(d_req_off, n, d_ends, st, lc) : e;
     }));
-    const uint64_t req_bytes = span(ends[0], ends[1]);
-    if (ends[2] || bodies_cap < vrq_bound(n, req_bytes)) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
+    if (ends[2] || !vrq_fits(ends, n, bodies_cap)) return AFC_EINVAL;
     VrqScratch S;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { vrq_scratch(k, S, n, req_bytes, ks->n_keys); }));
-    cudaError_t e = vrq_enqueue(ctx, ks, d_reqs, d_req_off, n, S, d_state, d_body_off, st, lc);
-    if (e == cudaSuccess) e = launch::vrq_emit(S.bind, S.status, S.fields, S.docs, S.doc_off, n, S.b64_at, d_body_off, d_bodies, st, lc);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    return dev_scratch(ctx, st, [&](Carve& k) { vrq_scratch(k, S, n, span(ends[0], ends[1]), ks->n_keys); }, [&] {
+        cudaError_t e = vrq_enqueue(ctx, ks, d_reqs, d_req_off, n, S, d_state, d_body_off, st, lc);
+        if (e == cudaSuccess) e = launch::vrq_emit(S.bind, S.status, S.fields, S.docs, S.doc_off, n, S.b64_at, d_body_off, d_bodies, st, lc);
+        return e;
+    });
 }
 
 int afc_vc_verify_request_batch(afc_ctx* ctx, afc_keyset* ks, const uint8_t* reqs, const uint64_t* req_off, uint32_t n, uint8_t* bodies,
@@ -1507,7 +1546,8 @@ int afc_vc_verify_request_batch(afc_ctx* ctx, afc_keyset* ks, const uint8_t* req
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
     if (!monotone(req_off, n)) return AFC_EINVAL;
     for (uint32_t i = 0; i < n; i++) if (req_off[i + 1] - req_off[i] > 0x7fffffffull) return AFC_EINVAL;     // 2^31 bytes
-    if (bodies_cap < afc_vc_verify_request_bound(req_off, n)) return AFC_EINVAL;
+    uint64_t ends[2];
+    if (!vrq_fits(host_ends(doc_spans(req_off), n, ends), n, bodies_cap)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     const uint64_t per = vrq_bound(1, 0);
     // chunks of whole requests, sized by what they stage (the requests, their gathered values and signing messages) and the most their
@@ -1539,67 +1579,6 @@ int afc_vc_verify_request_batch(afc_ctx* ctx, afc_keyset* ks, const uint8_t* req
     });
 }
 
-// audit: the arguments of afc_vc_verify_stored_batch, plus columns exactly for execution documents
-static int vc_audit_check(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
-                          const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
-    int rc = vc_stored_check(ctx, ks, doc_kind, docs, doc_off, n, status);
-    if (rc != AFC_OK && rc != AFC_ESTATE) return rc;
-    if (n && !issues) return AFC_EINVAL;
-    if (doc_kind == AFC_DOC_EXECUTION_VC ? (!col_off || (n && !cols)) : (cols || col_off)) return AFC_EINVAL;
-    return rc;
-}
-int afc_vc_audit_stored_batch(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* docs, const uint64_t* doc_off, const uint8_t* cols,
-                              const uint64_t* col_off, uint32_t n, uint8_t* status, uint32_t* issues) {
-    int rc = vc_audit_check(ctx, ks, doc_kind, docs, doc_off, cols, col_off, n, status, issues);
-    if (rc != AFC_OK || n == 0) return rc;
-    const uint32_t C = AFC_AUDIT_COLUMNS;
-    CK(cudaSetDevice(ctx->device));
-    Ring ring(ctx);
-    auto measure = [&](uint32_t i0, uint32_t i) {
-        if (col_off) for (uint32_t k = 0; k < C; k++) if (col_off[(size_t)i * C + k + 1] < col_off[(size_t)i * C + k]) return kBadOffsets;
-        return msg_bytes(doc_off)(i0, i);
-    };
-    return ring.walk(n, measure, [&](Ring& r) {
-        Msgs D;
-        const uint8_t* d_cols = nullptr;
-        const uint64_t* d_coff = nullptr;
-        uint8_t* d_status;
-        uint32_t* d_issues;
-        VcScratch S;
-        RC(r.stage([&](Stager& k) {
-            D = stage_msgs(k, docs, doc_off, r.i0, r.cnt);
-            if (col_off) {
-                const uint64_t cbase = col_off[(size_t)r.i0 * C];
-                d_cols = k.in_at(cols, cbase, col_off[(size_t)(r.i0 + r.cnt) * C] - cbase, 16);
-                d_coff = k.in(col_off, (size_t)r.i0 * C, (size_t)r.cnt * C + 1);
-            }
-            d_status = k.take((size_t)r.cnt + 16);
-            d_issues = k.take<uint32_t>((size_t)r.cnt + 4);
-            vc_scratch(k, S, r.cnt, doc_off[r.i0 + r.cnt] - doc_off[r.i0], ks->n_keys, true);
-        }));
-        CK(vc_stored_enqueue(ctx, ks, doc_kind, D.d, D.off, r.cnt, d_status, nullptr, S, r.st, r.lc, d_issues, d_cols, d_coff));
-        return r.copy_back({{status, r.i0, d_status, r.cnt}, {issues, (size_t)r.i0 * 4, d_issues, (size_t)r.cnt * 4}});
-    });
-}
-int afc_vc_audit_stored_batch_dev(afc_ctx* ctx, afc_keyset* ks, int doc_kind, const uint8_t* d_docs, const uint64_t* d_doc_off, const uint8_t* d_cols,
-                                  const uint64_t* d_col_off, uint32_t n, uint8_t* d_status, uint32_t* d_issues, void* stream) {
-    int rc = vc_audit_check(ctx, ks, doc_kind, d_docs, d_doc_off, d_cols, d_col_off, n, d_status, d_issues);
-    if (rc != AFC_OK || n == 0) return rc;
-    CK(cudaSetDevice(ctx->device));
-    CallLog lc(ctx);
-    cudaStream_t st = (cudaStream_t)stream;
-    uint64_t ends[2];                       // the batch's byte size bounds the message buffer
-    RC(read_ends(ctx, doc_spans(d_doc_off), n, ends, st));
-    if (ends[1] < ends[0]) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
-    VcScratch S;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { vc_scratch(k, S, n, ends[1] - ends[0], ks->n_keys, true); }));
-    cudaError_t e = vc_stored_enqueue(ctx, ks, doc_kind, d_docs, d_doc_off, n, d_status, nullptr, S, st, lc, d_issues, d_cols, d_col_off);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
-}
-
 // ---------------------------------------------------------------------------------- issuing execution credentials
 // Bounds from the column bytes alone (so that the _dev call needs nothing but the two ends of col_off): each credential's constant
 // text, four digests, a 20-character int64, the 86 proofValue characters and the errorMessage member's frame and suffix, plus at
@@ -1610,12 +1589,13 @@ static uint64_t issue_doc_bound(uint32_t n, uint64_t col_bytes) { return (uint64
 static uint64_t issue_msg_bound(uint32_t n, uint64_t col_bytes) { return (uint64_t)n * issue_fixed_bytes() + 12 * col_bytes; }
 
 static launch::OffsetSpans issue_spans(const uint64_t* col_off) { return {{{col_off, AFC_ISSUE_COLUMNS, -1}}, 1}; }
+// the capacity a batch with these ends (issue_spans) needs
+static bool issue_fits(const uint64_t* ends, uint32_t n, uint64_t cap) { return cap >= issue_doc_bound(n, span(ends[0], ends[1])); }
 
 uint64_t afc_vc_issue_bound(const uint64_t* col_off, uint32_t n) {
     if (!col_off || n == 0) return 0;
-    const launch::OffsetSpans S = issue_spans(col_off);
     uint64_t e[2];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(issue_spans(col_off), n, e);
     return issue_doc_bound(n, span(e[0], e[1]));
 }
 
@@ -1672,20 +1652,16 @@ int afc_vc_issue_execution_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, 
     cudaStream_t st = (cudaStream_t)stream;
     uint64_t ends[2];                       // the column bytes bound the documents
     RC(read_ends(ctx, issue_spans(d_col_off), n, ends, st));
-    const uint64_t cb = span(ends[0], ends[1]);
-    if (ends[1] < ends[0] || docs_cap < issue_doc_bound(n, cb)) return AFC_EINVAL;
+    if (!issue_fits(ends, n, docs_cap)) return AFC_EINVAL;
     uint8_t* hashes = (flags & AFC_ISSUE_HASH_DATA) ? d_hashes : nullptr;
-    {
-        CallLog lc(ctx);
-        uint8_t* scratch = nullptr;
-        IssueScratch S;
-        CK(pool_carve(&scratch, st, [&](Carve& k) { issue_scratch(k, S, n, cb); }));
+    CallLog lc(ctx);
+    IssueScratch S;
+    RC(dev_scratch(ctx, st, [&](Carve& k) { issue_scratch(k, S, n, ends[1] - ends[0]); }, [&] {
         cudaError_t e = issue_sizes(d_cols, d_col_off, d_duration_ms, d_payloads, d_payload_off, d_payload_nil, hashes, n, d_doc_off, S, st, lc);
         if (e == cudaSuccess) e = issue_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_duration_ms, hashes, n, d_docs, d_doc_off,
                                                d_proof_values, S, st, lc);
-        cudaFreeAsync(scratch, st);
-        CK(e);
-    }
+        return e;
+    }));
     return log ? afc_merkle_append_dev(log, d_docs, d_doc_off, n, stream) : AFC_OK;
 }
 
@@ -1699,9 +1675,9 @@ int afc_vc_issue_execution_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32
     if (n == 0) { doc_off[0] = 0; return AFC_OK; }
     const bool hash = (flags & AFC_ISSUE_HASH_DATA) != 0;
     for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
-    if (!monotone(col_off, (uint64_t)n * AFC_ISSUE_COLUMNS) || (hash && !monotone(payload_off, 2 * (uint64_t)n)) ||
-        docs_cap < afc_vc_issue_bound(col_off, n))
-        return AFC_EINVAL;
+    if (!monotone(col_off, (uint64_t)n * AFC_ISSUE_COLUMNS) || (hash && !monotone(payload_off, 2 * (uint64_t)n))) return AFC_EINVAL;
+    uint64_t ends[2];
+    if (!issue_fits(host_ends(issue_spans(col_off), n, ends), n, docs_cap)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of credentials through the ring.  A chunk's documents land at their final offsets, so its stream is synchronised once after
     // the sizes pass to learn where the chunk ends (the next chunk's copies are enqueued after that).
@@ -1766,12 +1742,16 @@ static uint64_t wf_doc_bound(uint32_t n, uint64_t col_bytes, uint64_t records, u
 static launch::OffsetSpans wf_spans(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off) {
     return {{{col_off, AFC_WORKFLOW_COLUMNS, -1}, {rec_off, 1, -1}, {rec_col_off, 2, 1}}, 3};
 }
+// a batch with these ends (wf_spans): record columns and times when it has records, and the capacity its documents need
+static bool wf_fits(const uint64_t* ends, uint32_t n, uint64_t cap, const uint8_t* rec_cols, const int64_t* created_at) {
+    const uint64_t m = ends[3] - ends[2];
+    return (!m || (rec_cols && created_at)) && cap >= wf_doc_bound(n, span(ends[0], ends[1]), m, span(ends[4], ends[5]));
+}
 
 uint64_t afc_vc_workflow_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, uint32_t n) {
     if (!col_off || !rec_off || !rec_col_off || n == 0) return 0;
-    const launch::OffsetSpans S = wf_spans(col_off, rec_off, rec_col_off);
     uint64_t e[6];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(wf_spans(col_off, rec_off, rec_col_off), n, e);
     return wf_doc_bound(n, span(e[0], e[1]), span(e[2], e[3]), span(e[4], e[5]));
 }
 
@@ -1832,20 +1812,15 @@ int afc_vc_issue_workflow_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
     CallLog lc(ctx);
     uint64_t ends[6];                       // the ends of the three offset arrays bound the documents
     RC(read_ends(ctx, wf_spans(d_col_off, d_rec_off, d_rec_col_off), n, ends, st));
-    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] > 0xffffffffull) return AFC_EINVAL;
+    if (ends[3] - ends[2] > 0xffffffffull || !wf_fits(ends, n, docs_cap, d_rec_cols, d_created_at)) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
-    if (m && (!d_rec_cols || !d_created_at)) return AFC_EINVAL;
-    const uint64_t bound = wf_doc_bound(n, span(ends[0], ends[1]), m, span(ends[4], ends[5]));
-    if (docs_cap < bound) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
     WorkflowScratch S;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { wf_scratch(k, S, n, m, bound); }));
-    cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, d_doc_off, d_summary, d_state, S, st, lc);
-    if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m,
-                                        d_docs, d_doc_off, d_proof_values, d_state, d_summary, S, st, lc);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    return dev_scratch(ctx, st, [&](Carve& k) { wf_scratch(k, S, n, m, wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4])); }, [&] {
+        cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, d_doc_off, d_summary, d_state, S, st, lc);
+        if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n,
+                                            m, d_docs, d_doc_off, d_proof_values, d_state, d_summary, S, st, lc);
+        return e;
+    });
 }
 
 int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
@@ -1858,8 +1833,9 @@ int afc_vc_issue_workflow_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
     for (uint32_t i = 0; i < n; i++) if (key_index[i] >= n_keys) return AFC_EINVAL;
     if (!monotone(col_off, (uint64_t)n * AFC_WORKFLOW_COLUMNS) || !monotone(rec_off, n)) return AFC_EINVAL;
     for (uint32_t i = 0; i < n; i++) if (rec_off[i + 1] - rec_off[i] > 0xffffffffull) return AFC_EINVAL;      // a chunk's records are counted in 32 bits
-    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n]) || docs_cap < afc_vc_workflow_bound(col_off, rec_off, rec_col_off, n)) return AFC_EINVAL;
-    if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at)) return AFC_EINVAL;
+    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n])) return AFC_EINVAL;
+    uint64_t ends[6];
+    if (!wf_fits(host_ends(wf_spans(col_off, rec_off, rec_col_off), n, ends), n, docs_cap, rec_cols, created_at)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of whole workflows through the ring, as for execution credentials.  A chunk's records travel with it (the kernels index them
     // by absolute record, so the staged record arrays are addressed from a shifted base); a workflow larger than a chunk's byte budget
@@ -1988,18 +1964,24 @@ static launch::OffsetSpans vcc_spans(const uint64_t* col_off, const uint64_t* re
 uint64_t afc_vc_workflow_chain_bound(const uint64_t* col_off, const uint64_t* rec_off, const uint64_t* rec_col_off, const uint64_t* chain_col_off,
                                      const uint64_t* chain_rec_col_off, uint32_t n) {
     if (!col_off || !rec_off || !rec_col_off || !chain_col_off || !chain_rec_col_off || n == 0) return 0;
-    const launch::OffsetSpans S = vcc_spans(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off);
     uint64_t e[10];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(vcc_spans(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off), n, e);
     return vcc_bound(n, span(e[0], e[1]), span(e[2], e[3]), span(e[4], e[5]), span(e[6], e[7]), span(e[8], e[9]));
 }
+// a batch with these ends (vcc_spans): the record arrays when it has records, and the capacity its bodies need
+static bool vcc_fits(const uint64_t* ends, uint32_t n, uint64_t cap, const uint8_t* rec_cols, const int64_t* created_at, const uint8_t* chain_rec_cols,
+                     const uint8_t* rec_flags, const int64_t* doc_size, const int32_t* created_off) {
+    const uint64_t m = ends[3] - ends[2];
+    return (!m || (rec_cols && created_at && chain_rec_cols && rec_flags && doc_size && created_off)) &&
+           cap >= vcc_bound(n, span(ends[0], ends[1]), m, span(ends[4], ends[5]), span(ends[6], ends[7]), span(ends[8], ends[9]));
+}
 
-// per-call device scratch: the workflow-credential call's outputs and scratch, then the chain's (launch::VccArgs)
+// per-call device scratch: the workflow-credential call's outputs and scratch, then the chain's; binds A to them and to the directory
 struct ChainScratch {
     WorkflowScratch W;
     uint8_t* docs; uint64_t* doc_off; uint8_t* pv; uint8_t* wstate; uint32_t* summary;
 };
-static void vcc_scratch(Carve& k, ChainScratch& s, launch::VccArgs& A, uint32_t n, uint32_t m, uint64_t doc_bound) {
+static void vcc_scratch(Carve& k, ChainScratch& s, launch::VccArgs& A, const afc_did_directory* dir, uint32_t n, uint32_t m, uint64_t doc_bound) {
     const uint64_t O = 3 * (uint64_t)m + n, most = O > n ? O : n;
     s.docs = k.take(doc_bound + 64);
     s.doc_off = k.take<uint64_t>((size_t)n + 1);
@@ -2016,12 +1998,19 @@ static void vcc_scratch(Carve& k, ChainScratch& s, launch::VccArgs& A, uint32_t 
     A.ndist = k.take<uint32_t>(n);
     A.lay = k.take<uint64_t>((size_t)n * launch::vcc_lay_words());
     A.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes((uint32_t)most));
-}
-static void vcc_bind(launch::VccArgs& A, const ChainScratch& s, const afc_did_directory* dir, uint32_t n, uint32_t m) {
     A.dir_dids = dir->d_dids; A.dir_off = dir->d_did_off; A.dir_slots = dir->d_slots; A.dir_mask = dir->slot_mask; A.dir_rank = dir->d_rank;
     A.dir_order = dir->d_order; A.dir_pks = dir->d_pks;
     A.n = n; A.m = m;
     A.docs = s.docs; A.doc_off = s.doc_off; A.pv = s.pv; A.wstate = s.wstate; A.summary = s.summary; A.id_off = s.W.id_off; A.arr = s.W.arr;
+}
+// the workflow credentials, then the chain's sizes: A.body_off is complete when this has run, and vcc_emit writes the bodies
+static cudaError_t vcc_credentials(afc_ctx* ctx, const uint8_t* d_exp, uint32_t n_keys, const uint32_t* key_index, const launch::VccArgs& A,
+                                   const ChainScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
+    cudaError_t e = wf_sizes(A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, A.n, A.m, S.doc_off, S.summary, S.wstate, S.W, st, lg);
+    if (e == cudaSuccess) e = wf_finish(ctx, d_exp, n_keys, key_index, A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, A.n, A.m,
+                                        S.docs, S.doc_off, S.pv, S.wstate, S.summary, S.W, st, lg);
+    if (e == cudaSuccess) e = launch::vcc_sizes(A, st, lg);
+    return e;
 }
 static int vcc_check(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols, const uint64_t* col_off,
                      const uint64_t* rec_off, const uint64_t* rec_col_off, const uint8_t* chain_cols, const uint64_t* chain_col_off, const int64_t* clock,
@@ -2048,30 +2037,19 @@ int afc_vc_workflow_chain_batch_dev(afc_ctx* ctx, const uint8_t* d_expanded96, u
     CallLog lc(ctx);
     uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies
     RC(read_ends(ctx, vcc_spans(d_col_off, d_rec_off, d_rec_col_off, d_chain_col_off, d_chain_rec_col_off), n, ends, st));
-    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[7] < ends[6] || ends[9] < ends[8] || !vcc_slots_fit(ends[3] - ends[2], n))
-        return AFC_EINVAL;
+    if (!vcc_slots_fit(ends[3] - ends[2], n)) return AFC_EINVAL;
+    if (!vcc_fits(ends, n, bodies_cap, d_rec_cols, d_created_at, d_chain_rec_cols, d_rec_flags, d_doc_size, d_created_off)) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
-    if (m && (!d_rec_cols || !d_created_at || !d_chain_rec_cols || !d_rec_flags || !d_doc_size || !d_created_off)) return AFC_EINVAL;
-    const uint64_t cb = span(ends[0], ends[1]), rb = span(ends[4], ends[5]);
-    if (bodies_cap < vcc_bound(n, cb, m, rb, span(ends[6], ends[7]), span(ends[8], ends[9]))) return AFC_EINVAL;
-    const uint64_t dbound = wf_doc_bound(n, cb, m, rb);
     launch::VccArgs A{};
     ChainScratch S;
-    uint8_t* scratch = nullptr;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { vcc_scratch(k, S, A, n, m, dbound); }));
-    vcc_bind(A, S, dir, n, m);
     A.cols = d_cols; A.col_off = d_col_off; A.rec_off = d_rec_off; A.rec_cols = d_rec_cols; A.rec_col_off = d_rec_col_off; A.created_at = d_created_at;
     A.chain_cols = d_chain_cols; A.chain_col_off = d_chain_col_off; A.clock = d_clock; A.chain_rec_cols = d_chain_rec_cols;
     A.chain_rec_col_off = d_chain_rec_col_off; A.rec_flags = d_rec_flags; A.doc_size = d_doc_size; A.created_off = d_created_off;
     A.bodies = d_bodies; A.body_off = d_body_off; A.state = d_state;
-    cudaError_t e = wf_sizes(d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m, S.doc_off, S.summary, S.wstate, S.W, st, lc);
-    if (e == cudaSuccess) e = wf_finish(ctx, d_expanded96, n_keys, d_key_index, d_cols, d_col_off, d_rec_off, d_rec_cols, d_rec_col_off, d_created_at, n, m,
-                                        S.docs, S.doc_off, S.pv, S.wstate, S.summary, S.W, st, lc);
-    if (e == cudaSuccess) e = launch::vcc_sizes(A, st, lc);
-    if (e == cudaSuccess) e = launch::vcc_emit(A, st, lc);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    return dev_scratch(ctx, st, [&](Carve& k) { vcc_scratch(k, S, A, dir, n, m, wf_doc_bound(n, ends[1] - ends[0], m, ends[5] - ends[4])); }, [&] {
+        const cudaError_t e = vcc_credentials(ctx, d_expanded96, n_keys, d_key_index, A, S, st, lc);
+        return e == cudaSuccess ? launch::vcc_emit(A, st, lc) : e;
+    });
 }
 
 int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_t n_keys, const uint32_t* key_index, const uint8_t* cols,
@@ -2089,10 +2067,11 @@ int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
     if (!monotone(col_off, (uint64_t)n * C) || !monotone(chain_col_off, (uint64_t)n * CC) || !monotone(rec_off, n) ||
         !vcc_slots_fit(rec_off[n] - rec_off[0], n))
         return AFC_EINVAL;
-    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n]) || !monotone(chain_rec_col_off, RC_ * rec_off[0], RC_ * rec_off[n]) ||
-        bodies_cap < afc_vc_workflow_chain_bound(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off, n))
+    if (!monotone(rec_col_off, 2 * rec_off[0], 2 * rec_off[n]) || !monotone(chain_rec_col_off, RC_ * rec_off[0], RC_ * rec_off[n])) return AFC_EINVAL;
+    uint64_t ends[10];
+    if (!vcc_fits(host_ends(vcc_spans(col_off, rec_off, rec_col_off, chain_col_off, chain_rec_col_off), n, ends), n, bodies_cap, rec_cols, created_at,
+                  chain_rec_cols, rec_flags, doc_size, created_off))
         return AFC_EINVAL;
-    if (rec_off[n] != rec_off[0] && (!rec_cols || !created_at || !chain_rec_cols || !rec_flags || !doc_size || !created_off)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of whole workflows through the ring, as for workflow credentials: the record arrays are staged for the chunk's records and
     // addressed from a shifted base, so absolute record indices stay valid; a workflow larger than a chunk's byte budget goes alone.
@@ -2135,7 +2114,7 @@ int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
                 A.bodies = k.take(bbound + 64);
                 A.body_off = k.take<uint64_t>((size_t)cnt + 1);
                 A.state = k.take(cnt);
-                vcc_scratch(k, S, A, cnt, m, dbound);
+                vcc_scratch(k, S, A, dir, cnt, m, dbound);
             }));
             A.rec_col_off -= 2 * r0;                // absolute record indices stay valid
             A.created_at -= 2 * r0;
@@ -2143,11 +2122,7 @@ int afc_vc_workflow_chain_batch(afc_ctx* ctx, const uint8_t* expanded96, uint32_
             A.rec_flags -= r0;
             A.doc_size -= r0;
             A.created_off -= r0;
-            vcc_bind(A, S, dir, cnt, m);
-            CK(wf_sizes(A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, cnt, m, S.doc_off, S.summary, S.wstate, S.W, r.st, r.lc));
-            CK(wf_finish(ctx, d_keys, n_keys, d_ki, A.cols, A.col_off, A.rec_off, A.rec_cols, A.rec_col_off, A.created_at, cnt, m, S.docs, S.doc_off,
-                         S.pv, S.wstate, S.summary, S.W, r.st, r.lc));
-            CK(launch::vcc_sizes(A, r.st, r.lc));
+            CK(vcc_credentials(ctx, d_keys, n_keys, d_ki, A, S, r.st, r.lc));
             uint64_t bytes;
             RC(r.read(&bytes, {A.body_off + cnt}));
             CK(launch::vcc_emit(A, r.st, r.lc));
@@ -2232,11 +2207,12 @@ static uint64_t dres_bound(const afc_did_directory* dir, uint32_t n, uint64_t re
 }
 // the _dev call reads these ends with k_dres_ends, which also checks every request's offsets
 static launch::OffsetSpans dres_spans(const uint64_t* req_off) { return {{{req_off, 1, -1}}, 1}; }
+// the capacity a batch with these ends (dres_spans) needs
+static bool dres_fits(const afc_did_directory* dir, const uint64_t* ends, uint32_t n, uint64_t cap) { return cap >= dres_bound(dir, n, span(ends[0], ends[1])); }
 uint64_t afc_did_resolve_bound(const afc_did_directory* dir, const uint64_t* req_off, uint32_t n) {
     if (!dir || !dir->has_ids || !req_off || n == 0) return 0;
-    const launch::OffsetSpans S = dres_spans(req_off);
     uint64_t e[2];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(dres_spans(req_off), n, e);
     return dres_bound(dir, n, span(e[0], e[1]));
 }
 
@@ -2246,6 +2222,12 @@ static int dres_check(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t*
     if (n == 0) return AFC_OK;
     if (!kinds || !reqs || !bodies || !state) return AFC_EINVAL;
     return AFC_OK;
+}
+// per-call device scratch: each request's directory entry, scan tiles
+struct DresScratch { uint32_t* ent; uint64_t* scan; };
+static void dres_scratch(Carve& k, DresScratch& s, uint32_t n) {
+    s.ent = k.take<uint32_t>(n);
+    s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
 }
 
 int afc_did_resolve_batch_dev(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* d_kinds, const uint8_t* d_reqs, const uint64_t* d_req_off,
@@ -2260,20 +2242,14 @@ int afc_did_resolve_batch_dev(afc_ctx* ctx, const afc_did_directory* dir, const 
         const cudaError_t e = cudaMemsetAsync(d_ends, 0, sizeof ends, st);
         return e == cudaSuccess ? launch::dres_ends(d_req_off, n, d_ends, st, lc) : e;
     }));
-    if (ends[2] || bodies_cap < dres_bound(dir, n, span(ends[0], ends[1]))) return AFC_EINVAL;
+    if (ends[2] || !dres_fits(dir, ends, n, bodies_cap)) return AFC_EINVAL;
     const launch::DresDir D = dres_dir(dir);
-    uint32_t* ent = nullptr;
-    uint64_t* scan = nullptr;
-    uint8_t* scratch = nullptr;
-    CK(pool_carve(&scratch, st, [&](Carve& k) {
-        ent = k.take<uint32_t>(n);
-        scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
-    }));
-    cudaError_t e = launch::dres_probe(D, d_kinds, d_reqs, d_req_off, n, d_state, ent, d_body_off, scan, st, lc);
-    if (e == cudaSuccess) e = launch::dres_emit(D, d_kinds, d_reqs, d_req_off, n, d_state, ent, d_body_off, d_bodies, st, lc);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    DresScratch S;
+    return dev_scratch(ctx, st, [&](Carve& k) { dres_scratch(k, S, n); }, [&] {
+        cudaError_t e = launch::dres_probe(D, d_kinds, d_reqs, d_req_off, n, d_state, S.ent, d_body_off, S.scan, st, lc);
+        if (e == cudaSuccess) e = launch::dres_emit(D, d_kinds, d_reqs, d_req_off, n, d_state, S.ent, d_body_off, d_bodies, st, lc);
+        return e;
+    });
 }
 
 int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint8_t* kinds, const uint8_t* reqs, const uint64_t* req_off, uint32_t n,
@@ -2282,7 +2258,8 @@ int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
     if (!monotone(req_off, n)) return AFC_EINVAL;
     for (uint32_t i = 0; i < n; i++) if (req_off[i + 1] - req_off[i] > 0x7fffffffull) return AFC_EINVAL;     // 2^31 bytes
-    if (bodies_cap < afc_did_resolve_bound(dir, req_off, n)) return AFC_EINVAL;
+    uint64_t ends[2];
+    if (!dres_fits(dir, host_ends(dres_spans(req_off), n, ends), n, bodies_cap)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     const launch::DresDir D = dres_dir(dir);
     const uint64_t per = dres_bound(dir, 1, 0);
@@ -2296,21 +2273,20 @@ int afc_did_resolve_batch(afc_ctx* ctx, const afc_did_directory* dir, const uint
         Msgs m;
         const uint8_t* d_kinds;
         uint8_t *d_bodies, *d_state;
-        uint64_t *d_off, *scan;
-        uint32_t* ent;
+        uint64_t* d_off;
+        DresScratch S;
         RC(r.stage([&](Stager& k) {
             m = stage_msgs(k, reqs, req_off, i0, cnt);
             d_kinds = k.in(kinds, i0, cnt);
             d_bodies = k.take(bbound + 64);
             d_off = k.take<uint64_t>((size_t)cnt + 1);
             d_state = k.take(cnt);
-            ent = k.take<uint32_t>(cnt);
-            scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(cnt));
+            dres_scratch(k, S, cnt);
         }));
-        CK(launch::dres_probe(D, d_kinds, m.d, m.off, cnt, d_state, ent, d_off, scan, r.st, r.lc));
+        CK(launch::dres_probe(D, d_kinds, m.d, m.off, cnt, d_state, S.ent, d_off, S.scan, r.st, r.lc));
         uint64_t bytes;
         RC(r.read(&bytes, {d_off + cnt}));
-        CK(launch::dres_emit(D, d_kinds, m.d, m.off, cnt, d_state, ent, d_off, d_bodies, r.st, r.lc));
+        CK(launch::dres_emit(D, d_kinds, m.d, m.off, cnt, d_state, S.ent, d_off, d_bodies, r.st, r.lc));
         RC(r.copy_back({offsets_out(body_off, i0, d_off, (size_t)cnt + 1, base), {state, i0, d_state, cnt}, {bodies, base, d_bodies, bytes}}));
         base += bytes;
         return AFC_OK;
@@ -2325,12 +2301,15 @@ static uint64_t wh_bound(uint32_t n, uint64_t bytes) { return (uint64_t)n * laun
 static launch::OffsetSpans wh_spans(const uint64_t* col_off, const uint64_t* result_off) {
     return {{{col_off, AFC_WEBHOOK_COLUMNS, -1}, {result_off, 1, -1}}, 2};
 }
+// a batch with these ends (wh_spans): results when it has result bytes, and the capacity its bodies need
+static bool wh_fits(const uint64_t* ends, uint32_t n, uint64_t cap, const uint8_t* results) {
+    return (results || ends[3] == ends[2]) && cap >= wh_bound(n, span(ends[0], ends[1]) + span(ends[2], ends[3]));
+}
 
 uint64_t afc_webhook_bound(const uint64_t* col_off, const uint64_t* result_off, uint32_t n) {
     if (!col_off || !result_off || n == 0) return 0;
-    const launch::OffsetSpans S = wh_spans(col_off, result_off);
     uint64_t e[4];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(wh_spans(col_off, result_off), n, e);
     return wh_bound(n, span(e[0], e[1]) + span(e[2], e[3]));
 }
 
@@ -2342,14 +2321,19 @@ static void wh_scratch(Carve& k, WebhookScratch& s, uint32_t n, uint64_t result_
     s.mac = k.take((size_t)n * 32);
     s.scan = (uint64_t*)k.take(launch::json_scan_scratch_bytes(n));
 }
-static cudaError_t wh_enqueue(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
-                              const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, uint64_t* body_off,
-                              uint8_t* headers, uint8_t* status, const WebhookScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
-    cudaError_t e = launch::wh_sizes(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off + 1, status, st, lg);
-    if (e == cudaSuccess) e = launch::offsets_from_lengths(body_off, n, S.scan, st, lg);
-    if (e == cudaSuccess) e = launch::wh_emit(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off, bodies, st, lg);
-    if (e == cudaSuccess) e = launch::wh_sign(sec, sec_off, flags, status, bodies, body_off, n, S.mac, headers, st, lg);
-    return e;
+// the plans, lengths and the scan: body_off is complete when this has run
+static cudaError_t wh_layout(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
+                             const uint64_t* res_off, uint32_t n, uint64_t* body_off, uint8_t* status, const WebhookScratch& S, cudaStream_t st,
+                             launch::LaunchLog* lg) {
+    const cudaError_t e = launch::wh_sizes(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off + 1, status, st, lg);
+    return e == cudaSuccess ? launch::offsets_from_lengths(body_off, n, S.scan, st, lg) : e;
+}
+// the bodies and their signatures
+static cudaError_t wh_finish(const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
+                             const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, uint8_t* bodies, const uint64_t* body_off,
+                             uint8_t* headers, const uint8_t* status, const WebhookScratch& S, cudaStream_t st, launch::LaunchLog* lg) {
+    const cudaError_t e = launch::wh_emit(cols, col_off, dur, flags, res, res_off, n, S.tape, S.plan, body_off, bodies, st, lg);
+    return e == cudaSuccess ? launch::wh_sign(sec, sec_off, flags, status, bodies, body_off, n, S.mac, headers, st, lg) : e;
 }
 static int wh_check(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* dur, const uint8_t* flags, const uint8_t* res,
                     const uint64_t* res_off, const uint8_t* sec, const uint32_t* sec_off, uint32_t n, const uint8_t* bodies, const uint64_t* body_off,
@@ -2370,18 +2354,15 @@ int afc_webhook_sign_batch_dev(afc_ctx* ctx, const uint8_t* d_cols, const uint64
     cudaStream_t st = (cudaStream_t)stream;
     uint64_t ends[4];                       // the column and result bytes bound the bodies and size the tapes
     RC(read_ends(ctx, wh_spans(d_col_off, d_result_off), n, ends, st));
-    const uint64_t rb = span(ends[2], ends[3]);
-    if (ends[1] < ends[0] || ends[3] < ends[2] || bodies_cap < wh_bound(n, span(ends[0], ends[1]) + rb)) return AFC_EINVAL;
-    if ((!d_results && ends[3] != ends[2]) || !d_secrets) return AFC_EINVAL;
+    if (!wh_fits(ends, n, bodies_cap, d_results) || !d_secrets) return AFC_EINVAL;
     CallLog lc(ctx);
-    uint8_t* scratch = nullptr;
     WebhookScratch S;
-    CK(pool_carve(&scratch, st, [&](Carve& k) { wh_scratch(k, S, n, rb); }));
-    cudaError_t e = wh_enqueue(d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies, d_body_off,
-                               d_headers, d_status, S, st, lc);
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    return AFC_OK;
+    return dev_scratch(ctx, st, [&](Carve& k) { wh_scratch(k, S, n, ends[3] - ends[2]); }, [&] {
+        cudaError_t e = wh_layout(d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, n, d_body_off, d_status, S, st, lc);
+        if (e == cudaSuccess) e = wh_finish(d_cols, d_col_off, d_duration_ms, d_flags, d_results, d_result_off, d_secrets, d_secret_off, n, d_bodies,
+                                            d_body_off, d_headers, d_status, S, st, lc);
+        return e;
+    });
 }
 
 int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* col_off, const int64_t* duration_ms, const uint8_t* flags,
@@ -2392,10 +2373,9 @@ int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* co
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
     uint32_t bad = 0;
     for (uint32_t i = 0; i < n; i++) bad |= flags[i] & ~(uint32_t)(AFC_WEBHOOK_HAS_DURATION | AFC_WEBHOOK_HAS_ERROR_MESSAGE | AFC_WEBHOOK_HAS_SECRET);
-    if (bad || !monotone(col_off, (uint64_t)n * AFC_WEBHOOK_COLUMNS) || !monotone(result_off, n) || !monotone(secret_off, n) ||
-        bodies_cap < afc_webhook_bound(col_off, result_off, n))
-        return AFC_EINVAL;
-    if ((!results && result_off[n] != result_off[0]) || (!secrets && secret_off[n] != secret_off[0])) return AFC_EINVAL;
+    if (bad || !monotone(col_off, (uint64_t)n * AFC_WEBHOOK_COLUMNS) || !monotone(result_off, n) || !monotone(secret_off, n)) return AFC_EINVAL;
+    uint64_t ends[4];
+    if (!wh_fits(host_ends(wh_spans(col_off, result_off), n, ends), n, bodies_cap, results) || (!secrets && secret_off[n] != secret_off[0])) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     // Chunks of deliveries through the ring, as for execution credentials: a chunk's stream is synchronised once after the sizes pass to
     // learn where its bodies end.  The staged secrets are marked secret.
@@ -2431,12 +2411,10 @@ int afc_webhook_sign_batch(afc_ctx* ctx, const uint8_t* cols, const uint64_t* co
             d_st = k.take(cnt);
             wh_scratch(k, S, cnt, rbytes);
         }));
-        CK(launch::wh_sizes(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff + 1, d_st, r.st, r.lc));
-        CK(launch::offsets_from_lengths(d_boff, cnt, S.scan, r.st, r.lc));
+        CK(wh_layout(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, d_boff, d_st, S, r.st, r.lc));
         uint64_t bytes;
         RC(r.read(&bytes, {d_boff + cnt}));
-        CK(launch::wh_emit(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, cnt, S.tape, S.plan, d_boff, d_bodies, r.st, r.lc));
-        CK(launch::wh_sign(d_sec, d_soff, d_fl, d_st, d_bodies, d_boff, cnt, S.mac, d_h, r.st, r.lc));
+        CK(wh_finish(d_cols, d_coff, d_dur, d_fl, d_res, d_roff, d_sec, d_soff, cnt, d_bodies, d_boff, d_h, d_st, S, r.st, r.lc));
         RC(r.copy_back({offsets_out(body_off, i0, d_boff, (size_t)cnt + 1, base), {headers, (size_t)i0 * 71, d_h, (size_t)cnt * 71},
                         {status, i0, d_st, cnt}, {bodies, base, d_bodies, bytes}}));
         base += bytes;
@@ -2459,10 +2437,33 @@ static launch::OffsetSpans didr_spans(const uint64_t* node_off, const uint64_t* 
 
 uint64_t afc_did_register_bound(const uint64_t* node_off, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n, uint64_t server_id_len) {
     if (!node_off || !id_idx || !id_off || n == 0) return 0;
-    const launch::OffsetSpans S = didr_spans(node_off, id_idx, id_off);
     uint64_t e[6];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(didr_spans(node_off, id_idx, id_off), n, e);
     return didr_bound(n, span(e[0], e[1]), server_id_len, span(e[2], e[3]), span(e[4], e[5]));
+}
+
+// The arguments both forms check first: n == 0 needs only the offset arrays
+static int didr_check(afc_ctx* ctx, const uint8_t* master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* node_ids,
+                      const uint64_t* node_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint64_t* id_off, uint32_t n,
+                      const uint64_t* comp_off, const uint8_t* expanded96, const uint8_t* pks, const uint8_t* dids, const uint8_t* paths,
+                      const uint8_t* comp_flags, const uint8_t* body, const uint64_t* body_off) {
+    if (!ctx || !node_off || !id_idx || !id_off || !comp_off || !body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!master_seed || !node_ids || !agent_index || !expanded96 || !pks || !dids || !paths || !comp_flags || !body || (server_id_len && !server_id))
+        return AFC_EINVAL;
+    return AFC_OK;
+}
+// A batch's components (a key slot per request and per id) are counted in 32 bits
+static bool didr_slots_fit(uint64_t m, uint32_t n) { return m + n <= 0xffffffffull; }
+// a batch with these ends (didr_spans): id bytes when it has any, and the capacity its bodies need
+static bool didr_fits(const uint64_t* ends, uint32_t n, uint64_t server_len, uint64_t cap, const uint8_t* ids) {
+    return (ends[5] <= ends[4] || ids) && cap >= didr_bound(n, span(ends[0], ends[1]), server_len, ends[3] - ends[2], span(ends[4], ends[5]));
+}
+// the fields of a register or re-register call's arguments that come from the context and the call's sizes (DidrrArgs also takes G)
+extern "C++" template <class Args> void did_args(Args& A, afc_ctx* ctx, const uint8_t* server_id, uint64_t server_len, uint32_t n, uint32_t m) {
+    A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
+    A.h = did_hash(server_id, server_len) & 0x7fffffffu; A.server_len = server_len;
+    A.n = n; A.m = m;
 }
 
 // per-call device scratch (launch::DidrArgs); the derived seeds are secret
@@ -2483,41 +2484,31 @@ int afc_did_register_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, const
                                const uint64_t* d_node_off, const uint32_t* d_agent_index, const uint64_t* d_id_idx, const uint8_t* d_ids,
                                const uint64_t* d_id_off, uint32_t n, uint64_t* d_comp_off, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids,
                                uint8_t* d_paths, uint8_t* d_comp_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream) {
-    if (!ctx || !d_node_off || !d_id_idx || !d_id_off || !d_comp_off || !d_body_off) return AFC_EINVAL;
+    RC(didr_check(ctx, d_master_seed, server_id, server_id_len, d_node_ids, d_node_off, d_agent_index, d_id_idx, d_id_off, n, d_comp_off, d_expanded96,
+                  d_pks, d_dids, d_paths, d_comp_flags, d_body, d_body_off));
     if (n == 0) return AFC_OK;
-    if (!d_master_seed || !d_node_ids || !d_agent_index || !d_expanded96 || !d_pks || !d_dids || !d_paths || !d_comp_flags || !d_body ||
-        (server_id_len && !server_id))
-        return AFC_EINVAL;
     if (!aligned16(d_master_seed) || !aligned16(d_expanded96) || !aligned16(d_pks) || !aligned16(d_paths)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
     uint64_t ends[6];                       // the ends of the three offset arrays bound the bodies
     RC(read_ends(ctx, didr_spans(d_node_off, d_id_idx, d_id_off), n, ends, st));
-    if (ends[1] < ends[0] || ends[3] < ends[2] || ends[5] < ends[4] || ends[3] - ends[2] + n > 0xffffffffull) return AFC_EINVAL;
+    if (!didr_slots_fit(ends[3] - ends[2], n) || !didr_fits(ends, n, server_id_len, body_cap, d_ids)) return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]);
-    if (ends[5] > ends[4] && !d_ids) return AFC_EINVAL;
-    if (body_cap < didr_bound(n, span(ends[0], ends[1]), server_id_len, m, span(ends[4], ends[5]))) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
     launch::DidrArgs A{};
-    uint8_t* d_server;
-    CK(pool_carve(&scratch, st, [&](Carve& k) {
-        didr_scratch(k, A, n, m);
-        d_server = k.take(server_id_len + 16);
-    }));
-    A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
-    A.master = d_master_seed; A.h = did_hash(server_id, server_id_len) & 0x7fffffffu; A.server = d_server; A.server_len = server_id_len;
+    did_args(A, ctx, server_id, server_id_len, n, m);
+    A.master = d_master_seed;
     A.nodes = d_node_ids; A.node_off = d_node_off; A.agent_index = d_agent_index; A.id_idx = d_id_idx; A.ids = d_ids; A.id_off = d_id_off;
-    A.n = n; A.m = m;
     A.comp_off = d_comp_off; A.expanded96 = d_expanded96; A.pks = d_pks; A.dids = d_dids; A.paths = d_paths; A.comp_flags = d_comp_flags;
     A.body = d_body; A.body_off = d_body_off;
-    cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
-    if (e == cudaSuccess) e = launch::didr_register(A, st, lc);
-    const cudaError_t wipe = cudaMemsetAsync(A.seeds, 0, ((size_t)n + m) * 32, st);       // derived seeds do not outlive the call
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    CK(wipe);
-    return AFC_OK;
+    uint8_t* d_server;
+    return dev_scratch(ctx, st, [&](Carve& k) {
+        didr_scratch(k, A, n, m);
+        A.server = d_server = k.take(server_id_len + 16);
+    }, [&] {
+        const cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
+        return e == cudaSuccess ? launch::didr_register(A, st, lc) : e;
+    });
 }
 
 // Device bytes one chunk stages (its arena, to within alignment): inputs, per component its outputs (96 + 32 + 55 + 48 + 1) and seed, per id
@@ -2534,17 +2525,15 @@ int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8
                            const uint64_t* node_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint8_t* ids, const uint64_t* id_off,
                            uint32_t n, uint64_t* comp_off, uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* comp_flags,
                            uint8_t* body, uint64_t body_cap, uint64_t* body_off) {
-    if (!ctx || !node_off || !id_idx || !id_off || !comp_off || !body_off) return AFC_EINVAL;
+    RC(didr_check(ctx, master_seed, server_id, server_id_len, node_ids, node_off, agent_index, id_idx, id_off, n, comp_off, expanded96, pks, dids, paths,
+                  comp_flags, body, body_off));
     if (n == 0) { comp_off[0] = 0; body_off[0] = 0; return AFC_OK; }
-    if (!master_seed || !node_ids || !agent_index || !expanded96 || !pks || !dids || !paths || !comp_flags || !body || (server_id_len && !server_id))
-        return AFC_EINVAL;
     if (!monotone(node_off, n) || !monotone(id_idx, 2 * n)) return AFC_EINVAL;
     const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n];
-    if (r_last - r_first + n > 0xffffffffull) return AFC_EINVAL;
-    if (!monotone(id_off, r_first, r_last) || (id_off[r_last] > id_off[r_first] && !ids)) return AFC_EINVAL;
-    if (body_cap < afc_did_register_bound(node_off, id_idx, id_off, n, server_id_len)) return AFC_EINVAL;
+    if (!didr_slots_fit(r_last - r_first, n) || !monotone(id_off, r_first, r_last)) return AFC_EINVAL;
+    uint64_t ends[6];
+    if (!didr_fits(host_ends(didr_spans(node_off, id_idx, id_off), n, ends), n, server_id_len, body_cap, ids)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
     auto measure = [&](uint32_t i0, uint32_t i) {
         const uint64_t r0 = id_idx[2 * (size_t)i0], r = id_idx[2 * (size_t)i + 2];
         return didr_chunk_bytes(i + 1 - i0, node_off[i + 1] - node_off[i0], server_id_len, r - r0, id_off[r] - id_off[r0]);
@@ -2579,9 +2568,7 @@ int afc_did_register_batch(afc_ctx* ctx, const uint8_t* master_seed, const uint8
                 didr_scratch(k, A, cnt, mc);
             }));
             A.id_off -= r0;                         // absolute id indices stay valid
-            A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
-            A.h = h; A.server_len = server_id_len;
-            A.n = cnt; A.m = mc;
+            did_args(A, ctx, server_id, server_id_len, cnt, mc);
             CK(launch::didr_register(A, r.st, r.lc));
             uint64_t end[2];                        // components, body bytes
             RC(r.read(end, {A.comp_off + cnt, A.body_off + cnt}));
@@ -2621,10 +2608,31 @@ static launch::OffsetSpans didrr_spans(const uint64_t* agent_col_off, const uint
 uint64_t afc_did_reregister_bound(const uint64_t* agent_col_off, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
                                   const uint64_t* reg_col_off, uint32_t n, uint64_t server_id_len) {
     if (!agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || n == 0) return 0;
-    const launch::OffsetSpans S = didrr_spans(agent_col_off, id_idx, id_off, reg_idx, reg_col_off);
     uint64_t e[10];
-    offset_ends(S.s, S.k, n, e);
+    host_ends(didrr_spans(agent_col_off, id_idx, id_off, reg_idx, reg_col_off), n, e);
     return didrr_bound(n, span(e[0], e[1]), server_id_len, span(e[2], e[3]), span(e[4], e[5]), span(e[6], e[7]), span(e[8], e[9]));
+}
+
+// The arguments both forms check first: n == 0 needs only the offset arrays
+static int didrr_check(afc_ctx* ctx, const uint8_t* master_seed, const uint8_t* server_id, uint64_t server_id_len, const uint8_t* agent_cols,
+                       const uint64_t* agent_col_off, const uint32_t* agent_index, const uint64_t* id_idx, const uint64_t* id_off, const uint64_t* reg_idx,
+                       const uint64_t* reg_col_off, uint32_t n, const uint8_t* state, const uint32_t* counts, const uint8_t* expanded96,
+                       const uint8_t* pks, const uint8_t* dids, const uint8_t* paths, const uint8_t* body, const uint64_t* body_off) {
+    if (!ctx || !agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || !body_off) return AFC_EINVAL;
+    if (n == 0) return AFC_OK;
+    if (!master_seed || !agent_cols || !agent_index || !state || !counts || !expanded96 || !pks || !dids || !paths || !body ||
+        (server_id_len && !server_id))
+        return AFC_EINVAL;
+    return AFC_OK;
+}
+// A batch's ids, components and two key slots per request are counted in 32 bits
+static bool didrr_slots_fit(uint64_t m, uint64_t G, uint32_t n) { return m + G + 2 * (uint64_t)n <= 0xffffffffull; }
+// a batch with these ends (didrr_spans): id and component bytes and flags when it has any, and the capacity its bodies need
+static bool didrr_fits(const uint64_t* ends, uint32_t n, uint64_t server_len, uint64_t cap, const uint8_t* ids, const uint8_t* reg_cols,
+                       const uint8_t* id_flags, const uint8_t* reg_flags) {
+    const uint64_t m = ends[3] - ends[2], G = ends[7] - ends[6];
+    return (ends[5] <= ends[4] || ids) && (ends[9] <= ends[8] || reg_cols) && (!m || id_flags) && (!G || reg_flags) &&
+           cap >= didrr_bound(n, span(ends[0], ends[1]), server_len, m, span(ends[4], ends[5]), G, span(ends[8], ends[9]));
 }
 
 // per-call device scratch (launch::DidrrArgs); the derived seeds are secret
@@ -2648,44 +2656,34 @@ int afc_did_reregister_batch_dev(afc_ctx* ctx, const uint8_t* d_master_seed, con
                                  const uint64_t* d_id_off, const uint64_t* d_reg_idx, const uint8_t* d_reg_cols, const uint64_t* d_reg_col_off, uint32_t n,
                                  uint8_t* d_state, uint32_t* d_counts, uint8_t* d_expanded96, uint8_t* d_pks, uint8_t* d_dids, uint8_t* d_paths,
                                  uint8_t* d_reg_flags, uint8_t* d_id_flags, uint8_t* d_body, uint64_t body_cap, uint64_t* d_body_off, void* stream) {
-    if (!ctx || !d_agent_col_off || !d_id_idx || !d_id_off || !d_reg_idx || !d_reg_col_off || !d_body_off) return AFC_EINVAL;
+    RC(didrr_check(ctx, d_master_seed, server_id, server_id_len, d_agent_cols, d_agent_col_off, d_agent_index, d_id_idx, d_id_off, d_reg_idx,
+                   d_reg_col_off, n, d_state, d_counts, d_expanded96, d_pks, d_dids, d_paths, d_body, d_body_off));
     if (n == 0) return AFC_OK;
-    if (!d_master_seed || !d_agent_cols || !d_agent_index || !d_state || !d_counts || !d_expanded96 || !d_pks || !d_dids || !d_paths || !d_body ||
-        (server_id_len && !server_id))
-        return AFC_EINVAL;
     if (!aligned16(d_master_seed) || !aligned16(d_expanded96) || !aligned16(d_pks) || !aligned16(d_paths)) return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     CallLog lc(ctx);
     uint64_t ends[10];                      // the ends of the five offset arrays bound the bodies
     RC(read_ends(ctx, didrr_spans(d_agent_col_off, d_id_idx, d_id_off, d_reg_idx, d_reg_col_off), n, ends, st));
-    for (int k = 0; k < 10; k += 2)
-        if (ends[k + 1] < ends[k]) return AFC_EINVAL;
-    if ((ends[3] - ends[2]) + (ends[7] - ends[6]) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
+    if (!didrr_slots_fit(ends[3] - ends[2], ends[7] - ends[6], n) || !didrr_fits(ends, n, server_id_len, body_cap, d_ids, d_reg_cols, d_id_flags, d_reg_flags))
+        return AFC_EINVAL;
     const uint32_t m = (uint32_t)(ends[3] - ends[2]), G = (uint32_t)(ends[7] - ends[6]);
-    if ((ends[5] > ends[4] && !d_ids) || (ends[9] > ends[8] && !d_reg_cols) || (m && !d_id_flags) || (G && !d_reg_flags)) return AFC_EINVAL;
-    if (body_cap < didrr_bound(n, span(ends[0], ends[1]), server_id_len, m, span(ends[4], ends[5]), G, span(ends[8], ends[9]))) return AFC_EINVAL;
-    uint8_t* scratch = nullptr;
     launch::DidrrArgs A{};
-    uint8_t* d_server;
-    CK(pool_carve(&scratch, st, [&](Carve& k) {
-        didrr_scratch(k, A, n, m, G);
-        d_server = k.take(server_id_len + 16);
-    }));
-    A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
-    A.master = d_master_seed; A.h = did_hash(server_id, server_id_len) & 0x7fffffffu; A.server = d_server; A.server_len = server_id_len;
+    did_args(A, ctx, server_id, server_id_len, n, m);
+    A.G = G;
+    A.master = d_master_seed;
     A.agent_cols = d_agent_cols; A.agent_col_off = d_agent_col_off; A.agent_index = d_agent_index;
     A.id_idx = d_id_idx; A.ids = d_ids; A.id_off = d_id_off; A.reg_idx = d_reg_idx; A.reg_cols = d_reg_cols; A.reg_col_off = d_reg_col_off;
-    A.n = n; A.m = m; A.G = G;
     A.state = d_state; A.counts = d_counts; A.expanded96 = d_expanded96; A.pks = d_pks; A.dids = d_dids; A.paths = d_paths;
     A.reg_flags = d_reg_flags; A.id_flags = d_id_flags; A.body = d_body; A.body_off = d_body_off;
-    cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
-    if (e == cudaSuccess) e = launch::didrr_reregister(A, st, lc);
-    const cudaError_t wipe = cudaMemsetAsync(A.seeds, 0, (size_t)n * 64, st);             // derived seeds do not outlive the call
-    cudaFreeAsync(scratch, st);
-    CK(e);
-    CK(wipe);
-    return AFC_OK;
+    uint8_t* d_server;
+    return dev_scratch(ctx, st, [&](Carve& k) {
+        didrr_scratch(k, A, n, m, G);
+        A.server = d_server = k.take(server_id_len + 16);
+    }, [&] {
+        const cudaError_t e = server_id_len ? cudaMemcpyAsync(d_server, server_id, server_id_len, cudaMemcpyHostToDevice, st) : cudaSuccess;
+        return e == cudaSuccess ? launch::didrr_reregister(A, st, lc) : e;
+    });
 }
 
 // Device bytes one chunk stages (its arena, to within alignment): inputs and their offsets, per request its outputs and two key slots
@@ -2704,21 +2702,18 @@ int afc_did_reregister_batch(afc_ctx* ctx, const uint8_t* master_seed, const uin
                              const uint64_t* reg_idx, const uint8_t* reg_cols, const uint64_t* reg_col_off, uint32_t n, uint8_t* state, uint32_t* counts,
                              uint8_t* expanded96, uint8_t* pks, uint8_t* dids, uint8_t* paths, uint8_t* reg_flags, uint8_t* id_flags, uint8_t* body,
                              uint64_t body_cap, uint64_t* body_off) {
-    if (!ctx || !agent_col_off || !id_idx || !id_off || !reg_idx || !reg_col_off || !body_off) return AFC_EINVAL;
+    RC(didrr_check(ctx, master_seed, server_id, server_id_len, agent_cols, agent_col_off, agent_index, id_idx, id_off, reg_idx, reg_col_off, n, state,
+                   counts, expanded96, pks, dids, paths, body, body_off));
     if (n == 0) { body_off[0] = 0; return AFC_OK; }
-    if (!master_seed || !agent_cols || !agent_index || !state || !counts || !expanded96 || !pks || !dids || !paths || !body ||
-        (server_id_len && !server_id))
-        return AFC_EINVAL;
     if (!monotone(agent_col_off, 3 * n) || !monotone(id_idx, 2 * n) || !monotone(reg_idx, 2 * n)) return AFC_EINVAL;
     const uint64_t r_first = id_idx[0], r_last = id_idx[2 * (size_t)n], g_first = reg_idx[0], g_last = reg_idx[2 * (size_t)n];
-    if ((r_last - r_first) + (g_last - g_first) + 2 * (uint64_t)n > 0xffffffffull) return AFC_EINVAL;
-    if (!monotone(id_off, r_first, r_last) || !monotone(reg_col_off, 5 * g_first, 5 * g_last) || (id_off[r_last] > id_off[r_first] && !ids) ||
-        (reg_col_off[5 * g_last] > reg_col_off[5 * g_first] && !reg_cols) ||
-        (r_last > r_first && !id_flags) || (g_last > g_first && !reg_flags))
+    if (!didrr_slots_fit(r_last - r_first, g_last - g_first, n) || !monotone(id_off, r_first, r_last) || !monotone(reg_col_off, 5 * g_first, 5 * g_last))
         return AFC_EINVAL;
-    if (body_cap < afc_did_reregister_bound(agent_col_off, id_idx, id_off, reg_idx, reg_col_off, n, server_id_len)) return AFC_EINVAL;
+    uint64_t ends[10];
+    if (!didrr_fits(host_ends(didrr_spans(agent_col_off, id_idx, id_off, reg_idx, reg_col_off), n, ends), n, server_id_len, body_cap, ids, reg_cols,
+                    id_flags, reg_flags))
+        return AFC_EINVAL;
     CK(cudaSetDevice(ctx->device));
-    const uint32_t h = did_hash(server_id, server_id_len) & 0x7fffffffu;
     auto measure = [&](uint32_t i0, uint32_t i) {
         const uint64_t r0 = id_idx[2 * (size_t)i0], r = id_idx[2 * (size_t)i + 2], g0 = reg_idx[2 * (size_t)i0], g = reg_idx[2 * (size_t)i + 2];
         return didrr_chunk_bytes(i + 1 - i0, agent_col_off[3 * (size_t)i + 3] - agent_col_off[3 * (size_t)i0], server_id_len, r - r0, id_off[r] - id_off[r0],
@@ -2760,9 +2755,8 @@ int afc_did_reregister_batch(afc_ctx* ctx, const uint8_t* master_seed, const uin
         }));
         A.id_off -= r0;                             // absolute indices stay valid
         A.reg_col_off -= 5 * g0;
-        A.comb = ctx->comb; A.ct16 = afc_internal_sign_table(ctx);
-        A.h = h; A.server_len = server_id_len;
-        A.n = cnt; A.m = mc; A.G = gc;
+        did_args(A, ctx, server_id, server_id_len, cnt, mc);
+        A.G = gc;
         CK(launch::didrr_reregister(A, r.st, r.lc));
         uint64_t bytes;
         RC(r.read(&bytes, {A.body_off + cnt}));
